@@ -1,17 +1,22 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the block-sparse matmul hot path on B200.
+"""bench.py -- headline benchmark of the block-sparse matmul hot path on H100.
 
 A "step" = one fprop + one bprop + one updat of BlocksparseMatMul over one synthetic
 minibatch (BASELINE.json configs[1]: 4096x4096, block_size 32, bf16, N=4096 per GPU,
 density 25 % unless --density is given).  Metric = effective TFLOP/s
 = 3 * 2*nnz_blocks*bs^2*N / t  (the reference's own flop accounting, op.cc:102,182).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
+
+--dump-outputs DIR writes what the last timed step returned (rank 0) as float32 .npy files: y.npy and dx.npy
+(a fixed sample of DUMP_ROWS minibatch rows, all features) and dw.npy (a fixed sample of at most DUMP_BLOCKS weight
+blocks), with the sampled indices in y_rows.npy / dw_blocks.npy.  Inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 
 N>1 is launched by torchrun (one rank per GPU): the minibatch axis is sharded (weak
 scaling: every rank holds N=4096 columns), fprop/bprop need no communication and the
 updat output dW (fp32 when N>1) is all-reduced with NCCL on a side stream, overlapping the
-next step's fprop/bprop, with BSMM_SM_MARGIN SMs left free for the NCCL kernel (SURVEY.md 8e).
+next step's fprop/bprop, with BSMM_SM_MARGIN SMs left free for the NCCL kernel.
 
 Besides the headline the JSON line carries (rank 0, skipped with --no-extras):
   check           max_rel_err / l2_err of Y, DX, DW taken from the TIMED buffers against the oracle (row/block sample)
@@ -37,6 +42,7 @@ C = K = 4096
 BS = 32
 N_PER_GPU = 4096
 SEED = 1236
+DUMP_ROWS, DUMP_BLOCKS = 512, 4096          # <= 8 + 8 + 16 MB of float32 at the default shape
 
 
 def make_layout(density, cb=C // BS, kb=K // BS, seed=SEED):
@@ -82,7 +88,8 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, source="fallback")
+    # NVIDIA data sheet, H100 SXM at 700 W: 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s (a ceiling, not a reached rate)
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
@@ -162,8 +169,7 @@ def cpu_reference(density, axis, budget_s=20.0, steps=1):
         bprop_fast(orc, e, W)
         updat_fast(orc, x, e)
 
-    # NumPy's batched small matmuls do not scale monotonically with BLAS threads (64 threads were 3x slower than 1 on
-    # the B200 host): probe a few thread counts on a quarter-size sample and keep the fastest, up to all host cores.
+    # NumPy's batched small matmuls do not scale monotonically with BLAS threads: probe a few thread counts on a quarter-size sample and keep the fastest, up to all host cores.
     ncpu = os.cpu_count() or 1
     threads, limiter = ncpu, None
     try:
@@ -286,6 +292,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--sm-margin", type=int, default=None, help="SMs left free for NCCL when N>1 (default 8 at 2 GPUs, 12 beyond; BSMM_SM_MARGIN wins)")
     ap.add_argument("--blocking-allreduce", action="store_true", help="round-1 behaviour: all-reduce on the compute stream")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (seeded samples, float32 .npy) to DIR")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -313,9 +321,8 @@ def main():
     from blocksparse_b200 import dist as bdist
     margin = 0
     if world > 1 and not args.blocking_allreduce:
-        # measured (profiles/r2_scaling.txt): 8 NCCL CTAs hide the 17 MB fp32 all-reduce at 2 GPUs, 8 GPUs need 12.  The margin is
-        # 4 SMs LARGER than the CTAs NCCL may use: the persistent grids are dealt tiles statically, so a single CTA that finds
-        # its SM taken runs as a second wave and doubles the kernel time (the bimodal 0.23 / 0.40 ms steps seen with zero slack)
+        # NCCL may use 8 CTAs for the fp32 all-reduce of dW at 2 GPUs and 12 beyond; the margin leaves 4 SMs more than that
+        # free so that the reduction can run beside the matmul kernels
         ctas = (8 if world <= 2 else 12)
         margin = bdist.reserve_sms_for_nccl(ctas + 4 if args.sm_margin is None else args.sm_margin,
                                             nccl_ctas=ctas if args.sm_margin is None else max(1, args.sm_margin - 4))
@@ -397,9 +404,8 @@ def main():
     if side is not None:
         side.wait()
     if side is not None:
-        # Untimed settling + calibration.  Whether the NCCL kernel really runs BESIDE the persistent grids depends on where the
-        # block scheduler places it, and the first process on a fresh box has shown a transient 3.5 ms/step state
-        # (profiles/r2_scaling.txt).  Run 100 more untimed steps, then time both schemes for 20 steps each, agree across ranks
+        # Untimed settling + calibration.  Whether the NCCL kernel really runs BESIDE the matmul grids depends on where the
+        # block scheduler places it.  Run 100 more untimed steps, then time both schemes for 20 steps each, agree across ranks
         # (max over ranks) and keep the faster one for the timed region.
         for i in range(100):
             step(i)
@@ -449,6 +455,8 @@ def main():
             dw_l = bsmm.updat([Xs[li]], [Es[li]], dw_dtype=dw_dtype)
         check = check_against_oracle(torch, bsmm, lay, args.axis, W, Xs[li], Es[li], y_l, dx_l, dw_l)
         check["device_error"] = _lib.device_error()
+        if args.dump_outputs:
+            dump_outputs(torch, args.dump_outputs, args.axis, *last)
 
     # ---- per-kernel timing (each kernel alone) for the roofline object: cold (rotating inputs > L2) and warm L2
     pk = peaks()
@@ -469,15 +477,7 @@ def main():
         roof = {"bound": "tensor", "achieved": tf, "peak": pk["tf_burst"], "unit": "TFLOP/s", "frac": tf / pk["tf_burst"]}
     else:
         roof = {"bound": "hbm", "achieved": gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": gbs / pk["hbm"]}
-    traffic, traffic_src = None, None
-    for tname in ("r2_traffic.json", "r1_traffic.json"):       # dram bytes per launch from the committed ncu --set full capture
-        tpath = os.path.join(ROOT, "profiles", tname)
-        if os.path.exists(tpath) and abs(args.density - 0.25) < 1e-9:
-            traffic = json.load(open(tpath)).get(kernels[dom])
-            if traffic is not None:
-                traffic_src = "profiles/" + tname
-                break
-    roof.update({"kernel": "%s (%s)" % (dom, kernels[dom]), "traffic": traffic, "traffic_source": traffic_src,
+    roof.update({"kernel": "%s (%s)" % (dom, kernels[dom]),
                  "peak_source": pk["source"], "per_op_ms": per_op, "per_op_ms_warm_l2": {k: v["ms"] for k, v in warm.items()},
                  "per_op_tflops": {k: v["tflops"] for k, v in cold.items()},
                  "per_op_frac_tensor_peak": {k: v["frac_tensor_peak"] for k, v in cold.items()},
@@ -642,6 +642,21 @@ def main():
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(torch, out_dir, axis, y, dx, dw):
+    """y / dx: DUMP_ROWS minibatch rows drawn with a fixed seed; dw: at most DUMP_BLOCKS blocks, likewise."""
+    os.makedirs(out_dir, exist_ok=True)
+    N = y.shape[0] if axis else y.shape[1]
+    rng = np.random.default_rng(0)
+    rows = np.sort(rng.choice(N, size=min(DUMP_ROWS, N), replace=False))
+    blks = np.sort(rng.choice(dw.shape[0], size=min(DUMP_BLOCKS, dw.shape[0]), replace=False))
+    r = torch.as_tensor(rows, device=y.device)
+    for name, t in (("y", y), ("dx", dx)):
+        np.save(os.path.join(out_dir, name + ".npy"), t.index_select(0 if axis else 1, r).float().cpu().numpy())
+    np.save(os.path.join(out_dir, "dw.npy"), dw.index_select(0, torch.as_tensor(blks, device=dw.device)).float().cpu().numpy())
+    np.save(os.path.join(out_dir, "y_rows.npy"), rows.astype(np.int64))
+    np.save(os.path.join(out_dir, "dw_blocks.npy"), blks.astype(np.int64))
 
 
 def bench_attention(torch, _lib, dev, pk):

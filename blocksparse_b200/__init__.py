@@ -1,8 +1,8 @@
-"""blocksparse_b200 -- B200-native block-sparse matmul / block-sparse attention ops.
+"""blocksparse_b200 -- H100-native block-sparse matmul / block-sparse attention ops.
 
 Drop-in for the hot path of openai/blocksparse: `BlocksparseMatMul` (fprop / bprop /
 updat, group_param_grads) and `BlocksparseTransformer` (NT / NN / TN + masked softmax),
-implemented as hand-written sm_100a CUDA behind the C ABI in include/bsmm_b200.h.
+implemented as hand-written sm_90a CUDA behind the C ABI in include/bsmm_b200.h.
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
 from .optimize import blocksparse_l2_decay, blocksparse_norm, blocksparse_prune

@@ -1,5 +1,6 @@
 // C ABI of libbsmm_b200.so -- argument validation and kernel-family dispatch.
 // See include/bsmm_b200.h for the contract and the reference launchers each entry replaces.
+#include <atomic>
 #include "common.cuh"
 #include "generic.cuh"
 #include "softmax.cuh"
@@ -36,10 +37,8 @@ int bsmm_device_error(void) {
 }
 
 int bsmm_debug_trace(unsigned long long* out, int n) {
-  unsigned long long* b = xprop2_trace_buffer();
-  if (!b || !out || n <= 0 || n > 256 * 8) return fail(BSMM_E_ARG, "bsmm_debug_trace: tracing is off (BSMM_TRACE) or bad arguments");
-  cudaError_t e = cudaMemcpy(out, b, (size_t)n * 8, cudaMemcpyDeviceToHost);
-  return e == cudaSuccess ? 0 : fail((int)e, "bsmm_debug_trace: %s", cudaGetErrorString(e));
+  (void)out; (void)n;
+  return fail(BSMM_E_ARG, "bsmm_debug_trace: no kernel of this build records a trace");
 }
 
 int bsmm_set_wait_timeout_ms(int ms, int trap) {
@@ -53,13 +52,13 @@ int bsmm_set_wait_timeout_ms(int ms, int trap) {
 }
 
 // ---------------------------------------------------------------------------------------
-// A 16-bit call that cannot take the tcgen05 kernel runs ~25x slower on the CUDA-core path: say so once per process (the
+// A 16-bit call that cannot take the wgmma kernel runs many times slower on the CUDA-core path: say so once per process (the
 // reason is whatever tc_* recorded), unless BSMM_QUIET is set.  fp32 calls are expected there and stay silent.
 static void note_fallback(const char* op, int dtype) {
   static std::atomic<bool> warned{false};
   if (dtype == BSMM_F32 || warned.exchange(true)) return;
   if (getenv("BSMM_QUIET")) return;
-  fprintf(stderr, "[bsmm_b200] %s: no tensor-core kernel for this call (%s); using the CUDA-core FMA kernel (about 25x slower). "
+  fprintf(stderr, "[bsmm_b200] %s: no tensor-core kernel for this call (%s); using the CUDA-core FMA kernel (much slower). "
                   "This message is printed once.\n", op, err_buf());
 }
 
@@ -85,17 +84,17 @@ int bsmm_xprop(int dtype, int axis, int bsize, int bprop,
   if (N == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
 
+  (void)sched_list_off; (void)sched_ctas; (void)sched_ntiles;
   if (!(flags & BSMM_FLAG_FORCE_GENERIC)) {
     int rc;
-    if ((sched_tile_blocks >> 16) & 1)       // pair schedule (lut.py:build_pair_schedule) -> csrc/tc_xprop2.cuh
+    if (((sched_tile_blocks >> 16) & 1) && gate == nullptr)   // wide-tile schedule (lut.py:build_wide_schedule) -> csrc/tc_xprop2.cuh
       rc = tc_xprop2(dtype, axis, bprop, n_out, n_in, blocks, x, w, y, N, sched, sched_tiles, (sched_tile_blocks >> 8) & 0xff,
-                     sched_groups_off, sched_list_off, sched_ctas, sched_ntiles, s);
-    else                                      // sched_list_off = optional tile order table (heaviest first) for sched_ntiles minibatch tiles
-      rc = tc_xprop(dtype, axis, bsize, bprop, lut, n_out, n_in, blocks, x, w, y, N, gate, sched, sched_tiles, sched_tile_blocks & 0xffff,
-                    sched_groups_off, sched_list_off, sched_ntiles, s);
+                     sched_groups_off, s);
+    else                                                       // bit 12: 2-CTA clusters sharing the W blocks (pair tiles)
+      rc = tc_xprop(dtype, axis, bsize, bprop, lut, n_out, n_in, blocks, x, w, y, N, gate, (sched_tile_blocks >> 12) & 1, s);
     if (rc != TC_NOT_APPLICABLE) return rc;
     if (flags & BSMM_FLAG_FORCE_TC)
-      return fail(BSMM_E_ARG, "bsmm_xprop: no tcgen05 kernel for dtype=%d axis=%d bsize=%d (%s)", dtype, axis, bsize, err_buf());
+      return fail(BSMM_E_ARG, "bsmm_xprop: no wgmma kernel for dtype=%d axis=%d bsize=%d (%s)", dtype, axis, bsize, err_buf());
     note_fallback("bsmm_xprop", dtype);
   } else if (flags & BSMM_FLAG_FORCE_TC) {
     return fail(BSMM_E_ARG, "bsmm_xprop: contradictory flags");
@@ -135,11 +134,12 @@ int bsmm_updat(int dtype, int dw_dtype, int axis, int bsize,
   cudaStream_t s = (cudaStream_t)stream;
 
   if (!(flags & BSMM_FLAG_FORCE_GENERIC)) {
-    int rc = tc_updat(dtype, dw_dtype, axis, bsize, updat_lut, blocks, n_c_blocks, n_k_blocks, xs, dys, pcount,
-                      dw, N, alpha, beta, gate, gated_dw, sched, sched_tiles, sched_tile_blocks, sched_groups_off, s);
+    (void)sched_groups_off;
+    int rc = tc_updat(dtype, dw_dtype, axis, bsize, n_c_blocks, n_k_blocks, xs, dys, pcount,
+                      dw, N, alpha, beta, gate, gated_dw, sched, sched_tiles, sched_tile_blocks, s);
     if (rc != TC_NOT_APPLICABLE) return rc;
     if (flags & BSMM_FLAG_FORCE_TC)
-      return fail(BSMM_E_ARG, "bsmm_updat: no tcgen05 kernel for dtype=%d axis=%d bsize=%d (%s)", dtype, axis, bsize, err_buf());
+      return fail(BSMM_E_ARG, "bsmm_updat: no wgmma kernel for dtype=%d axis=%d bsize=%d (%s)", dtype, axis, bsize, err_buf());
     note_fallback("bsmm_updat", dtype);
   }
 
@@ -208,10 +208,11 @@ int bst_nt(int dtype, int c_dtype, int bsize,
   cudaStream_t s = (cudaStream_t)stream;
 
   if (!(flags & BSMM_FLAG_FORCE_GENERIC)) {
-    int rc = tc_bst_nt(dtype, c_dtype, bsize, nt_items, n_items, lut_heads, blocks, a, b, c, batch, heads, head_state,
+    (void)nt_items; (void)n_items;
+    int rc = tc_bst_nt(dtype, c_dtype, bsize, nt_lut, lut_heads, blocks, a, b, c, batch, heads, head_state,
                        ctx_blks_a, ctx_blks_b, s);
     if (rc != TC_NOT_APPLICABLE) return rc;
-    if (flags & BSMM_FLAG_FORCE_TC) return fail(BSMM_E_ARG, "bst_nt: no tcgen05 kernel for this configuration (%s)", err_buf());
+    if (flags & BSMM_FLAG_FORCE_TC) return fail(BSMM_E_ARG, "bst_nt: no wgmma kernel for this configuration (%s)", err_buf());
   }
 
   const long long S = (long long)heads * head_state;
@@ -241,10 +242,11 @@ int bst_xn(int a_dtype, int dtype, int bsize, int transpose_a,
   cudaStream_t s = (cudaStream_t)stream;
 
   if (!(flags & BSMM_FLAG_FORCE_GENERIC)) {
-    int rc = tc_bst_xn(a_dtype, dtype, bsize, transpose_a, lut, out_order, lut_heads, blocks, max_lut, a, b, c, batch, heads,
+    (void)out_order; (void)max_lut;
+    int rc = tc_bst_xn(a_dtype, dtype, bsize, transpose_a, lut, lut_heads, blocks, a, b, c, batch, heads,
                        head_state, ctx_blks_b, ctx_blks_c, s);
     if (rc != TC_NOT_APPLICABLE) return rc;
-    if (flags & BSMM_FLAG_FORCE_TC) return fail(BSMM_E_ARG, "bst_xn: no tcgen05 kernel for this configuration (%s)", err_buf());
+    if (flags & BSMM_FLAG_FORCE_TC) return fail(BSMM_E_ARG, "bst_xn: no wgmma kernel for this configuration (%s)", err_buf());
   }
 
   const long long S = (long long)heads * head_state;

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libbsmm_b200.so (sm_100a only).
+// Shared device/host helpers for libbsmm_b200.so (sm_90a only).
 #pragma once
 #include <stdlib.h>
 #include <cuda_runtime.h>
@@ -64,9 +64,8 @@ __host__ __device__ inline int dtype_size(int dt) { return dt == BSMM_F32 ? 4 : 
     default: return bsmm::fail(BSMM_E_BSIZE, "unsupported block size %d", (int)(bs)); \
   }
 
-// sm_grid = SMs the persistent tcgen05 grids are sized for: sm_count minus BSMM_SM_MARGIN (environment, default 0).
-// A margin leaves SMs free for a concurrent NCCL kernel: with every SM taken by persistent CTAs an all-reduce can only
-// run between kernels (profiles/r1_dist_diag.txt).
+// sm_grid = sm_count minus BSMM_SM_MARGIN (environment, default 0): the SMs host-side schedules are balanced for, so that
+// a margin stays free for a concurrent NCCL kernel.
 struct DeviceInfo { int sm_count, cc_major, cc_minor; bool ok; int sm_grid; };
 inline int sm_margin() {
   static const int margin = [] {

@@ -1,7 +1,7 @@
 // CUDA-core kernel families (fp32 FMA, any storage dtype, block size 8/16/32/64).
 //
 // These are the true-fp32 path (BASELINE cfg 1, <=1e-5) and the fallback for the
-// (dtype, block size, axis) combinations that have no tcgen05 kernel.  Two shapes
+// (dtype, block size, axis) combinations that have no wgmma kernel.  Two shapes
 // cover the whole hot path:
 //
 //   sdd_xn : sparse . dense -> dense     (bsmm fprop/bprop, bst NN/TN)
@@ -283,7 +283,7 @@ __global__ void gate_grad_kernel(const T* __restrict__ dw, const T* __restrict__
 }
 
 // w_out[w] = gate[w] * w[w]  (a zero gate gives an exact zero block).  Lets a gated fprop / bprop of 16-bit weights run
-// on the tcgen05 kernel: the reference's gated tensor-core kernels also scale the loaded 16-bit weights by the gate.
+// on the wgmma kernel: the reference's gated tensor-core kernels also scale the loaded 16-bit weights by the gate.
 template <typename T>
 __global__ void gate_weights_kernel(const T* __restrict__ w, const float* __restrict__ gate, T* __restrict__ out,
                                     long long total, int elems) {

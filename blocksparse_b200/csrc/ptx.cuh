@@ -1,7 +1,7 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) features the tensor-core kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / cp) and the
-// shared-memory / instruction descriptors.  No CUTLASS: bit layouts follow the PTX ISA
-// (cross-checked against cute/arch/mma_sm100_desc.hpp, which documents the same fields).
+// Thin inline-PTX wrappers for the Hopper (sm_90a) features the tensor-core kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor) and warpgroup MMA (wgmma.mma_async) with its shared-memory
+// matrix descriptor.  No CUTLASS: bit layouts follow the PTX ISA ("Matrix Descriptor Format" of the
+// asynchronous warpgroup-level matrix instructions).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -12,15 +12,6 @@ namespace ptx {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 // ---- mbarrier -------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -29,15 +20,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -52,9 +37,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a barrier that does not flip within g_wait_timeout_ns of wall clock (default 2 s, host-settable
 // through bsmm_set_wait_timeout_ms) is a protocol bug or a starved kernel.  The first wait that gives up records
-// code 100 in g_wait_error and -- unless trapping is disabled (probes, tests of the error path) -- executes
-// `trap`, so that the launch FAILS (the next CUDA call of the host returns a fault) instead of completing with
-// partially written outputs.
+// code 100 in g_wait_error and -- unless trapping is disabled -- executes `trap`, so that the launch FAILS (the
+// next CUDA call of the host returns a fault) instead of completing with partially written outputs.
 __device__ unsigned long long g_wait_timeout_ns = 2000000000ull;
 __device__ int g_wait_trap = 1;
 __device__ int g_wait_error = 0;
@@ -68,72 +52,38 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// `abort_flag` (shared memory) is raised by whichever wait times out first, and makes every other
-// wait of the CTA return immediately so a deadlock costs one timeout, not one per wait.
-__device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, volatile int* abort_flag = nullptr) {
+__device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return true;
   const uint64_t t0 = globaltimer_ns();
   for (;;) {
 #pragma unroll 1
     for (int i = 0; i < 64; ++i)
       if (mbar_try_wait(bar, parity)) return true;
-    if (abort_flag && *abort_flag) return false;
     if (globaltimer_ns() - t0 > g_wait_timeout_ns) {
-      if (abort_flag) *abort_flag = 1;
       wait_timed_out();
       return false;
     }
   }
 }
 
-// Hide a value's provenance from the optimiser (otherwise it re-materialises shared-window addresses at every use).
-__device__ __forceinline__ uint32_t opaque(uint32_t v) {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %1;" : "=r"(r) : "r"(v));
-  return r;
+// ---- TMA ---------------------------------------------------------------------------------
+__device__ __forceinline__ void prefetch_tensormap(const void* tmap) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
 }
-// Address-based variants: shared-window addresses on sm_100 embed the CTA rank (S2UR SR_CgaCtaId + LEA per cvta),
-// so hot loops convert a barrier array's base ONCE and index it arithmetically.
-__device__ __forceinline__ bool mbar_try_wait_a(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ bool mbar_wait_a(uint32_t bar, uint32_t parity, volatile int* abort_flag) {
-  if (mbar_try_wait_a(bar, parity)) return true;
-  const uint64_t t0 = globaltimer_ns();
-  for (;;) {
-#pragma unroll 1
-    for (int i = 0; i < 64; ++i)
-      if (mbar_try_wait_a(bar, parity)) return true;
-    if (abort_flag && *abort_flag) return false;
-    if (globaltimer_ns() - t0 > g_wait_timeout_ns) {
-      if (abort_flag) *abort_flag = 1;
-      wait_timed_out();
-      return false;
-    }
-  }
-}
-__device__ __forceinline__ void mbar_expect_tx_a(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const void* tmap, uint32_t bar, int c0, int c1) {
+__device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, int a, int b, int c, int d) {
-  asm volatile("st.shared.v4.s32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ void tc_commit_a(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+
+// TMA load delivered to every CTA of `mask` (thread-block cluster) at the same CTA-relative shared-memory offset; each
+// destination's mbarrier at the same offset receives the complete_tx for the bytes that landed there.
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
 }
 
 // ---- thread-block clusters ------------------------------------------------------------------
@@ -145,194 +95,117 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// TMA load delivered to every CTA of `mask` at the same CTA-relative shared-memory offset; each destination's mbarrier (same
-// offset) receives the complete_tx for the bytes that landed there.
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t smem_dst, const void* tmap, uint32_t bar, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-// tcgen05.commit that arrives on the mbarrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void tc_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
+
+// ---- wgmma ---------------------------------------------------------------------------------
+// Swizzle modes of the wgmma matrix descriptor (bits 62-63).
+enum : uint32_t { SWZ_NONE = 0, SWZ_128B = 1, SWZ_64B = 2, SWZ_32B = 3 };
+// Swizzle mode whose span equals a row of `row_bytes` (32, 64 or 128): the layout TMA writes with the matching
+// CU_TENSOR_MAP_SWIZZLE_*.
+__host__ __device__ constexpr uint32_t swz_for_row(int row_bytes) {
+  return row_bytes == 128 ? SWZ_128B : row_bytes == 64 ? SWZ_64B : SWZ_32B;
 }
 
-// ---- TMA ---------------------------------------------------------------------------------
-__device__ __forceinline__ void prefetch_tensormap(const void* tmap) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N> __device__ __forceinline__ void tma_store_wait() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// ---- tcgen05 ----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {     // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {       // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; one thread issues.
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A-collector hints (PTX ISA "collector_usage"): fill = keep A in the collector after this MMA,
-// use = A is already there (same descriptor as the previous MMA), lastuse = use and release.
-__device__ __forceinline__ void mma_ss_a_fill(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16.collector::a::fill [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ss_a_use(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16.collector::a::use [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ss_a_lastuse(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16.collector::a::lastuse [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05 async ops of this thread complete.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// smem -> tmem copy of a 128-lane x 256-bit slab (one K=16 slice of a 16-bit A operand)
-__device__ __forceinline__ void tc_cp_128x256b(uint32_t dst_tmem, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(dst_tmem), "l"(sdesc) : "memory");
-}
-
-// TMEM -> registers: each thread of the warp reads its own lane, N consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM (used by probes to stage an A operand)
-__device__ __forceinline__ void tmem_st_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-// zero 32 consecutive 32-bit columns of this thread's lane
-__device__ __forceinline__ void tmem_st_zero_x32(uint32_t taddr) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, "
-      "%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};"
-      ::"r"(taddr), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_zero_x16(uint32_t taddr) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};"
-      ::"r"(taddr), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- descriptors ---------------------------------------------------------------------------
-enum : uint32_t { SWZ_NONE = 0, SWZ_128B = 2, SWZ_64B = 4, SWZ_32B = 6 };
-
-// Shared-memory matrix descriptor (PTX ISA "tcgen05 matrix descriptor"):
-//   [ 0,14) start address >> 4      [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1 on sm_100
-//   [49,52) base offset (0: tiles are aligned to the swizzle repeat)   [61,64) swizzle mode
-__host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                            uint32_t swizzle) {
+// Shared-memory matrix descriptor:
+//   [ 0,14) start address >> 4      [16,30) leading-dimension byte offset >> 4
+//   [32,46) stride-dimension byte offset >> 4   [49,52) base offset (0: tiles aligned to the swizzle repeat)
+//   [62,64) swizzle mode
+// Swizzled K-major operands: rows of one swizzle span, SBO = distance between 8-row groups, LBO unused; a K=16 step
+// advances the start address by 32 bytes.  Swizzled MN-major operands: atoms of (span) MN elements x 8 K rows,
+// SBO = distance between 8-row K groups, LBO = distance between atoms along MN.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swizzle) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(swizzle & 7) << 61;
+  d |= (uint64_t)(swizzle & 3) << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16 (fp16/bf16 inputs, fp32 accumulate):
-//   [4,6) D format (1 = f32)  [7,10) A format  [10,13) B format (0 = f16, 1 = bf16)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(bool bf16, bool a_mn_major, bool b_mn_major, int M, int N) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= (bf16 ? 1u : 0u) << 7;
-  d |= (bf16 ? 1u : 0u) << 10;
-  d |= (a_mn_major ? 1u : 0u) << 15;
-  d |= (b_mn_major ? 1u : 0u) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Keeps the compiler from moving accumulator reads / writes across wgmma issue and wait.
+template <int R> __device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (fp32, registers) += A[64 x 16] * B[16 x N], both operands in shared memory (descriptors).
+// TA / TB: 0 = K-major, 1 = MN-major.  Accumulator layout (per warp w of the warpgroup, lane l):
+//   d[4j + 2h + e] = D[16w + l/4 + 8h][8j + 2(l%4) + e]
+#define BSMM_WG_OPS8(o)  "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), \
+                         "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+#define BSMM_WG_TAIL(bf, n)                                                                                      \
+  "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                                               \
+  "wgmma.mma_async.sync.aligned.m64n" #n "k16.f32." bf "." bf " "
+
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t a, uint64_t b) {
+  if constexpr (BF16)
+    asm volatile(BSMM_WG_TAIL("bf16", 16) "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %10, %11;\n\t}\n"
+                 : BSMM_WG_OPS8(0) : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  else
+    asm volatile(BSMM_WG_TAIL("f16", 16) "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %10, %11;\n\t}\n"
+                 : BSMM_WG_OPS8(0) : "l"(a), "l"(b), "n"(TA), "n"(TB));
+}
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b) {
+  if constexpr (BF16)
+    asm volatile(BSMM_WG_TAIL("bf16", 32)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %18, %19;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8) : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  else
+    asm volatile(BSMM_WG_TAIL("f16", 32)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %18, %19;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8) : "l"(a), "l"(b), "n"(TA), "n"(TB));
+}
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b) {
+  if constexpr (BF16)
+    asm volatile(BSMM_WG_TAIL("bf16", 64)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %34, %35;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24)
+                 : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  else
+    asm volatile(BSMM_WG_TAIL("f16", 64)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %34, %35;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24)
+                 : "l"(a), "l"(b), "n"(TA), "n"(TB));
+}
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b) {
+  if constexpr (BF16)
+    asm volatile(BSMM_WG_TAIL("bf16", 128)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+                 "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %66, %67;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24),
+                   BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56)
+                 : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  else
+    asm volatile(BSMM_WG_TAIL("f16", 128)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+                 "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %66, %67;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24),
+                   BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56)
+                 : "l"(a), "l"(b), "n"(TA), "n"(TB));
+}
+// N = 16, 32, 64 or 128 dispatch
+template <bool BF16, int TA, int TB, int N>
+__device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b) {
+  if constexpr (N == 16) wgmma_n16<BF16, TA, TB>(d, a, b);
+  else if constexpr (N == 32) wgmma_n32<BF16, TA, TB>(d, a, b);
+  else if constexpr (N == 64) wgmma_n64<BF16, TA, TB>(d, a, b);
+  else wgmma_n128<BF16, TA, TB>(d, a, b);
+}
+#undef BSMM_WG_TAIL
+#undef BSMM_WG_OPS8
 
 }  // namespace ptx

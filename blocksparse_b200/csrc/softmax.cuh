@@ -229,8 +229,7 @@ bst_softmax_kernel(const SoftmaxParams p) {
 // shared-memory access is one whole row of one block, conflict free -- keep the row's values in registers across max / exp /
 // sum / normalise, write the 16-bit results back IN PLACE, and one thread sends every piece to HBM with a bulk store.  HBM
 // sees each element exactly once in and once out, in 1-2 KB bursts, and with ~22 KB of shared memory per CTA ten CTAs share
-// an SM, so loads, arithmetic and stores of different chunks overlap.  (First version: one CTA per whole query block, 88 KB,
-// two per SM, phases serialised: 0.347 ms at cfg 3 against 0.165 ms for the register kernel, profiles/r2_softmax.txt.)
+// an SM, so loads, arithmetic and stores of different chunks overlap.
 constexpr int SOFTMAX_STAGED_THREADS = 128;
 constexpr int SOFTMAX_STAGED_ROWS = 16;
 

@@ -1,418 +1,202 @@
-// tcgen05 kernels for the block-sparse transformer GEMMs, block size 64, 16-bit dense operands.
+// wgmma kernels for the block-sparse transformer GEMMs, block size 64, 16-bit dense operands.
 //   tc_bst_nt_kernel : C[b,h,blk] = A[b, q-blk, h, :] . B[b, k-blk, h, :]^T          (dense . dense^T -> sparse)
 //                      replaces bst_hgemm_64x64x64_nt      (reference src/bst_hgemm_op_gpu.cu:651-1098)
 //   tc_bst_xn_kernel : C[b, o-blk, h, :] = sum_j op(A[b,h,blk_j]) . B[b, in_j, h, :]   (sparse . dense -> dense)
 //                      replaces bst_hgemm_64x64x64_xn<OP_A> (reference src/bst_hgemm_op_gpu.cu:16-646)
 //
-// Both ops are memory-bound at head_state 64 (SURVEY section 8d: ~32 flop/B), so the formulation favours simple,
-// fully coalesced traffic over tensor-pipe utilisation:
-//   NT: blocks that share a key block are processed two at a time -- their two 64-row query tiles are stacked into
-//       one M=128 A operand (two TMA boxes), B = the key tile, D[128 x 64] = both score blocks.  The head split is
-//       a TMA coordinate (column h*head_state), so no transpose kernel exists, as in the reference.
-//   XN: one CTA tile = one 64-row output block; the M=128 MMA reads 64 valid rows of the sparse block plus 64 stale
-//       rows of shared memory (rows of D are independent, the upper half is simply never read back), which avoids
-//       both the M=64 TMEM layout and doubling the global traffic of the sparse tensor.  NN uses a K-major A,
-//       TN the same tile as an MN-major A (transpose for free in the descriptor).
+// Both ops are memory-bound at head_state 64 (~32 flop/B), so the formulation favours simple,
+// fully coalesced TMA traffic and many small CTAs in flight over tensor-pipe utilisation.  One warpgroup per CTA:
+//   NT: one 64 x 64 score block per CTA: A = the query tile, B = the key tile, both K-major with the head split as a
+//       TMA coordinate (column h*head_state), so no transpose kernel exists, as in the reference.
+//   XN: one 64-row output block per CTA walking its LUT row through a ring of TMA stages.  NN reads the sparse block
+//       K-major, TN reads the same tile MN-major (transpose for free in the descriptor); B is the dense tile, MN-major.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace bsmm {
 
-constexpr int BST_THREADS = 6 * 32;      // warp 0 producer, warp 1 MMA, warps 2..5 epilogue
+constexpr int BST_THREADS = 128;
 constexpr int BST_STAGES = 4;
-constexpr int BST_NT_STAGES = 3;
 constexpr uint32_t BST_TILE = 64 * 64 * 2;   // one 64 x 64 16-bit tile with 128-byte rows (SW128)
 
 // ------------------------------------------------------------------------------------------------
 struct BstNtParams {
-  const int32_t* items;     // [lut_heads][n_items][8] = (k_blk, n_valid, blk0, q0, blk1, q1, -, -)
-  int n_items, lut_heads;
-  int batch, heads, blocks, head_state;
+  const int32_t* lut;       // [lut_heads][blocks][2] = (query block, key block)
+  long long lut_head_stride;
+  int heads, blocks, head_state;
   int ctx_rows_a, ctx_rows_b;   // rows per batch element of a / b
   void* c;
-  int tma_store;            // 16-bit outputs: stage the 8 KB block in shared memory and store it with one TMA op
 };
-struct BstNtTmaps { CUtensorMap a, b, c; };   // c: the sparse output as [batch*heads*blocks*64][64] (16-bit outputs only)
+struct BstNtTmaps { CUtensorMap a, b; };
 
 template <bool BF16, typename TC>
-__global__ void __launch_bounds__(BST_THREADS, 2)
+__global__ void __launch_bounds__(BST_THREADS)
 tc_bst_nt_kernel(const BstNtParams p, const __grid_constant__ BstNtTmaps maps) {
-  constexpr int ST = BST_NT_STAGES;                        // 72 KB of stages + 32 KB of output staging: two CTAs per SM
-  constexpr uint32_t STAGE_BYTES = 3 * BST_TILE;          // two query tiles + one key tile
-  constexpr int NBUF = 4;                                  // accumulator buffers of 64 columns
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sOut = smem + ST * STAGE_BYTES;                 // 2 x (two 8 KB blocks) of output staging
-  __shared__ uint64_t full[ST], empty[ST], acc_full[NBUF], acc_empty[NBUF];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ int abort_s;
-  volatile int* abort_flag = &abort_s;
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid / 32, 0), lane = tid % 32;   // provably warp-uniform role index
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ uint64_t full;
+  const uint32_t base = aligned_smem_base(smem_raw);          // query chunks at 0 / 8 KB, key chunks at 16 / 24 KB
+  const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
   const int chunks = p.head_state / 64;
-  const long long total = (long long)p.batch * p.heads * p.n_items;
+  const int blk = (int)(blockIdx.x % (unsigned)p.blocks);
+  const int z = (int)(blockIdx.x / (unsigned)p.blocks);
+  const int b = z / p.heads, h = z % p.heads;
+  const int32_t* lut = p.lut + h * p.lut_head_stride;
+  const int qb = lut[2 * blk], kb = lut[2 * blk + 1];
 
   if (tid == 0) {
-    abort_s = 0;
-    for (int i = 0; i < ST; ++i) { ptx::mbar_init(&full[i], 1); ptx::mbar_init(&empty[i], 1); }
-    for (int i = 0; i < NBUF; ++i) { ptx::mbar_init(&acc_full[i], 1); ptx::mbar_init(&acc_empty[i], 1); }
+    ptx::mbar_init(&full, 1);
     ptx::fence_mbar_init();
+    ptx::mbar_expect_tx(&full, (uint32_t)(2 * chunks) * BST_TILE);
+    for (int c = 0; c < chunks; ++c) {
+      const int col = h * p.head_state + c * 64;
+      ptx::tma_load_2d(base + c * BST_TILE, &maps.a, &full, col, b * p.ctx_rows_a + qb * 64);
+      ptx::tma_load_2d(base + (2 + c) * BST_TILE, &maps.b, &full, col, b * p.ctx_rows_b + kb * 64);
+    }
   }
-  if (warp == 1) { ptx::tmem_alloc(&tmem_base_s, 256); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  if (!ptx::mbar_wait(&full, 0)) g_tc_error = 21;
+  ptx::wg_fence();
+  for (int c = 0; c < chunks; ++c)
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks)
+      ptx::wgmma_n64<BF16, 0, 0>(acc, ptx::make_desc(base + c * BST_TILE + ks * 32, 16, 1024, ptx::SWZ_128B),
+                                 ptx::make_desc(base + (2 + c) * BST_TILE + ks * 32, 16, 1024, ptx::SWZ_128B));
+  ptx::wg_commit();
+  ptx::wg_wait<0>();
+  ptx::wg_fence_regs(acc);
 
-  if (warp == 0) {
-    uint32_t sc = 0;
-    bool alive = true;
-    for (long long it = blockIdx.x; it < total && alive; it += gridDim.x) {
-      const int item = (int)(it % p.n_items);
-      const int bh = (int)(it / p.n_items);
-      const int b = bh / p.heads, h = bh % p.heads;
-      const int32_t* rec = p.items + ((size_t)(p.lut_heads > 1 ? h : 0) * p.n_items + item) * 8;
-      const int kb = rec[0], nv = rec[1], q0 = rec[3], q1 = rec[5];
-      for (int c = 0; c < chunks; ++c, ++sc) {
-        const uint32_t st = sc % ST;
-        if (!__all_sync(0xffffffffu, ptx::mbar_wait(&empty[st], ((sc / ST) & 1) ^ 1, abort_flag))) { g_tc_error = 21; alive = false; break; }
-        uint8_t* stage = smem + st * STAGE_BYTES;
-        const int col = h * p.head_state + c * 64;
-        if (lane == 0) {
-          ptx::mbar_expect_tx(&full[st], (uint32_t)(nv + 1) * BST_TILE);
-          if (nv > 0) ptx::tma_load_2d(stage, &maps.a, &full[st], col, b * p.ctx_rows_a + q0 * 64);
-          if (nv > 1) ptx::tma_load_2d(stage + BST_TILE, &maps.a, &full[st], col, b * p.ctx_rows_a + q1 * 64);
-          ptx::tma_load_2d(stage + 2 * BST_TILE, &maps.b, &full[st], col, b * p.ctx_rows_b + kb * 64);
-        }
-        __syncwarp();
-      }
+  TC* out = reinterpret_cast<TC*>(p.c) + ((size_t)z * p.blocks + blk) * 64 * 64;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int row = warp * 16 + lane / 4 + 8 * hh;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int col = 8 * j + 2 * (lane % 4);
+      const float v0 = acc[4 * j + 2 * hh], v1 = acc[4 * j + 2 * hh + 1];
+      if constexpr (sizeof(TC) == 4) *reinterpret_cast<float2*>(out + row * 64 + col) = make_float2(v0, v1);
+      else *reinterpret_cast<uint32_t*>(out + row * 64 + col) = pack2<std::is_same<TC, __nv_bfloat16>::value>(v0, v1);
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = ptx::make_idesc_f16(BF16, false, false, 128, 64);
-    const uint64_t a_desc0 = ptx::make_smem_desc(ptx::smem_u32(smem), 16, 1024, ptx::SWZ_128B);
-    const uint64_t b_desc0 = ptx::make_smem_desc(ptx::smem_u32(smem) + 2 * BST_TILE, 16, 1024, ptx::SWZ_128B);
-    uint32_t sc = 0, n = 0;
-    bool alive = true;
-    for (long long it = blockIdx.x; it < total && alive; it += gridDim.x, ++n) {
-      const uint32_t buf = n % NBUF;
-      if (!__all_sync(0xffffffffu, ptx::mbar_wait(&acc_empty[buf], ((n / NBUF) & 1) ^ 1, abort_flag))) { g_tc_error = 23; break; }
-      ptx::tc_fence_after();
-      for (int c = 0; c < chunks; ++c, ++sc) {
-        const uint32_t st = sc % ST;
-        if (!__all_sync(0xffffffffu, ptx::mbar_wait(&full[st], (sc / ST) & 1, abort_flag))) { g_tc_error = 24; alive = false; break; }
-        ptx::tc_fence_after();
-        if (ptx::elect_one()) {
-          const uint64_t a_st = a_desc0 + (uint64_t)((st * STAGE_BYTES) >> 4);
-          const uint64_t b_st = b_desc0 + (uint64_t)((st * STAGE_BYTES) >> 4);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            ptx::mma_ss(tmem + buf * 64, a_st + (uint64_t)(ks * 2), b_st + (uint64_t)(ks * 2), idesc, (c > 0 || ks > 0) ? 1u : 0u);
-          ptx::tc_commit(&empty[st]);
-        }
-        __syncwarp();
-      }
-      if (ptx::elect_one()) ptx::tc_commit(&acc_full[buf]);
-      __syncwarp();
-    }
-  } else {
-    const int quad = warp & 3;
-    const int half = quad >> 1;                         // which of the two stacked blocks
-    const int row = (quad & 1) * 32 + lane;             // query row inside the block
-    TC* cbase = reinterpret_cast<TC*>(p.c);
-    uint32_t n = 0;
-    for (long long it = blockIdx.x; it < total; it += gridDim.x, ++n) {
-      const int item = (int)(it % p.n_items);
-      const int bh = (int)(it / p.n_items);
-      const int h = bh % p.heads;
-      const int32_t* rec = p.items + ((size_t)(p.lut_heads > 1 ? h : 0) * p.n_items + item) * 8;
-      const int nv = rec[1];
-      const int blk = half ? rec[4] : rec[2];
-      const uint32_t buf = n % NBUF;
-      ptx::mbar_wait(&acc_full[buf], (n / NBUF) & 1, abort_flag);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (*abort_flag) { g_tc_error = 26; break; }
-      ptx::tc_fence_after();
-      if constexpr (sizeof(TC) == 2) {
-        if (p.tma_store) {
-          // A thread owns one 128-byte row of a block; writing rows straight to global memory costs one 16-byte
-          // request per lane (profiles: L1->L2 request port 56 % busy, HBM 41 %).  Stage the block swizzled (the
-          // layout the SW128 tensor map expects) and let one TMA store write the contiguous 8 KB.
-          uint8_t* sbuf = sOut + (n & 1u) * (2 * BST_TILE);
-          if (warp == 2 && lane == 0) ptx::tma_store_wait_read<1>();      // the store that last read this buffer is done
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          if (half < nv) {
-            uint8_t* dst = sbuf + half * BST_TILE + row * 128;
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              uint32_t v[32];
-              ptx::tmem_ld_x32(tmem + ((uint32_t)(quad * 32) << 16) + buf * 64 + hh * 32, v);
-              ptx::tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                uint32_t pk[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float a = __uint_as_float(v[8 * i + 2 * e]), bq = __uint_as_float(v[8 * i + 2 * e + 1]);
-                  typename Pair<TC>::type q; q.x = from_f32<TC>(a); q.y = from_f32<TC>(bq);
-                  pk[e] = *reinterpret_cast<uint32_t*>(&q);
-                }
-                const uint32_t chunk = (uint32_t)(hh * 4 + i);
-                *reinterpret_cast<uint4*>(dst + ((chunk ^ ((uint32_t)row & 7u)) * 16)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-              }
-            }
-          }
-          ptx::tc_fence_before();
-          ptx::fence_proxy_async();
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          if (warp == 2 && lane == 0) {
-            ptx::mbar_arrive(&acc_empty[buf]);
-            for (int hb = 0; hb < nv; ++hb)
-              ptx::tma_store_2d(&maps.c, sbuf + hb * BST_TILE, 0, (int)(((long long)bh * p.blocks + rec[2 + 2 * hb]) * 64));
-            ptx::tma_store_commit();
-          }
-          continue;
-        }
-      }
-      if (half < nv) {
-        TC* out = cbase + (((size_t)bh * p.blocks + blk) * 64 + row) * 64;
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          uint32_t v[32];
-          ptx::tmem_ld_x32(tmem + ((uint32_t)(quad * 32) << 16) + buf * 64 + hh * 32, v);
-          ptx::tmem_ld_wait();
-          if constexpr (sizeof(TC) == 4) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              reinterpret_cast<float4*>(out + hh * 32)[i] = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]),
-                                                                        __uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3]));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              uint32_t pk[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float a = __uint_as_float(v[8 * i + 2 * e]), bq = __uint_as_float(v[8 * i + 2 * e + 1]);
-                typename Pair<TC>::type q; q.x = from_f32<TC>(a); q.y = from_f32<TC>(bq);
-                pk[e] = *reinterpret_cast<uint32_t*>(&q);
-              }
-              reinterpret_cast<uint4*>(out + hh * 32)[i] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            }
-          }
-        }
-      }
-      ptx::tc_fence_before();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (warp == 2 && lane == 0) ptx::mbar_arrive(&acc_empty[buf]);
-    }
-    if (warp == 2 && lane == 0) ptx::tma_store_wait<0>();
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem, 256);
 }
 
 // ------------------------------------------------------------------------------------------------
 struct BstXnParams {
   const int32_t* lut;       // [lut_heads][n_out + blocks][2]
-  const int32_t* order;     // optional [lut_heads][n_out]: output blocks by decreasing LUT row length (longest first)
   long long lut_head_stride;
-  int n_out, lut_heads;
-  int batch, heads, blocks, head_state;
+  int n_out, heads, blocks, head_state;
   int ctx_rows_b, ctx_rows_c;
-  int transpose_a;
   void* c;
 };
 struct BstXnTmaps { CUtensorMap a, b; };
 
-template <bool BF16>
-__global__ void __launch_bounds__(BST_THREADS, 2)
+template <bool BF16, bool TRANS_A>
+__global__ void __launch_bounds__(BST_THREADS)
 tc_bst_xn_kernel(const BstXnParams p, const __grid_constant__ BstXnTmaps maps) {
   constexpr int ST = BST_STAGES;
-  // stage: A tile (64 valid rows) + B up to 2 tiles (head_state <= 128).  The M=128 MMA also reads 64 rows past the
-  // A tile -- that is the first B tile; those accumulator lanes (64..127) are never read back.  96 KB of stages and
-  // 256 TMEM columns per CTA => two CTAs per SM, i.e. 8 stages in flight per SM (the kernel is bound by the TMA round trip).
-  constexpr uint32_t STAGE_BYTES = 3 * BST_TILE;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t full[ST], empty[ST], acc_full[2], acc_empty[2];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ int abort_s;
-  volatile int* abort_flag = &abort_s;
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid / 32, 0), lane = tid % 32;   // provably warp-uniform role index
-  const int chunks = p.head_state / 64;              // 1 or 2 column atoms of B / D
-  const long long total = (long long)p.batch * p.heads * p.n_out;
+  constexpr uint32_t STAGE_BYTES = 3 * BST_TILE;     // sparse block + up to two 64-column tiles of B (head_state <= 128)
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ uint64_t full[ST];
+  const uint32_t base = aligned_smem_base(smem_raw);
+  const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
+  const int chunks = p.head_state / 64;
+  const int o = (int)(blockIdx.x % (unsigned)p.n_out);
+  const int z = (int)(blockIdx.x / (unsigned)p.n_out);
+  const int b = z / p.heads, h = z % p.heads;
+  const int32_t* lut = p.lut + h * p.lut_head_stride;
+  const int first = lut[2 * o], count = lut[2 * o + 1];
+  const int2* ent = reinterpret_cast<const int2*>(lut) + first;
 
+  auto issue = [&](int e) {                          // one thread: stage entry e = (sparse block, input block)
+    const int2 bi = ent[e];
+    const uint32_t st = base + (uint32_t)(e % ST) * STAGE_BYTES;
+    uint64_t* bar = &full[e % ST];
+    ptx::mbar_expect_tx(bar, (uint32_t)(1 + chunks) * BST_TILE);
+    ptx::tma_load_2d(st, &maps.a, bar, 0, (int)(((long long)z * p.blocks + bi.x) * 64));
+    for (int c = 0; c < chunks; ++c)
+      ptx::tma_load_2d(st + (1 + c) * BST_TILE, &maps.b, bar, h * p.head_state + c * 64, b * p.ctx_rows_b + bi.y * 64);
+  };
   if (tid == 0) {
-    abort_s = 0;
-    for (int i = 0; i < ST; ++i) { ptx::mbar_init(&full[i], 1); ptx::mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&acc_full[i], 1); ptx::mbar_init(&acc_empty[i], 1); }
+    for (int i = 0; i < ST; ++i) ptx::mbar_init(&full[i], 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) { ptx::tmem_alloc(&tmem_base_s, 256); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
+  if (tid == 0)
+    for (int e = 0; e < count && e < ST; ++e) issue(e);
 
-  if (warp == 0) {
-    uint32_t sc = 0;
-    bool alive = true;
-    for (long long it = blockIdx.x; it < total && alive; it += gridDim.x) {
-      const int bh = (int)(it / p.n_out);
-      const int b = bh / p.heads, h = bh % p.heads;
-      const int hl = p.lut_heads > 1 ? h : 0;
-      const int o = p.order ? p.order[hl * p.n_out + (int)(it % p.n_out)] : (int)(it % p.n_out);
-      const int32_t* lut = p.lut + hl * p.lut_head_stride;
-      const int first = lut[2 * o], count = lut[2 * o + 1];
-      const int2* ent = reinterpret_cast<const int2*>(lut) + first;
-      for (int e0 = 0; e0 < count && alive; e0 += 32) {
-        const int2 my = (e0 + lane < count) ? ent[e0 + lane] : make_int2(0, 0);
-        const int m = min(32, count - e0);
-        for (int e = 0; e < m; ++e, ++sc) {
-          const int blk = __shfl_sync(0xffffffffu, my.x, e);
-          const int in = __shfl_sync(0xffffffffu, my.y, e);
-          const uint32_t st = sc % ST;
-          if (!__all_sync(0xffffffffu, ptx::mbar_wait(&empty[st], ((sc / ST) & 1) ^ 1, abort_flag))) { g_tc_error = 31; alive = false; break; }
-          uint8_t* stage = smem + st * STAGE_BYTES;
-          if (lane == 0) {
-            ptx::mbar_expect_tx(&full[st], (uint32_t)(1 + chunks) * BST_TILE);
-            ptx::tma_load_2d(stage, &maps.a, &full[st], 0, (int)(((long long)bh * p.blocks + blk) * 64));
-            for (int c = 0; c < chunks; ++c)
-              ptx::tma_load_2d(stage + (1 + c) * BST_TILE, &maps.b, &full[st], h * p.head_state + c * 64, b * p.ctx_rows_b + in * 64);
-          }
-          __syncwarp();
-        }
-      }
+  float acc[2][32];
+#pragma unroll
+  for (int c = 0; c < 2; ++c)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+  for (int e = 0; e < count; ++e) {
+    const uint32_t st = base + (uint32_t)(e % ST) * STAGE_BYTES;
+    if (!ptx::mbar_wait(&full[e % ST], (uint32_t)(e / ST) & 1)) g_tc_error = 31;
+    ptx::wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      // NN: A[i][j], M = i, K = j contiguous (K-major).  TN: A^T, M = j contiguous (MN-major), K=16 step = 16 rows.
+      const uint64_t adesc = TRANS_A ? ptx::make_desc(st + ks * 2048, BST_TILE, 1024, ptx::SWZ_128B)
+                                     : ptx::make_desc(st + ks * 32, 16, 1024, ptx::SWZ_128B);
+      // B = dense tile [64 rows = K][64 columns = N], MN-major
+      ptx::wgmma_n64<BF16, TRANS_A ? 1 : 0, 1>(acc[0], adesc, ptx::make_desc(st + BST_TILE + ks * 2048, BST_TILE, 1024, ptx::SWZ_128B));
+      if (chunks == 2)
+        ptx::wgmma_n64<BF16, TRANS_A ? 1 : 0, 1>(acc[1], adesc, ptx::make_desc(st + 2 * BST_TILE + ks * 2048, BST_TILE, 1024, ptx::SWZ_128B));
     }
-  } else if (warp == 1) {
-    // NN: A[blk][i][j], M = i, K = j contiguous -> K-major, K=16 slice = +32 B.
-    // TN: A^T, M = j contiguous -> MN-major SW128 (one 64-wide atom + 64 stale columns: LBO = one tile), K=16 slice = 16 rows.
-    const uint32_t idesc = ptx::make_idesc_f16(BF16, p.transpose_a != 0, true, 128, p.head_state);
-    const uint64_t a_desc0 = p.transpose_a ? ptx::make_smem_desc(ptx::smem_u32(smem), BST_TILE, 1024, ptx::SWZ_128B)
-                                           : ptx::make_smem_desc(ptx::smem_u32(smem), 16, 1024, ptx::SWZ_128B);
-    const uint32_t a_kstep16 = p.transpose_a ? (2048u >> 4) : 2u;
-    // B = V tile [64 keys][head_state], MN-major SW128: 64-column atoms one tile apart, K=16 slice = 16 rows
-    const uint64_t b_desc0 = ptx::make_smem_desc(ptx::smem_u32(smem) + BST_TILE, BST_TILE, 1024, ptx::SWZ_128B);
-    uint32_t sc = 0, n = 0;
-    bool alive = true;
-    for (long long it = blockIdx.x; it < total && alive; it += gridDim.x, ++n) {
-      const int h = (int)((it / p.n_out) % p.heads);
-      const int hl = p.lut_heads > 1 ? h : 0;
-      const int o = p.order ? p.order[hl * p.n_out + (int)(it % p.n_out)] : (int)(it % p.n_out);
-      const int32_t* lut = p.lut + hl * p.lut_head_stride;
-      const int count = lut[2 * o + 1];
-      const uint32_t buf = n & 1;
-      if (!__all_sync(0xffffffffu, ptx::mbar_wait(&acc_empty[buf], ((n >> 1) & 1) ^ 1, abort_flag))) { g_tc_error = 33; break; }
-      ptx::tc_fence_after();
-      for (int e = 0; e < count; ++e, ++sc) {
-        const uint32_t st = sc % ST;
-        if (!__all_sync(0xffffffffu, ptx::mbar_wait(&full[st], (sc / ST) & 1, abort_flag))) { g_tc_error = 34; alive = false; break; }
-        ptx::tc_fence_after();
-        if (ptx::elect_one()) {
-          const uint64_t a_st = a_desc0 + (uint64_t)((st * STAGE_BYTES) >> 4);
-          const uint64_t b_st = b_desc0 + (uint64_t)((st * STAGE_BYTES) >> 4);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            ptx::mma_ss(tmem + buf * 128, a_st + (uint64_t)(ks * a_kstep16), b_st + (uint64_t)(ks * (2048u >> 4)), idesc,
-                        (e > 0 || ks > 0) ? 1u : 0u);
-          ptx::tc_commit(&empty[st]);
-        }
-        __syncwarp();
-      }
-      if (ptx::elect_one()) ptx::tc_commit(&acc_full[buf]);
-      __syncwarp();
-    }
-  } else {
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;                   // rows 0..63 are the output block, 64..127 are scratch
-    uint16_t* cbase = reinterpret_cast<uint16_t*>(p.c);
-    const long long S = (long long)p.heads * p.head_state;
-    uint32_t n = 0;
-    for (long long it = blockIdx.x; it < total; it += gridDim.x, ++n) {
-      const int bh = (int)(it / p.n_out);
-      const int b = bh / p.heads, h = bh % p.heads;
-      const int hl = p.lut_heads > 1 ? h : 0;
-      const int o = p.order ? p.order[hl * p.n_out + (int)(it % p.n_out)] : (int)(it % p.n_out);
-      const int32_t* lut = p.lut + hl * p.lut_head_stride;
-      const int count = lut[2 * o + 1];
-      const uint32_t buf = n & 1;
-      ptx::mbar_wait(&acc_full[buf], (n >> 1) & 1, abort_flag);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (*abort_flag) { g_tc_error = 36; break; }
-      ptx::tc_fence_after();
-      if (quad < 2) {
-        uint16_t* out = cbase + ((long long)b * p.ctx_rows_c + o * 64 + row) * S + (long long)h * p.head_state;
-        for (int hh = 0; hh < p.head_state / 32; ++hh) {
-          uint32_t v[32];
-          if (count > 0) {
-            ptx::tmem_ld_x32(tmem + ((uint32_t)(quad * 32) << 16) + buf * 128 + hh * 32, v);
-            ptx::tmem_ld_wait();
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = 0u;       // output block with an empty LUT row
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float a = __uint_as_float(v[8 * i + 2 * e]), bq = __uint_as_float(v[8 * i + 2 * e + 1]);
-              if (BF16) { __nv_bfloat162 q = __floats2bfloat162_rn(a, bq); pk[e] = *reinterpret_cast<uint32_t*>(&q); }
-              else      { __half2 q = __floats2half2_rn(a, bq);           pk[e] = *reinterpret_cast<uint32_t*>(&q); }
-            }
-            reinterpret_cast<uint4*>(out + hh * 32)[i] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          }
-        }
-      }
-      ptx::tc_fence_before();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (warp == 2 && lane == 0) ptx::mbar_arrive(&acc_empty[buf]);
-    }
+    ptx::wg_commit();
+    ptx::wg_wait<1>();
+    __syncthreads();
+    if (tid == 0 && e >= 1 && e - 1 + ST < count) issue(e - 1 + ST);
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem, 256);
+  ptx::wg_wait<0>();
+  ptx::wg_fence_regs(acc[0]);
+  ptx::wg_fence_regs(acc[1]);
+
+  // epilogue (also zero-fills output blocks whose LUT row is empty)
+  const long long S = (long long)p.heads * p.head_state;
+  uint16_t* cbase = reinterpret_cast<uint16_t*>(p.c);
+  for (int c = 0; c < chunks; ++c)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = warp * 16 + lane / 4 + 8 * hh;
+      uint16_t* out = cbase + ((long long)b * p.ctx_rows_c + o * 64 + row) * S + (long long)h * p.head_state + c * 64;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int col = 8 * j + 2 * (lane % 4);
+        const float v0 = c ? acc[1][4 * j + 2 * hh] : acc[0][4 * j + 2 * hh];
+        const float v1 = c ? acc[1][4 * j + 2 * hh + 1] : acc[0][4 * j + 2 * hh + 1];
+        *reinterpret_cast<uint32_t*>(out + col) = pack2<BF16>(v0, v1);
+      }
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
-template <typename K>
-inline int bst_set_smem(K kern, size_t smem) {
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return fail((int)e, "cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
-  return 0;
-}
-
 inline bool bst_tc_applicable(int dtype, int bsize, int head_state, const void* a, const void* b, const void* c) {
   if (dtype != BSMM_F16 && dtype != BSMM_BF16) { fail(0, "fp32 runs on the FMA path"); return false; }
   if (bsize != 64) { fail(0, "block size %d uses the CUDA-core path", bsize); return false; }
   if (head_state != 64 && head_state != 128) { fail(0, "head_state %d uses the CUDA-core path", head_state); return false; }
   if (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) & 15) { fail(0, "pointers must be 16-byte aligned for TMA"); return false; }
-  const DeviceInfo& dev = device_info();
-  if (!dev.ok || dev.cc_major != 10) { fail(0, "tcgen05 needs an sm_100 device"); return false; }
-  static thread_local bool ctx_bound = false;
-  if (!ctx_bound) { cudaFree(nullptr); ctx_bound = true; }
-  return true;
+  return wgmma_device();
 }
 
-// items: device array built by the host layer (blocksparse_b200/lut.py:build_nt_items)
-inline int tc_bst_nt(int dtype, int c_dtype, int bsize, const int32_t* items, int n_items, int lut_heads, int blocks,
+inline int tc_bst_nt(int dtype, int c_dtype, int bsize, const int32_t* nt_lut, int lut_heads, int blocks,
                      const void* a, const void* b, void* c, int batch, int heads, int head_state, int ctx_blks_a,
                      int ctx_blks_b, cudaStream_t s) {
-  if (items == nullptr || n_items <= 0) { fail(0, "no NT item list supplied"); return TC_NOT_APPLICABLE; }
   if (!bst_tc_applicable(dtype, bsize, head_state, a, b, c)) return TC_NOT_APPLICABLE;
   const uint64_t S = (uint64_t)heads * head_state;
   BstNtTmaps maps;
   if (int e = cached_tmap_2d(&maps.a, dtype, a, S, (uint64_t)batch * ctx_blks_a * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   if (int e = cached_tmap_2d(&maps.b, dtype, b, S, (uint64_t)batch * ctx_blks_b * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   BstNtParams p;
-  p.items = items; p.n_items = n_items; p.lut_heads = lut_heads; p.batch = batch; p.heads = heads; p.blocks = blocks;
-  p.head_state = head_state; p.ctx_rows_a = ctx_blks_a * 64; p.ctx_rows_b = ctx_blks_b * 64; p.c = c;
-  const unsigned long long c_rows = (unsigned long long)batch * heads * blocks * 64;
-  p.tma_store = (c_dtype != BSMM_F32 && c_rows < (1ull << 31)) ? 1 : 0;
-  if (p.tma_store) { if (int e = cached_tmap_2d(&maps.c, c_dtype, c, 64, c_rows, 64, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e; }
-  else maps.c = maps.a;
-  const size_t smem = (size_t)BST_NT_STAGES * 3 * BST_TILE + 4 * BST_TILE;
-  const long long total = (long long)batch * heads * n_items;
-  const int sm = 2 * device_info().sm_grid;             // two CTAs per SM
-  const int grid = (int)(total < sm ? total : sm);
+  p.lut = nt_lut; p.lut_head_stride = lut_heads > 1 ? 2LL * blocks : 0;
+  p.heads = heads; p.blocks = blocks; p.head_state = head_state;
+  p.ctx_rows_a = ctx_blks_a * 64; p.ctx_rows_b = ctx_blks_b * 64; p.c = c;
+  const size_t smem = 4 * BST_TILE + SMEM_ALIGN_SLACK;
+  const unsigned grid = (unsigned)((long long)batch * heads * blocks);     // < 2^20: the output has < 2^32 elements
   const bool bf = dtype == BSMM_BF16;
 #define BSMM_LAUNCH_NT(BFV, TCV)                                                         \
   { auto kern = tc_bst_nt_kernel<BFV, TCV>;                                              \
@@ -423,13 +207,12 @@ inline int tc_bst_nt(int dtype, int c_dtype, int bsize, const int32_t* items, in
   else if (c_dtype == BSMM_BF16) { if (bf) BSMM_LAUNCH_NT(true, __nv_bfloat16) else BSMM_LAUNCH_NT(false, __nv_bfloat16) }
   else { if (bf) BSMM_LAUNCH_NT(true, __half) else BSMM_LAUNCH_NT(false, __half) }
 #undef BSMM_LAUNCH_NT
-  return check_launch("tcgen05_bst_nt");
+  return check_launch("wgmma_bst_nt");
 }
 
-inline int tc_bst_xn(int a_dtype, int dtype, int bsize, int transpose_a, const int32_t* lut, const int32_t* order, int lut_heads, int blocks,
-                     int max_lut, const void* a, const void* b, void* c, int batch, int heads, int head_state,
+inline int tc_bst_xn(int a_dtype, int dtype, int bsize, int transpose_a, const int32_t* lut, int lut_heads, int blocks,
+                     const void* a, const void* b, void* c, int batch, int heads, int head_state,
                      int ctx_blks_b, int ctx_blks_c, cudaStream_t s) {
-  (void)max_lut;
   if (a_dtype != dtype) { fail(0, "mixed sparse/dense dtypes use the CUDA-core path"); return TC_NOT_APPLICABLE; }
   if (!bst_tc_applicable(dtype, bsize, head_state, a, b, c)) return TC_NOT_APPLICABLE;
   if ((unsigned long long)batch * heads * blocks * 64 >= (1ull << 31)) { fail(0, "sparse tensor too large for one tensor map"); return TC_NOT_APPLICABLE; }
@@ -438,25 +221,21 @@ inline int tc_bst_xn(int a_dtype, int dtype, int bsize, int transpose_a, const i
   if (int e = cached_tmap_2d(&maps.a, dtype, a, 64, (uint64_t)batch * heads * blocks * 64, 64, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   if (int e = cached_tmap_2d(&maps.b, dtype, b, S, (uint64_t)batch * ctx_blks_b * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   BstXnParams p;
-  p.lut = lut; p.order = order; p.lut_head_stride = lut_heads > 1 ? 2LL * (ctx_blks_c + blocks) : 0; p.n_out = ctx_blks_c; p.lut_heads = lut_heads;
-  p.batch = batch; p.heads = heads; p.blocks = blocks; p.head_state = head_state;
-  p.ctx_rows_b = ctx_blks_b * 64; p.ctx_rows_c = ctx_blks_c * 64; p.transpose_a = transpose_a; p.c = c;
-  const size_t smem = (size_t)BST_STAGES * 3 * BST_TILE;
-  const long long total = (long long)batch * heads * ctx_blks_c;
-  const int sm = 2 * device_info().sm_grid;             // two CTAs per SM
-  const int grid = (int)(total < sm ? total : sm);
-  if (dtype == BSMM_BF16) {
-    auto kern = tc_bst_xn_kernel<true>;
-    static thread_local uint64_t cfg = 0;
-    if (int e = ensure_dyn_smem(kern, smem, cfg)) return e;
-    kern<<<grid, BST_THREADS, smem, s>>>(p, maps);
-  } else {
-    auto kern = tc_bst_xn_kernel<false>;
-    static thread_local uint64_t cfg = 0;
-    if (int e = ensure_dyn_smem(kern, smem, cfg)) return e;
-    kern<<<grid, BST_THREADS, smem, s>>>(p, maps);
-  }
-  return check_launch(transpose_a ? "tcgen05_bst_tn" : "tcgen05_bst_nn");
+  p.lut = lut; p.lut_head_stride = lut_heads > 1 ? 2LL * (ctx_blks_c + blocks) : 0; p.n_out = ctx_blks_c;
+  p.heads = heads; p.blocks = blocks; p.head_state = head_state;
+  p.ctx_rows_b = ctx_blks_b * 64; p.ctx_rows_c = ctx_blks_c * 64; p.c = c;
+  const size_t smem = (size_t)BST_STAGES * 3 * BST_TILE + SMEM_ALIGN_SLACK;
+  const unsigned grid = (unsigned)((long long)batch * heads * ctx_blks_c);
+#define BSMM_LAUNCH_XN(BFV, TRV)                                                         \
+  { auto kern = tc_bst_xn_kernel<BFV, TRV>;                                              \
+    static thread_local uint64_t cfg = 0;                                                \
+    if (int e = ensure_dyn_smem(kern, smem, cfg)) return e;                              \
+    kern<<<grid, BST_THREADS, smem, s>>>(p, maps); }
+  const bool bf = dtype == BSMM_BF16;
+  if (transpose_a) { if (bf) BSMM_LAUNCH_XN(true, true) else BSMM_LAUNCH_XN(false, true) }
+  else { if (bf) BSMM_LAUNCH_XN(true, false) else BSMM_LAUNCH_XN(false, false) }
+#undef BSMM_LAUNCH_XN
+  return check_launch(transpose_a ? "wgmma_bst_tn" : "wgmma_bst_nn");
 }
 
 }  // namespace bsmm

@@ -1,29 +1,24 @@
-// tcgen05 updat kernel: DW[w] = alpha * sum_p X_p[:, c-blk]^T . DY_p[:, k-blk]  (+ beta * DW[w])
-// for 16-bit dtypes, feature_axis = 1, block size 32 / 64.
+// wgmma updat kernel: DW[w] = alpha * sum_p X_p[:, c-blk]^T . DY_p[:, k-blk]  (+ beta * DW[w])
+// for 16-bit dtypes, both feature axes, block size 16 / 32 / 64.
 //   Replaces hgemm_blocksparse_64x64x64_tn_dds / 32x32x64_tn_dds
 //   (reference src/blocksparse_hgemm_nc_op_gpu.cu:553-897) and their Volta parameter-bank hack.
 //
 // Formulation ("gathered dense GEMM", schedule = blocksparse_b200/lut.py:build_updat_schedule):
-//   M axis   = 128 input features = a group of 128/bs consecutive input blocks      (A = X^T, MN-major)
-//   N axis   = the output blocks that have at least one active block in that group, COMPACTED side by
-//              side in shared memory and in tensor memory                             (B = DY, MN-major)
-//   K axis   = the minibatch (reduction), 64 rows per pipeline stage, 4 MMAs of K=16 per stage
-// so every K step is one wide tcgen05.mma (N = n_act*bs <= 256): no small-MMA issue bottleneck, output
-// blocks with nothing to update are neither loaded nor multiplied, and the reference's one-CTA-per-block
-// re-read of X and DY (nnz/CB times) becomes one pass per (group, window).  The epilogue writes only the
-// blocks that exist; a thread owns one row of a block, so stores are contiguous 64/128/256-byte rows.
-//
-// Warp roles (224 threads, 1 CTA / SM, persistent over tiles):
-//   warps 0,1   TMA producers (alternating stages): 2 activation boxes + n_act gradient boxes per stage
-//   warp 2      TMEM allocator + MMA issuer (accumulators double-buffered: 2 x 256 columns)
-//   warps 3..6  epilogue
+//   M axis   = 128 input features = a group of 128/bs consecutive input blocks; warpgroup g owns features 64g..64g+63
+//   N axis   = the output blocks that have at least one active block in that group, COMPACTED side by side in
+//              shared memory (n_act*bs <= 256 columns, multiplied in 64-column wgmma chunks: absent slots cost nothing)
+//   K axis   = the minibatch (reduction), 64 rows per pipeline stage, 4 wgmma K=16 steps per stage
+// Output blocks with nothing to update are neither loaded nor multiplied, and the reference's one-CTA-per-block
+// re-read of X and DY becomes one pass per (group, window).  The epilogue writes only the blocks that exist.
+//   axis 1: A = X[n][c] (MN-major, two 64-feature boxes), B = DY[n][k] (MN-major, one box per kept block).
+//   axis 0: A = X[c][n], B = DY[k][n]: both K-major with 128-byte rows; kept blocks continue the row index.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace bsmm {
 
-constexpr int UPDAT_THREADS = 7 * 32;
+constexpr int UPDAT_THREADS = 2 * 128;  // two warpgroups
 constexpr int UPDAT_STAGES = 4;
 constexpr int UPDAT_KCHUNK = 64;        // minibatch rows per stage
 // record layout of lut.py:build_updat_schedule: 64 ints for <= 8 slots per tile (bs 32 / 64), 192 for the 16 slots of bs 16
@@ -32,288 +27,193 @@ __host__ __device__ constexpr int updat_tab_off(int bs) { return bs >= 32 ? 16 :
 
 struct UpdatTcParams {
   const int32_t* sched;     // build_updat_schedule
-  int n_tiles;
-  int k_per_tile;           // KT: slots per tile (record stride for the block table)
   int N;                    // minibatch rows per pair
   int pcount;
-  int axis0;                // activations are (C, N): both operands K-major
   float alpha, beta;
   const float* gate;        // optional, only with gated
   int gated;
   void* dw;
-  int* counter;             // tile queue (csrc/tc.cuh): tiles are already sorted heaviest first by the schedule
 };
 struct UpdatTmaps { CUtensorMap x[BSMM_MAX_PAIRS]; CUtensorMap dy[BSMM_MAX_PAIRS]; };
 
-template <int BS, bool BF16, typename TO>
+template <int BS>
+constexpr size_t updat_smem_bytes() {
+  return (size_t)UPDAT_STAGES * (128 * UPDAT_KCHUNK * 2 + 256 * UPDAT_KCHUNK * 2) + SMEM_ALIGN_SLACK;
+}
+
+template <int BS, bool BF16, bool AXIS0, typename TO>
 __global__ void __launch_bounds__(UPDAT_THREADS, 1)
 tc_updat_kernel(const UpdatTcParams p, const __grid_constant__ UpdatTmaps maps) {
   constexpr int ST = UPDAT_STAGES;
-  constexpr int G = 128 / BS;                         // input blocks per group
-  constexpr int KT = 256 / BS;                        // max slots per tile
-  constexpr uint32_t ABYTES = 128 * UPDAT_KCHUNK * 2; // 16 KB: two 64-feature x 64-row boxes (SW128)
-  constexpr uint32_t BSLOT = BS * UPDAT_KCHUNK * 2;   // 4 KB (bs 32, SW64) / 8 KB (bs 64, SW128)
+  constexpr int KT = 256 / BS;                        // slots per tile
+  constexpr uint32_t ABYTES = 128 * UPDAT_KCHUNK * 2; // 16 KB
+  constexpr uint32_t BSLOT = BS * UPDAT_KCHUNK * 2;   // one kept output block
   constexpr uint32_t STAGE_BYTES = ABYTES + KT * BSLOT;
-  constexpr uint32_t B_SWZ = (BS == 16) ? ptx::SWZ_32B : (BS == 32) ? ptx::SWZ_64B : ptx::SWZ_128B;
-  constexpr uint32_t B_SBO = 8 * BS * 2;                    // 8 rows of BS*2 bytes
-  constexpr int REC = updat_rec_ints(BS), TAB = updat_tab_off(BS);   // record stride / offset of the W-id table (lut.py)
-  constexpr uint32_t B_KSTEP = 16 * BS * 2;                 // 16 minibatch rows
+  constexpr uint32_t B_ROW = BS * 2;                  // axis 1: bytes per row of a DY box
+  constexpr int REC = updat_rec_ints(BS), TAB = updat_tab_off(BS);
 
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t full[ST], empty[ST], acc_full[2], acc_empty[2];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ int abort_s;
-  __shared__ TileQueue tq;
-  volatile int* abort_flag = &abort_s;
-
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid / 32, 0), lane = tid % 32;   // provably warp-uniform role index
-  const int32_t* recs = p.sched + 4;
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ uint64_t full[ST];
+  __shared__ int rec[REC];
+  const uint32_t base = aligned_smem_base(smem_raw);
+  const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32, wg = warp / 4;
   const int chunks_per_pair = (p.N + UPDAT_KCHUNK - 1) / UPDAT_KCHUNK;
   const int n_chunks = chunks_per_pair * p.pcount;
 
+  for (int i = tid; i < REC; i += UPDAT_THREADS) rec[i] = p.sched[4 + (size_t)blockIdx.x * REC + i];
   if (tid == 0) {
-    abort_s = 0;
-    tile_queue_init(&tq, UPDAT_THREADS / 32);
-    for (int i = 0; i < ST; ++i) { ptx::mbar_init(&full[i], 1); ptx::mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&acc_full[i], 1); ptx::mbar_init(&acc_empty[i], 1); }
+    for (int i = 0; i < ST; ++i) ptx::mbar_init(&full[i], 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 2) { ptx::tmem_alloc(&tmem_base_s, 512); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
+  const int c0 = rec[0], n_act = rec[1];
+  const int nch = (n_act * BS + 63) / 64;             // 64-column wgmma chunks holding kept blocks
 
-  if (warp < 2) {
-    // ================================ TMA producers ================================
-    uint32_t sbase = 0;                     // stages of earlier tiles
-    bool alive = true;
-    const bool fetcher = warp == 0 && lane == 0;
-    int drawn = 0;
-    if (fetcher) tile_queue_publish(&tq, 0, (int)blockIdx.x, nullptr, p.n_tiles, abort_flag);
-    for (uint32_t tk = 0; alive; ++tk) {
-      const int t = tile_queue_next(&tq, tk, lane, abort_flag);
-      if (t < 0) break;
-      if (fetcher) drawn = tile_queue_draw(p.counter, tk + 1);
-      const int32_t* rec = recs + (size_t)t * REC;
-      const int c0 = rec[0], n_act = rec[1];
-      const int my_k = (lane >= 2 && lane < 2 + n_act) ? rec[8 + lane - 2] : 0;
-      int ch = (int)((2 + warp - (sbase % 2)) % 2);
-      for (; ch < n_chunks; ch += 2) {
-        const uint32_t sc = sbase + ch;
-        const uint32_t st = sc % ST;
-        if (!__all_sync(0xffffffffu, ptx::mbar_wait(&empty[st], ((sc / ST) & 1) ^ 1, abort_flag))) { g_tc_error = 11; alive = false; break; }
-        const int pair = ch / chunks_per_pair;
-        const int n0 = (ch % chunks_per_pair) * UPDAT_KCHUNK;
-        uint8_t* stage = smem + st * STAGE_BYTES;
-        if (lane == 0) ptx::mbar_expect_tx(&full[st], ABYTES + (uint32_t)n_act * BSLOT);
-        __syncwarp();
-        if (!p.axis0) {
-          if (lane < 2)
-            ptx::tma_load_2d(stage + lane * (ABYTES / 2), &maps.x[pair], &full[st], c0 * BS + lane * 64, n0);
-          else if (lane < 2 + n_act)
-            ptx::tma_load_2d(stage + ABYTES + (lane - 2) * BSLOT, &maps.dy[pair], &full[st], my_k * BS, n0);
-        } else {
-          if (lane == 0)           // [128 features][64 n], 128-byte rows
-            ptx::tma_load_2d(stage, &maps.x[pair], &full[st], n0, c0 * BS);
-          else if (lane >= 2 && lane < 2 + n_act)
-            ptx::tma_load_2d(stage + ABYTES + (lane - 2) * BSLOT, &maps.dy[pair], &full[st], n0, my_k * BS);
-        }
-        __syncwarp();
-      }
-      sbase += n_chunks;
-      if (fetcher && alive) tile_queue_publish(&tq, tk + 1, drawn, nullptr, p.n_tiles, abort_flag);
+  auto issue = [&](int ch) {                          // one thread: stage minibatch chunk ch
+    const uint32_t st = base + (uint32_t)(ch % ST) * STAGE_BYTES;
+    uint64_t* bar = &full[ch % ST];
+    const int pair = ch / chunks_per_pair;
+    const int n0 = (ch % chunks_per_pair) * UPDAT_KCHUNK;
+    ptx::mbar_expect_tx(bar, ABYTES + (uint32_t)n_act * BSLOT);
+    if (!AXIS0) {
+      ptx::tma_load_2d(st, &maps.x[pair], bar, c0 * BS, n0);
+      ptx::tma_load_2d(st + ABYTES / 2, &maps.x[pair], bar, c0 * BS + 64, n0);
+      for (int s = 0; s < n_act; ++s) ptx::tma_load_2d(st + ABYTES + s * BSLOT, &maps.dy[pair], bar, rec[8 + s] * BS, n0);
+    } else {                                          // [128 features][64 n], 128-byte rows
+      ptx::tma_load_2d(st, &maps.x[pair], bar, n0, c0 * BS);
+      for (int s = 0; s < n_act; ++s) ptx::tma_load_2d(st + ABYTES + s * BSLOT, &maps.dy[pair], bar, n0, rec[8 + s] * BS);
     }
-  } else if (warp == 2) {
-    // ================================ MMA issuer ================================
-    // axis 1: A = X[n][c] (MN-major, two 64-feature boxes), B = DY[n][k] (MN-major, one box per kept block).
-    // axis 0: A = X[c][n], B = DY[k][n]: both K-major with 128-byte rows; kept blocks continue the row index.
-    const uint64_t a_desc0 = p.axis0 ? ptx::make_smem_desc(ptx::smem_u32(smem), 16, 1024, ptx::SWZ_128B)
-                                     : ptx::make_smem_desc(ptx::smem_u32(smem), ABYTES / 2, 1024, ptx::SWZ_128B);
-    const uint64_t b_desc0 = p.axis0 ? ptx::make_smem_desc(ptx::smem_u32(smem) + ABYTES, 16, 1024, ptx::SWZ_128B)
-                                     : ptx::make_smem_desc(ptx::smem_u32(smem) + ABYTES, BSLOT, B_SBO, B_SWZ);
-    const uint32_t a_kstep16 = p.axis0 ? 2u : (2048u >> 4);
-    const uint32_t b_kstep16 = p.axis0 ? 2u : (B_KSTEP >> 4);
-    uint32_t sc = 0, tile_it = 0;
-    bool alive = true;
-    for (; alive; ++tile_it) {
-      const int t = tile_queue_next(&tq, tile_it, lane, abort_flag);
-      if (t < 0) break;
-      const int n_act = recs[(size_t)t * REC + 1];
-      const uint32_t buf = tile_it & 1;
-      const uint32_t idesc = ptx::make_idesc_f16(BF16, !p.axis0, !p.axis0, 128, n_act * BS);
-      if (!__all_sync(0xffffffffu, ptx::mbar_wait(&acc_empty[buf], ((tile_it >> 1) & 1) ^ 1, abort_flag))) { g_tc_error = 13; break; }
-      ptx::tc_fence_after();
-      const uint32_t d = tmem + buf * 256;
-      for (int ch = 0; ch < n_chunks; ++ch, ++sc) {
-        const uint32_t st = sc % ST;
-        if (!__all_sync(0xffffffffu, ptx::mbar_wait(&full[st], (sc / ST) & 1, abort_flag))) { g_tc_error = 14; alive = false; break; }
-        ptx::tc_fence_after();
-        if (ptx::elect_one()) {
-          const uint64_t a_st = a_desc0 + (uint64_t)((st * STAGE_BYTES) >> 4);
-          const uint64_t b_st = b_desc0 + (uint64_t)((st * STAGE_BYTES) >> 4);
+  };
+  if (tid == 0)
+    for (int ch = 0; ch < n_chunks && ch < ST; ++ch) issue(ch);
+
+  float acc[4][32];
 #pragma unroll
-          for (int ks = 0; ks < UPDAT_KCHUNK / 16; ++ks)
-            ptx::mma_ss(d, a_st + (uint64_t)(ks * a_kstep16), b_st + (uint64_t)(ks * b_kstep16), idesc,
-                        (ch > 0 || ks > 0) ? 1u : 0u);
-          ptx::tc_commit(&empty[st]);
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
+
+  for (int ch = 0; ch < n_chunks; ++ch) {
+    const uint32_t st = base + (uint32_t)(ch % ST) * STAGE_BYTES;
+    if (!ptx::mbar_wait(&full[ch % ST], (uint32_t)(ch / ST) & 1)) g_tc_error = 11;
+    ptx::wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < UPDAT_KCHUNK / 16; ++ks) {
+      const uint64_t adesc = AXIS0 ? ptx::make_desc(st + wg * (ABYTES / 2) + ks * 32, 16, 1024, ptx::SWZ_128B)
+                                   : ptx::make_desc(st + wg * (ABYTES / 2) + ks * 2048, ABYTES / 2, 1024, ptx::SWZ_128B);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        if (q < nch) {                                // uniform across the CTA
+          const uint32_t b0 = st + ABYTES + q * 8192;  // 64 columns = 64 rows of 128 bytes (axis 0) or 64/BS slots (axis 1)
+          const uint64_t bdesc = AXIS0 ? ptx::make_desc(b0 + ks * 32, 16, 1024, ptx::SWZ_128B)
+                                       : ptx::make_desc(b0 + ks * 16 * B_ROW, BSLOT, 8 * B_ROW, ptx::swz_for_row(B_ROW));
+          if (AXIS0) ptx::wgmma_n64<BF16, 0, 0>(acc[q], adesc, bdesc);
+          else       ptx::wgmma_n64<BF16, 1, 1>(acc[q], adesc, bdesc);
         }
-        __syncwarp();
       }
-      if (ptx::elect_one()) ptx::tc_commit(&acc_full[buf]);
-      __syncwarp();
     }
-  } else {
-    // ================================ epilogue ================================
-    const int quad = warp & 3;                          // TMEM lanes [32*quad, 32*quad+32)
-    const int blk_i = (quad * 32 + lane) / BS;          // input block of the group this lane's feature row belongs to
-    const int row = (quad * 32 + lane) % BS;            // row inside the BS x BS block
-    constexpr int CW = BS < 32 ? BS : 32, NH = BS / CW; // columns per tcgen05.ld
-    TO* dw = reinterpret_cast<TO*>(p.dw);
-    uint32_t tile_it = 0;
-    for (;; ++tile_it) {
-      const int t = tile_queue_next(&tq, tile_it, lane, abort_flag);
-      if (t < 0) break;
-      const int32_t* rec = recs + (size_t)t * REC;
-      const int n_act = rec[1];
-      const uint32_t buf = tile_it & 1;
-      ptx::mbar_wait(&acc_full[buf], (tile_it >> 1) & 1, abort_flag);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (*abort_flag) { g_tc_error = 16; break; }
-      ptx::tc_fence_after();
-      for (int s = 0; s < n_act; ++s) {
-        const int w = rec[TAB + blk_i * p.k_per_tile + s];       // warp-uniform for bs >= 32; two blocks per warp for bs 16
-        if (!__any_sync(0xffffffffu, w >= 0)) continue;          // tcgen05.ld is warp-collective: skip only when no lane stores
+    ptx::wg_commit();
+    ptx::wg_wait<1>();
+    __syncthreads();
+    if (tid == 0 && ch >= 1 && ch - 1 + ST < n_chunks) issue(ch - 1 + ST);
+  }
+  ptx::wg_wait<0>();
+#pragma unroll
+  for (int q = 0; q < 4; ++q) ptx::wg_fence_regs(acc[q]);
+
+  // epilogue: accumulator (feature row r of the group, column c) -> DW[w][r % BS][c % BS], w from the record's table
+  TO* dw = reinterpret_cast<TO*>(p.dw);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    if (q >= nch) continue;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int col = q * 64 + 8 * j + 2 * (lane % 4);
+      const int s = col / BS, jj = col % BS;
+      if (s >= n_act) continue;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = wg * 64 + (warp % 4) * 16 + lane / 4 + 8 * h;
+        const int w = rec[TAB + (r / BS) * KT + s];
+        if (w < 0) continue;
         float g = p.alpha;
-        if (p.gated && w >= 0) g *= p.gate[w];
-        TO* out = dw + ((size_t)(w >= 0 ? w : 0) * BS + row) * BS;
-#pragma unroll
-        for (int h = 0; h < NH; ++h) {
-          uint32_t v[32];
-          if constexpr (CW == 32) ptx::tmem_ld_x32(tmem + ((uint32_t)(quad * 32) << 16) + buf * 256 + (uint32_t)(s * BS + h * 32), v);
-          else { uint32_t t16[16]; ptx::tmem_ld_x16(tmem + ((uint32_t)(quad * 32) << 16) + buf * 256 + (uint32_t)(s * BS), t16);
-#pragma unroll
-                 for (int i = 0; i < 16; ++i) v[i] = t16[i]; }
-          ptx::tmem_ld_wait();
-          if (w < 0) continue;
-          float f[32];
-#pragma unroll
-          for (int i = 0; i < CW; ++i) f[i] = __uint_as_float(v[i]) * g;
-          if (sizeof(TO) == 4) {
-            float4* o4 = reinterpret_cast<float4*>(out + h * 32);
-#pragma unroll
-            for (int i = 0; i < CW / 4; ++i) {
-              float4 q = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-              if (p.beta != 0.f) { const float4 o = o4[i]; q.x += o.x; q.y += o.y; q.z += o.z; q.w += o.w; }
-              o4[i] = q;
-            }
-          } else {
-            uint4* o4 = reinterpret_cast<uint4*>(out + h * 32);
-#pragma unroll
-            for (int i = 0; i < CW / 8; ++i) {
-              uint32_t pk[4];
-              uint4 old = make_uint4(0, 0, 0, 0);
-              if (p.beta != 0.f) old = o4[i];
-              const uint32_t oldw[4] = {old.x, old.y, old.z, old.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float a = f[8 * i + 2 * e], b = f[8 * i + 2 * e + 1];
-                if (BF16) {
-                  if (p.beta != 0.f) {
-                    const __nv_bfloat162 o = *reinterpret_cast<const __nv_bfloat162*>(&oldw[e]);
-                    a += __bfloat162float(o.x); b += __bfloat162float(o.y);
-                  }
-                  __nv_bfloat162 q = __floats2bfloat162_rn(a, b); pk[e] = *reinterpret_cast<uint32_t*>(&q);
-                } else {
-                  if (p.beta != 0.f) {
-                    const __half2 o = *reinterpret_cast<const __half2*>(&oldw[e]);
-                    a += __half2float(o.x); b += __half2float(o.y);
-                  }
-                  __half2 q = __floats2half2_rn(a, b); pk[e] = *reinterpret_cast<uint32_t*>(&q);
-                }
-              }
-              o4[i] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            }
+        if (p.gated) g *= p.gate[w];
+        float a = acc[q][4 * j + 2 * h] * g, b = acc[q][4 * j + 2 * h + 1] * g;
+        TO* out = dw + ((size_t)w * BS + r % BS) * BS + jj;
+        if constexpr (sizeof(TO) == 4) {
+          float2* o2 = reinterpret_cast<float2*>(out);
+          if (p.beta != 0.f) { const float2 old = *o2; a += old.x; b += old.y; }
+          *o2 = make_float2(a, b);
+        } else {
+          uint32_t* o2 = reinterpret_cast<uint32_t*>(out);
+          if (p.beta != 0.f) {
+            const uint32_t old = *o2;
+            if constexpr (BF16) { const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&old); a += __bfloat162float(v.x); b += __bfloat162float(v.y); }
+            else                { const __half2 v = *reinterpret_cast<const __half2*>(&old);        a += __half2float(v.x);     b += __half2float(v.y); }
           }
+          *o2 = pack2<BF16>(a, b);
         }
       }
-      ptx::tc_fence_before();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (warp == 3 && lane == 0) ptx::mbar_arrive(&acc_empty[buf]);
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) ptx::tmem_dealloc(tmem, 512);
-  if (tid == 0 && p.counter) tile_queue_retire(p.counter);
 }
 
-template <int BS>
-constexpr size_t updat_smem_bytes() {
-  return (size_t)UPDAT_STAGES * (128 * UPDAT_KCHUNK * 2 + (256 / BS) * BS * UPDAT_KCHUNK * 2);
-}
-
-template <int BS, bool BF16, typename TO>
-int launch_tc_updat(const UpdatTcParams& p, const UpdatTmaps& maps, int sm_count, cudaStream_t s) {
-  auto kern = tc_updat_kernel<BS, BF16, TO>;
+template <int BS, bool BF16, bool AXIS0, typename TO>
+int launch_tc_updat(const UpdatTcParams& p, const UpdatTmaps& maps, int n_tiles, cudaStream_t s) {
+  auto kern = tc_updat_kernel<BS, BF16, AXIS0, TO>;
   constexpr size_t smem = updat_smem_bytes<BS>();
   static thread_local uint64_t configured = 0;
   if (int e = ensure_dyn_smem(kern, smem, configured)) return e;
-  const int grid = p.n_tiles < sm_count ? p.n_tiles : sm_count;
-  kern<<<grid, UPDAT_THREADS, smem, s>>>(p, maps);
-  return check_launch(BS == 16 ? "tcgen05_updat_bs16" : BS == 32 ? "tcgen05_updat_bs32" : "tcgen05_updat_bs64");
+  kern<<<n_tiles, UPDAT_THREADS, smem, s>>>(p, maps);
+  return check_launch(BS == 16 ? "wgmma_updat_bs16" : BS == 32 ? "wgmma_updat_bs32" : "wgmma_updat_bs64");
 }
 
-inline int tc_updat(int dtype, int dw_dtype, int axis, int bsize, const int32_t* updat_lut, int blocks, int n_c_blocks,
-                    int n_k_blocks, const void* const* xs, const void* const* dys, int pcount, void* dw, int N, float alpha,
+template <int BS, bool BF16, typename TO>
+int dispatch_tc_updat(const UpdatTcParams& p, const UpdatTmaps& maps, int n_tiles, bool axis0, cudaStream_t s) {
+  return axis0 ? launch_tc_updat<BS, BF16, true, TO>(p, maps, n_tiles, s) : launch_tc_updat<BS, BF16, false, TO>(p, maps, n_tiles, s);
+}
+
+inline int tc_updat(int dtype, int dw_dtype, int axis, int bsize, int n_c_blocks, int n_k_blocks,
+                    const void* const* xs, const void* const* dys, int pcount, void* dw, int N, float alpha,
                     float beta, const float* gate, int gated_dw, const int32_t* sched, int sched_tiles, int sched_tile_blocks,
-                    int sched_groups_off, cudaStream_t s) {
-  (void)updat_lut; (void)blocks; (void)sched_groups_off;
+                    cudaStream_t s) {
   if (dtype != BSMM_F16 && dtype != BSMM_BF16) { fail(0, "fp32 runs on the FMA path"); return TC_NOT_APPLICABLE; }
   if (axis == 0 && (N & 7)) { fail(0, "feature_axis 0 needs N %% 8 == 0 for TMA"); return TC_NOT_APPLICABLE; }
   if (bsize != 16 && bsize != 32 && bsize != 64) { fail(0, "block size %d uses the CUDA-core path", bsize); return TC_NOT_APPLICABLE; }
   if (sched == nullptr || sched_tiles <= 0) { fail(0, "no updat schedule supplied"); return TC_NOT_APPLICABLE; }
   if (sched_tile_blocks != 256 / bsize) return fail(BSMM_E_ARG, "bsmm_updat: schedule built for %d slots per tile, kernel needs %d", sched_tile_blocks, 256 / bsize);
   if (N <= 0) return TC_NOT_APPLICABLE;
-  const DeviceInfo& dev = device_info();
-  if (!dev.ok || dev.cc_major != 10) { fail(0, "tcgen05 needs an sm_100 device"); return TC_NOT_APPLICABLE; }
   if ((uintptr_t)dw & 15) { fail(0, "dw must be 16-byte aligned"); return TC_NOT_APPLICABLE; }
   for (int i = 0; i < pcount; ++i)
     if (((uintptr_t)xs[i] | (uintptr_t)dys[i]) & 15) { fail(0, "pointers must be 16-byte aligned for TMA"); return TC_NOT_APPLICABLE; }
-  static thread_local bool ctx_bound = false;
-  if (!ctx_bound) { cudaFree(nullptr); ctx_bound = true; }
+  if (!wgmma_device()) return TC_NOT_APPLICABLE;
 
   const uint64_t C = (uint64_t)n_c_blocks * bsize, K = (uint64_t)n_k_blocks * bsize;
   UpdatTmaps maps;
   memset(&maps, 0, sizeof(maps));
-  const CUtensorMapSwizzle bswz = bsize == 16 ? CU_TENSOR_MAP_SWIZZLE_32B : bsize == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
   for (int i = 0; i < pcount; ++i) {
     if (axis == 1) {
       if (int e = cached_tmap_2d(&maps.x[i], dtype, xs[i], C, (uint64_t)N, C, 64, UPDAT_KCHUNK, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
-      if (int e = cached_tmap_2d(&maps.dy[i], dtype, dys[i], K, (uint64_t)N, K, bsize, UPDAT_KCHUNK, bswz)) return e;
+      if (int e = cached_tmap_2d(&maps.dy[i], dtype, dys[i], K, (uint64_t)N, K, bsize, UPDAT_KCHUNK, tmap_swizzle_for_row(bsize * 2))) return e;
     } else {       // (features, N): inner dim = minibatch, 64 columns = 128-byte rows
       if (int e = cached_tmap_2d(&maps.x[i], dtype, xs[i], (uint64_t)N, C, (uint64_t)N, UPDAT_KCHUNK, 128, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
       if (int e = cached_tmap_2d(&maps.dy[i], dtype, dys[i], (uint64_t)N, K, (uint64_t)N, UPDAT_KCHUNK, bsize, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
     }
   }
   UpdatTcParams p;
-  p.axis0 = axis == 0;
-  p.sched = sched; p.n_tiles = sched_tiles; p.k_per_tile = sched_tile_blocks; p.N = N; p.pcount = pcount;
+  p.sched = sched; p.N = N; p.pcount = pcount;
   p.alpha = alpha; p.beta = beta; p.gate = gate; p.gated = (gated_dw && gate) ? 1 : 0; p.dw = dw;
-  p.counter = static_tiles() ? nullptr : next_tile_counter();
-  if (!p.counter && !static_tiles()) return fail(BSMM_E_NODEV, "bsmm_updat: tile counters not available");
-  const bool bf = dtype == BSMM_BF16;
+  const bool bf = dtype == BSMM_BF16, a0 = axis == 0;
   const bool f32out = dw_dtype == BSMM_F32;
-  if (bsize == 16) {
-    if (f32out) return bf ? launch_tc_updat<16, true, float>(p, maps, dev.sm_grid, s) : launch_tc_updat<16, false, float>(p, maps, dev.sm_grid, s);
-    return bf ? launch_tc_updat<16, true, __nv_bfloat16>(p, maps, dev.sm_grid, s) : launch_tc_updat<16, false, __half>(p, maps, dev.sm_grid, s);
-  }
-  if (bsize == 32) {
-    if (f32out) return bf ? launch_tc_updat<32, true, float>(p, maps, dev.sm_grid, s) : launch_tc_updat<32, false, float>(p, maps, dev.sm_grid, s);
-    return bf ? launch_tc_updat<32, true, __nv_bfloat16>(p, maps, dev.sm_grid, s) : launch_tc_updat<32, false, __half>(p, maps, dev.sm_grid, s);
-  }
-  if (f32out) return bf ? launch_tc_updat<64, true, float>(p, maps, dev.sm_grid, s) : launch_tc_updat<64, false, float>(p, maps, dev.sm_grid, s);
-  return bf ? launch_tc_updat<64, true, __nv_bfloat16>(p, maps, dev.sm_grid, s) : launch_tc_updat<64, false, __half>(p, maps, dev.sm_grid, s);
+#define BSMM_UPDAT_BS(BSV)                                                                                            \
+  if (f32out) return bf ? dispatch_tc_updat<BSV, true, float>(p, maps, sched_tiles, a0, s)                            \
+                        : dispatch_tc_updat<BSV, false, float>(p, maps, sched_tiles, a0, s);                          \
+  return bf ? dispatch_tc_updat<BSV, true, __nv_bfloat16>(p, maps, sched_tiles, a0, s)                                \
+            : dispatch_tc_updat<BSV, false, __half>(p, maps, sched_tiles, a0, s);
+  if (bsize == 16) { BSMM_UPDAT_BS(16) }
+  if (bsize == 32) { BSMM_UPDAT_BS(32) }
+  BSMM_UPDAT_BS(64)
+#undef BSMM_UPDAT_BS
 }
 
 }  // namespace bsmm

@@ -1,439 +1,181 @@
-// tcgen05 xprop, second generation: block-sparse fprop / bprop for 16-bit dtypes and 32 x 32 blocks, both feature axes.
+// wgmma xprop over WIDE output tiles: block-sparse fprop / bprop for 16-bit dtypes and 32 x 32 blocks, both feature axes.
 //   Replaces hgemm_blocksparse_64x32x32_nx_dsd (reference src/blocksparse_hgemm_nc_op_gpu.cu:38-551) and the
 //   feature-axis-0 family hgemm_blocksparse_xn_64_sdd (src/blocksparse_hgemm_cn_64_op_gpu.cu:9-717).
 //
-// What changed against csrc/tc.cuh (which stays for 64 x 64 blocks and dense layouts), and why:
-//   * The round-1 kernel was bound by the SM's L1 -> crossbar REQUEST port, not by bytes: the port issues one request
-//     per cycle, a TMA box row is one request, and the 128 x 32 activation tile has 64-byte rows.  ncu showed the port
-//     67 % busy at 2.2 sectors per request (45 B/clk/SM, profiles/r1_ncu_tc_kernels.txt).  Here a schedule GROUP is
-//     an input-block PAIR: the activation tile is 128 rows x 64 features = 128-byte rows (SWIZZLE_128B), half the
-//     requests per byte, and about twice the W blocks consume each staged tile (half the groups, barriers and turns).
-//   * Tiles are handed to CTAs through a host-built list (longest-processing-time assignment, lut.py:lpt_tile_lists)
-//     instead of tile t -> CTA t mod grid: skewed layouts no longer leave CTAs idle, results stay deterministic.
-//   * The tile width / CTAs per SM, W slots per stage, ring depth, pipelines and epilogue warps are template
-//     parameters (Xp2Cfg); the variants that are instantiated are listed at the bottom.
-//
-// Formulation (unchanged): minibatch on the MMA M axis (128 rows per tile), a W block is a B operand (N = K = 32),
-// the tile's <= TB output blocks own side-by-side fp32 accumulators in tensor memory.  Within a group the runs of
-// half 0 (input block 2p: K slices 0,1 of the tile) are issued first, then those of half 1 (K slices 2,3); the first
-// MMA of every K slice fills the A collector, the rest reuse it.
-//
-// Warp roles ((2*NP + EW) warps, persistent over the CTA's tile list):
-//   warps 0..NP-1     TMA producers (one per pipeline): activation tile + the group's W blocks -> one mbarrier;
-//                     lanes 16..31 expand the packed runs of the record into ready-to-issue MMA commands
-//   warps NP..2NP-1   MMA issuers, taking turns in group order (deterministic accumulation order)
-//   last EW warps     epilogue: tcgen05.ld -> 16-bit -> swizzled smem -> TMA store, accumulators left zeroed
+// What differs from csrc/tc.cuh (one output block per CTA): a CTA owns TB = 2 or 4 consecutive output blocks and walks
+// the MERGED LUT rows of the tile (lut.py:build_wide_schedule): one entry per input block that any of them consumes,
+// carrying the TB W blocks (absent ones are read from beyond the end of the weight tensor, which TMA fills with zeros).
+// Each activation tile is therefore staged once for up to TB output blocks instead of once per block, and every K=16
+// step is one MMA of N = TB*32 instead of TB MMAs of N = 32.  The price is multiplying the zero blocks of the tile.
+// Opt-in (BlocksparseMatMul, BSMM_XPROP2=1..3); variants (blocks per tile, m64 row groups per CTA):
+//   1 = (2, 1)  64 minibatch rows per CTA: more CTAs for small minibatches
+//   2 = (2, 2)  128 rows
+//   3 = (4, 2)  128 rows, 128 output features
+// Accumulation order is the merged entry order (ascending input block), so results are deterministic.
 #pragma once
 #include "tc.cuh"
 
 namespace bsmm {
 
-template <int TB_, int OCC_, int WPS_, int XS_, int NP_, int STG_, int EW_>
-struct Xp2Cfg {
-  static constexpr int TB = TB_, OCC = OCC_, WPS = WPS_, XS = XS_, NP = NP_, STG = STG_, EW = EW_;
-  static constexpr int TCOLS = TB_ * 32 <= 256 ? 256 : 512;
-  static constexpr int THREADS = (2 * NP_ + EW_) * 32;
-  static constexpr uint32_t XBYTES = 128 * 64 * 2, WBYTES = 32 * 32 * 2, OBYTES = 128 * 32 * 2;
-  static constexpr uint32_t STAGE_BYTES = XBYTES + WPS_ * WBYTES;
-  static constexpr size_t SMEM = (size_t)XS_ * STAGE_BYTES + (size_t)STG_ * OBYTES;
-  static_assert(XS_ % NP_ == 0, "stages are split evenly between the pipelines");
-  static_assert(EW_ == 4 || EW_ == 8, "4 or 8 epilogue warps");
-  static_assert(STG_ % (EW_ / 4) == 0, "staging buffers are split between the epilogue warp groups");
-  static_assert(WPS_ <= 14, "group records hold 14 W blocks");
+template <int TB, int MI> struct Xp2Shape {
+  static constexpr uint32_t XBYTES = MI * 64 * 32 * 2;                    // MI*64 minibatch rows x 32 features
+  static constexpr uint32_t WBYTES = 32 * 32 * 2;
+  static constexpr uint32_t STAGE = (XBYTES + TB * WBYTES + 1023) / 1024 * 1024;
+  static constexpr size_t SMEM = XP_STAGES * STAGE + SMEM_ALIGN_SLACK;
 };
+constexpr int XP2_REC = 8;           // ints per merged entry: (input block, W block of output 0..3 or -1, pad)
 
 struct Xprop2Params {
-  const int32_t* sched;      // lut.py:build_pair_schedule
-  int groups_off;            // int32 index of the first group record
-  int list_off;              // int32 index of the per-CTA tile lists
-  int n_ktiles;              // output tiles along the feature axis
-  int bprop;
-  int axis0;                 // activations are (C, N): A operand is MN-major, output stored transposed
+  const int32_t* tile_off;   // [n_tiles + 1] first merged entry of every tile
+  const int32_t* ent;        // [entries][XP2_REC]
+  int n_out;
+  int w_absent;              // W block index whose TMA box lies wholly out of bounds (= number of blocks): zeros
   void* y;
   long long y_pitch;         // elements
   int N;
-  unsigned long long* trace; // tuning aid (BSMM_TRACE): CTA 0 records clock64 at 5 pipeline events of its first 256 groups
-  int ablate;                // tuning aid (BSMM_ABLATE): 1 no MMAs, 2 no TMA loads, 4 no epilogue work, 8 no W loads, 16 no X loads
 };
 
-template <class Cfg, bool BF16>
-__global__ void __launch_bounds__(Cfg::THREADS, Cfg::OCC)
+template <int TB, int MI, bool BF16, bool AXIS0, bool BPROP>
+__global__ void __launch_bounds__(XP_THREADS)
 tc_xprop2_kernel(const Xprop2Params p, const __grid_constant__ XpropTmaps maps) {
-  constexpr int XS = Cfg::XS, WPS = Cfg::WPS, STG = Cfg::STG, NP = Cfg::NP, EW = Cfg::EW;
-  constexpr uint32_t HS = XS / NP;                 // stages per pipeline
-  constexpr uint32_t XBYTES = Cfg::XBYTES, WBYTES = Cfg::WBYTES, OBYTES = Cfg::OBYTES, STAGE_BYTES = Cfg::STAGE_BYTES;
-  constexpr int BS = 32;
+  using Sh = Xp2Shape<TB, MI>;
+  constexpr int ST = XP_STAGES, NW = TB * 32;
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ uint64_t full[ST];
+  const uint32_t base = aligned_smem_base(smem_raw);
+  const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
+  const int nt = blockIdx.x, t = blockIdx.y;
+  const int first = p.tile_off[t], count = p.tile_off[t + 1] - first;
+  const int32_t* ent = p.ent + (size_t)first * XP2_REC;
 
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sStage = smem;                          // XS x (activation tile | WPS W blocks)
-  uint8_t* sO = smem + XS * STAGE_BYTES;           // STG x output-block staging
-  __shared__ uint64_t full[XS], empty[XS], acc_full, acc_empty, turn[NP];
-  __shared__ __align__(16) int2 cmd[XS][16];       // per run: (B descriptor low word, accumulator column | N/8 << 12 | run count << 20)
-  __shared__ uint32_t tmem_base_s;
-  __shared__ int abort_s;
-  volatile int* abort_flag = &abort_s;
-
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid / 32, 0), lane = tid % 32;   // provably warp-uniform role index
-  const int32_t* sched = p.sched;
-  const int32_t* tlist = sched + p.list_off;
-  const int li0 = tlist[blockIdx.x], li1 = tlist[blockIdx.x + 1];
-  const int32_t* tiles = tlist + gridDim.x + 1;
+  auto issue = [&](int e) {                                // one thread: stage merged entry e
+    const int32_t* r = ent + e * XP2_REC;
+    const uint32_t st = base + (uint32_t)(e % ST) * Sh::STAGE;
+    uint64_t* bar = &full[e % ST];
+    ptx::mbar_expect_tx(bar, Sh::XBYTES + TB * Sh::WBYTES);
+    if (!AXIS0) {
+      ptx::tma_load_2d(st, &maps.x, bar, r[0] * 32, nt * MI * 64);                       // [MI*64 n][32 c]
+    } else {
+#pragma unroll
+      for (int m = 0; m < MI; ++m) ptx::tma_load_2d(st + m * 4096, &maps.x, bar, nt * MI * 64 + m * 64, r[0] * 32);
+    }
+#pragma unroll
+    for (int j = 0; j < TB; ++j) {
+      const int wb = r[1 + j];
+      ptx::tma_load_2d(st + Sh::XBYTES + j * Sh::WBYTES, &maps.w, bar, 0, (wb < 0 ? p.w_absent : wb) * 32);
+    }
+  };
 
   if (tid == 0) {
-    abort_s = 0;
-    for (int i = 0; i < XS; ++i) { ptx::mbar_init(&full[i], 1); ptx::mbar_init(&empty[i], 1); }
-    ptx::mbar_init(&acc_full, NP);
-    ptx::mbar_init(&acc_empty, 1);
-    for (int i = 0; i < NP; ++i) ptx::mbar_init(&turn[i], 1);
+    for (int i = 0; i < ST; ++i) ptx::mbar_init(&full[i], 1);
     ptx::fence_mbar_init();
-    ptx::prefetch_tensormap(&maps.x); ptx::prefetch_tensormap(&maps.w); ptx::prefetch_tensormap(&maps.y);
+    ptx::prefetch_tensormap(&maps.x); ptx::prefetch_tensormap(&maps.w);
   }
-  if (warp == NP) { ptx::tmem_alloc(&tmem_base_s, Cfg::TCOLS); ptx::tmem_relinquish(); }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
+  if (tid == 0)
+    for (int e = 0; e < count && e < ST; ++e) issue(e);
 
-  if (warp < NP) {
-    // ================================ TMA producers ================================
-    uint32_t gbase = 0;                   // groups of earlier tiles
-    bool alive = true;
-    const uint32_t full0 = ptx::opaque(ptx::smem_u32(&full[0])), empty0 = ptx::opaque(ptx::smem_u32(&empty[0])),
-                   cmd0 = ptx::opaque(ptx::smem_u32(&cmd[0][0])), stage0 = ptx::opaque(ptx::smem_u32(sStage));
-    // fprop: B = W[c][k] read as K x N, N contiguous (MN-major), next 32-column block = next slot (LBO = WBYTES)
-    // bprop: B = W[c][k] read as N x K, K contiguous (K-major), rows simply continue into the next slot
-    const uint32_t p_bdesc_lo = (uint32_t)ptx::make_smem_desc(ptx::smem_u32(sStage) + XBYTES, p.bprop ? 16u : WBYTES, 512, ptx::SWZ_64B);
-    for (int li = li0; li < li1 && alive; ++li) {
-      const int t = tiles[li];
-      const int nt = t / p.n_ktiles, kt = t - nt * p.n_ktiles;
-      const int32_t* th = sched + 4 + 4 * kt;
-      const int first_group = th[0], n_groups = th[1];
-      const int32_t* grec = sched + p.groups_off + (size_t)first_group * 32;
-      int g = (int)((NP + warp - (gbase % NP)) % NP);       // first group of this tile owned by this pipeline
-      int rec = (g < n_groups) ? grec[g * 32 + lane] : 0;
-      for (; g < n_groups; g += NP) {
-        const int cur = rec;
-        const int gn = g + NP;
-        if (gn < n_groups) rec = grec[gn * 32 + lane];      // prefetch the next record
-        const uint32_t gc = gbase + g;
-        const uint32_t pj = gc / NP;                         // running group count of this pipeline
-        const uint32_t st = (uint32_t)warp + NP * (pj % HS);
-        const int in_pair = __shfl_sync(0xffffffffu, cur, 0);
-        const int counts = __shfl_sync(0xffffffffu, cur, 1);
-        const int n_w = counts & 0xff, nr0 = (counts >> 8) & 0xff, nr1 = (counts >> 16) & 0xff;
-        if (!__all_sync(0xffffffffu, ptx::mbar_wait_a(empty0 + st * 8, ((pj / HS) & 1) ^ 1, abort_flag))) { g_tc_error = 1; alive = false; break; }
-        if (p.trace && blockIdx.x == 0 && lane == 0 && gc < 256) p.trace[gc * 8 + 0] = clock64();
-        if (lane >= 16) {
-          const int r = lane - 16;                           // 0..7 half 0, 8..15 half 1
-          const int nr = r < 8 ? nr0 : nr1;
-          if ((r & 7) < nr || (r & 7) == 0) {
-            const uint32_t pk = (uint32_t)cur;
-            asm volatile("st.shared.v2.s32 [%0], {%1, %2};" ::"r"(cmd0 + st * (16 * 8) + r * 8),
-                         "r"((int)(p_bdesc_lo + ((st * STAGE_BYTES) >> 4) + (pk & 0xfffu))),
-                         "r"((int)(((pk >> 12) & 0x1ffu) | (((pk >> 21) & 0x3fu) << 12) | ((uint32_t)nr << 20))) : "memory");
-          }
-        }
-        __syncwarp();
-        const uint32_t stage = stage0 + st * STAGE_BYTES, fbar = full0 + st * 8;
-        if (p.ablate & 26) {                       // timing ablations: drop some or all loads (results are garbage)
-          const bool no_x = p.ablate & (2 | 16), no_w = p.ablate & (2 | 8);
-          if (lane == 0) {
-            ptx::mbar_expect_tx_a(fbar, (no_x ? 0u : XBYTES) + (no_w ? 0u : (uint32_t)n_w * WBYTES));
-            if (!no_x) ptx::tma_load_2d_a(stage, &maps.x, fbar, in_pair * 64, nt * 128);
-          }
-          if (!no_w && lane >= 2 && lane < 2 + n_w)
-            ptx::tma_load_2d_a(stage + XBYTES + (lane - 2) * WBYTES, &maps.w, fbar, 0, cur * BS);
-          __syncwarp();
-          if (p.trace && blockIdx.x == 0 && lane == 0 && gc < 256) p.trace[gc * 8 + 1] = clock64();
-          continue;
-        }
-        if (lane == 0) {
-          ptx::mbar_expect_tx_a(fbar, XBYTES + (uint32_t)n_w * WBYTES);
-          if (!p.axis0) {
-            ptx::tma_load_2d_a(stage, &maps.x, fbar, in_pair * 64, nt * 128);            // [128 n][64 c], K-major A, 128-byte rows
-          } else {                                                                      // [64 c][128 n] as two 64-column boxes, MN-major A
-            ptx::tma_load_2d_a(stage, &maps.x, fbar, nt * 128, in_pair * 64);
-            ptx::tma_load_2d_a(stage + XBYTES / 2, &maps.x, fbar, nt * 128 + 64, in_pair * 64);
-          }
-        }
-        if (lane >= 2 && lane < 2 + n_w)
-          ptx::tma_load_2d_a(stage + XBYTES + (lane - 2) * WBYTES, &maps.w, fbar, 0, cur * BS);
-        __syncwarp();
-        if (p.trace && blockIdx.x == 0 && lane == 0 && gc < 256) p.trace[gc * 8 + 1] = clock64();
-      }
-      gbase += n_groups;
-    }
-  } else if (warp < 2 * NP) {
-    // ================================ MMA issuers ================================
-    const uint32_t iw = (uint32_t)(warp - NP);
-    const uint32_t b_kstep16 = (p.bprop ? 32u : 16u * 64u) >> 4;       // K=16 slice of a W block: 32 B along the row / 16 rows
-    // axis 1: A = X[n][c] tile, K-major SW128 (128-byte rows, 8-row groups 1 KB apart), K=16 slice = +32 B.
-    // axis 0: A = X[c][n] tile, MN-major SW128: two [64 x 64] boxes (LBO = box), K=16 slice = 16 rows = 2 KB.
-    const uint64_t a_desc0 = p.axis0 ? ptx::make_smem_desc(ptx::smem_u32(sStage), XBYTES / 2, 1024, ptx::SWZ_128B)
-                                     : ptx::make_smem_desc(ptx::smem_u32(sStage), 16, 1024, ptx::SWZ_128B);
-    const uint32_t a_kstep16 = p.axis0 ? (16u * 128u) >> 4 : 2u;
-    const uint32_t b_desc_hi = (uint32_t)(ptx::make_smem_desc(0, 16, 512, ptx::SWZ_64B) >> 32);
-    const uint32_t idesc0 = ptx::make_idesc_f16(BF16, p.axis0 != 0, !p.bprop, 128, 0);
-    const uint32_t full0 = ptx::opaque(ptx::smem_u32(&full[0])), empty0 = ptx::opaque(ptx::smem_u32(&empty[0])),
-                   cmd0 = ptx::opaque(ptx::smem_u32(&cmd[0][0]));
-    uint32_t tile_it = 0, gbase = 0;
-    const uint32_t a_lo0 = (uint32_t)a_desc0, a_hi = (uint32_t)(a_desc0 >> 32);
-    bool alive = true;
-    for (int li = li0; li < li1 && alive; ++li, ++tile_it) {
-      const int t = tiles[li];
-      const int kt = t % p.n_ktiles;
-      const int n_groups = sched[4 + 4 * kt + 1];
-      if (!__all_sync(0xffffffffu, ptx::mbar_wait(&acc_empty, tile_it & 1, abort_flag))) { g_tc_error = 3; break; }
-      ptx::tc_fence_after();
-      int g = (int)((NP + iw - (gbase % NP)) % NP);
-      uint32_t pj = (gbase + g) / NP;
-      uint32_t js = pj % HS, ph = (pj / HS) & 1;
-      for (; g < n_groups; g += NP) {
-        const uint32_t st = iw + NP * js;
-        if (!__all_sync(0xffffffffu, ptx::mbar_wait_a(full0 + st * 8, ph, abort_flag))) { g_tc_error = 4; alive = false; break; }
-        const bool tr = p.trace && blockIdx.x == 0 && lane == 0 && (gbase + g) < 256;
-        if (tr) p.trace[(gbase + g) * 8 + 2] = clock64();
-        bool my_turn = true;
-        if (NP > 1)
-          my_turn = (iw == 0) ? (pj == 0 || ptx::mbar_wait(&turn[0], (pj - 1) & 1, abort_flag))
-                              : ptx::mbar_wait(&turn[iw], pj & 1, abort_flag);
-        if (!__all_sync(0xffffffffu, my_turn)) { g_tc_error = 5; alive = false; break; }
-        if (tr) p.trace[(gbase + g) * 8 + 3] = clock64();
-        ptx::tc_fence_after();
-        if (ptx::elect_one()) {
-          const uint32_t a_lo = a_lo0 + st * (STAGE_BYTES >> 4);
-          const uint32_t cq = cmd0 + st * (16 * 8);
-          int2 c[16];
+  float acc[MI][NW / 2];
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+  for (int m = 0; m < MI; ++m)
 #pragma unroll
-            for (int r = 0; r < 4; r += 2)
-              asm volatile("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];"
-                           : "=r"(c[h * 8 + r].x), "=r"(c[h * 8 + r].y), "=r"(c[h * 8 + r + 1].x), "=r"(c[h * 8 + r + 1].y) : "r"(cq + (h * 8 + r) * 8));
-          const int n0 = (int)((uint32_t)c[0].y >> 20), n1 = (int)((uint32_t)c[8].y >> 20);
-          if (n0 > 4) {
+    for (int i = 0; i < NW / 2; ++i) acc[m][i] = 0.f;
+
+  for (int e = 0; e < count; ++e) {
+    const uint32_t st = base + (uint32_t)(e % ST) * Sh::STAGE;
+    if (!ptx::mbar_wait(&full[e % ST], (uint32_t)(e / ST) & 1)) g_tc_error = 41;
+    ptx::wg_fence();
 #pragma unroll
-            for (int r = 4; r < 8; r += 2)
-              asm volatile("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(c[r].x), "=r"(c[r].y), "=r"(c[r + 1].x), "=r"(c[r + 1].y) : "r"(cq + r * 8));
-          }
-          if (n1 > 4) {
+    for (int ks = 0; ks < 2; ++ks) {
+      // fprop: the TB W blocks are TB MN atoms of 32 columns, one block apart (LBO); bprop: their rows simply continue
+      const uint64_t bdesc = BPROP ? ptx::make_desc(st + Sh::XBYTES + ks * 32, 16, 512, ptx::SWZ_64B)
+                                   : ptx::make_desc(st + Sh::XBYTES + ks * 1024, Sh::WBYTES, 512, ptx::SWZ_64B);
 #pragma unroll
-            for (int r = 12; r < 16; r += 2)
-              asm volatile("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];" : "=r"(c[r].x), "=r"(c[r].y), "=r"(c[r + 1].x), "=r"(c[r + 1].y) : "r"(cq + r * 8));
-          }
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            if (p.ablate & 1) break;
-            const int h = ks >> 1;
-            const int nr = h ? n1 : n0;
-            const uint64_t adesc = ((uint64_t)a_hi << 32) | (uint32_t)(a_lo + ks * a_kstep16);
-#pragma unroll
-            for (int r = 0; r < 8; ++r) {
-              if (r >= nr) break;              // uniform branch: skipped runs cost nothing
-              const int2 cc = c[h * 8 + r];
-              const uint64_t bdesc = ((uint64_t)b_desc_hi << 32) | (uint32_t)((uint32_t)cc.x + (ks & 1) * b_kstep16);
-              const uint32_t d_addr = tmem + ((uint32_t)cc.y & 0xfffu);
-              const uint32_t idesc = idesc0 | ((((uint32_t)cc.y >> 12) & 0x3fu) << 17);
-              if (r == 0) ptx::mma_ss_a_fill(d_addr, adesc, bdesc, idesc, 1u);
-              else        ptx::mma_ss_a_use(d_addr, adesc, bdesc, idesc, 1u);
-            }
-          }
-          ptx::tc_commit_a(empty0 + st * 8);   // the stage is free once these MMAs retire
-          if (NP > 1) {
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&turn[iw + 1 == NP ? 0 : iw + 1]);     // hand the turn to the next issuer
-          }
-        }
-        __syncwarp();
-        if (tr) p.trace[(gbase + g) * 8 + 4] = clock64();
-        ++pj;
-        if (++js == HS) { js = 0; ph ^= 1; }
-      }
-      if (ptx::elect_one()) ptx::tc_commit(&acc_full);   // arrives when this warp's MMAs of the tile have retired
-      __syncwarp();
-      gbase += (uint32_t)n_groups;
-    }
-  } else {
-    // ================================ epilogue ================================
-    constexpr int EG = EW / 4;                         // warp groups; group eg handles slots with (slot - s0) % EG == eg
-    constexpr int ETH = EW * 32;
-    const int ew = warp - 2 * NP;
-    const int quad = warp & 3;                         // TMEM lane quadrant this warp may access
-    const int eg = ew / 4;
-    const int row = quad * 32 + lane;                  // row of the 128-row tile
-    const int etid = ew * 32 + lane;
-    uint32_t tile_it = 0;
-    // accumulators start from zero: clear this warp's share once, then after every read-out
-    for (int c = eg * 32; c < Cfg::TCOLS; c += 32 * EG) ptx::tmem_st_zero_x32(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)c);
-    ptx::tmem_st_wait();
-    ptx::tc_fence_before();
-    asm volatile("bar.sync 1, %0;" ::"n"(ETH) : "memory");
-    if (etid == 0) ptx::mbar_arrive(&acc_empty);
-    for (int li = li0; li < li1; ++li, ++tile_it) {
-      const int t = tiles[li];
-      const int nt = t / p.n_ktiles, kt = t - nt * p.n_ktiles;
-      const int32_t* th = sched + 4 + 4 * kt;
-      const int first_out = th[2];
-      const int n_out = th[3] & 0xff;
-      const uint32_t mask = (uint32_t)th[3] >> 8;
-      ptx::mbar_wait(&acc_full, tile_it & 1, abort_flag);
-      asm volatile("bar.sync 1, %0;" ::"n"(ETH) : "memory");
-      if (*abort_flag) { g_tc_error = 6; break; }       // uniform across the epilogue threads
-      ptx::tc_fence_after();
-      if (p.ablate & 4) {
-        asm volatile("bar.sync 1, %0;" ::"n"(ETH) : "memory");
-        if (etid == 0) ptx::mbar_arrive(&acc_empty);
-        continue;
-      }
-      if (p.axis0) {
-        // Y is (K, N): lane = minibatch column, register j = output feature -> for every j a warp writes 32
-        // consecutive 16-bit values (one 64-byte segment); no staging needed.
-        const long long gcol = (long long)nt * 128 + row;
-        uint16_t* ycol = reinterpret_cast<uint16_t*>(p.y) + (long long)first_out * BS * p.y_pitch + gcol;
-        for (int slot = eg; slot < n_out; slot += EG) {
-          uint32_t v[32];
-          if ((mask >> slot) & 1u) {
-            ptx::tmem_ld_x32(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(slot * BS), v);
-            ptx::tmem_ld_wait();
-            ptx::tmem_st_zero_x32(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(slot * BS));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = 0u;
-          }
-          if (gcol < p.N) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              uint16_t o;
-              if (BF16) { __nv_bfloat16 q = __float2bfloat16_rn(__uint_as_float(v[j])); o = *reinterpret_cast<uint16_t*>(&q); }
-              else      { __half q = __float2half_rn(__uint_as_float(v[j]));            o = *reinterpret_cast<uint16_t*>(&q); }
-              ycol[(long long)(slot * BS + j) * p.y_pitch] = o;
-            }
-          }
-        }
-        ptx::tmem_st_wait();
-        ptx::tc_fence_before();
-        asm volatile("bar.sync 1, %0;" ::"n"(ETH) : "memory");
-        if (etid == 0) ptx::mbar_arrive(&acc_empty);
-      } else {
-        for (int s0 = 0; s0 < n_out; s0 += STG) {
-          // the staging buffers must have been drained by the TMA stores issued before
-          if (etid == 0) ptx::tma_store_wait_read<0>();
-          asm volatile("bar.sync 1, %0;" ::"n"(ETH) : "memory");
-          const int s1 = min(n_out, s0 + STG);
-          for (int slot = s0 + eg; slot < s1; slot += EG) {
-            uint8_t* dst = sO + (slot - s0) * OBYTES + row * 64;
-            uint32_t v[32];
-            if ((mask >> slot) & 1u) {
-              ptx::tmem_ld_x32(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(slot * BS), v);
-              ptx::tmem_ld_wait();
-              ptx::tmem_st_zero_x32(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(slot * BS));
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] = 0u;    // output block with an empty LUT row
-            }
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {                // four 16-byte chunks (8 elements each)
-              uint32_t pk[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float a = __uint_as_float(v[c * 8 + 2 * e]), b = __uint_as_float(v[c * 8 + 2 * e + 1]);
-                if (BF16) { __nv_bfloat162 q = __floats2bfloat162_rn(a, b); pk[e] = *reinterpret_cast<uint32_t*>(&q); }
-                else      { __half2 q = __floats2half2_rn(a, b);           pk[e] = *reinterpret_cast<uint32_t*>(&q); }
-              }
-              const uint32_t swz = (uint32_t)c ^ ((row >> 1) & 3);               // SWIZZLE_64B: chunk ^= (row / 2) % 4
-              *reinterpret_cast<uint4*>(dst + swz * 16) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            }
-          }
-          ptx::tmem_st_wait();
-          ptx::tc_fence_before();
-          ptx::fence_proxy_async();
-          asm volatile("bar.sync 1, %0;" ::"n"(ETH) : "memory");
-          if (etid == 0) {
-            if (s1 == n_out) ptx::mbar_arrive(&acc_empty);     // accumulators are free for the next tile
-            for (int slot = s0; slot < s1; ++slot)
-              ptx::tma_store_2d(&maps.y, sO + (slot - s0) * OBYTES, (first_out + slot) * BS, nt * 128);
-            ptx::tma_store_commit();
-          }
-        }
+      for (int m = 0; m < MI; ++m) {
+        const uint64_t adesc = AXIS0 ? ptx::make_desc(st + m * 4096 + ks * 2048, 4096, 1024, ptx::SWZ_128B)
+                                     : ptx::make_desc(st + m * 64 * 64 + ks * 32, 16, 512, ptx::SWZ_64B);
+        ptx::wgmma<BF16, AXIS0 ? 1 : 0, BPROP ? 0 : 1, NW>(acc[m], adesc, bdesc);
       }
     }
-    if (etid == 0) ptx::tma_store_wait<0>();
+    ptx::wg_commit();
+    ptx::wg_wait<1>();
+    __syncthreads();
+    if (tid == 0 && e >= 1 && e - 1 + ST < count) issue(e - 1 + ST);
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == NP) ptx::tmem_dealloc(tmem, Cfg::TCOLS);
+  ptx::wg_wait<0>();
+#pragma unroll
+  for (int m = 0; m < MI; ++m) ptx::wg_fence_regs(acc[m]);
+
+  // epilogue (output blocks with no entry are written as zeros)
+  uint16_t* y = reinterpret_cast<uint16_t*>(p.y);
+#pragma unroll
+  for (int m = 0; m < MI; ++m)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long long n = (long long)nt * MI * 64 + m * 64 + warp * 16 + lane / 4 + 8 * h;
+      if (n >= p.N) continue;
+#pragma unroll
+      for (int j = 0; j < NW / 8; ++j) {
+        const int cl = 8 * j + 2 * (lane % 4);
+        const int o = t * TB + cl / 32;
+        if (o >= p.n_out) continue;
+        const int col = o * 32 + cl % 32;
+        const float a = acc[m][4 * j + 2 * h], b = acc[m][4 * j + 2 * h + 1];
+        if (!AXIS0) {
+          *reinterpret_cast<uint32_t*>(y + n * p.y_pitch + col) = pack2<BF16>(a, b);
+        } else {
+          y[(long long)col * p.y_pitch + n] = pack1<BF16>(a);
+          y[(long long)(col + 1) * p.y_pitch + n] = pack1<BF16>(b);
+        }
+      }
+    }
 }
 
-inline unsigned long long* xprop2_trace_buffer() {
-  static unsigned long long* buf = [] {
-    unsigned long long* b = nullptr;
-    if (getenv("BSMM_TRACE") && cudaMalloc(&b, 256 * 8 * sizeof(unsigned long long)) == cudaSuccess) cudaMemset(b, 0, 256 * 8 * 8);
-    return b;
-  }();
-  return buf;
-}
-
-template <class Cfg, bool BF16>
-int launch_tc_xprop2(const Xprop2Params& p, const XpropTmaps& maps, int n_ctas, cudaStream_t s) {
-  auto kern = tc_xprop2_kernel<Cfg, BF16>;
+template <int TB, int MI, bool BF16, bool AXIS0, bool BPROP>
+int launch_tc_xprop2(const Xprop2Params& p, const XpropTmaps& maps, int n_tiles, cudaStream_t s) {
+  auto kern = tc_xprop2_kernel<TB, MI, BF16, AXIS0, BPROP>;
+  constexpr size_t smem = Xp2Shape<TB, MI>::SMEM;
   static thread_local uint64_t configured = 0;
-  if (int e = ensure_dyn_smem(kern, Cfg::SMEM, configured)) return e;
-  kern<<<n_ctas, Cfg::THREADS, Cfg::SMEM, s>>>(p, maps);
-  return check_launch("tcgen05_xprop2_bs32");
+  if (int e = ensure_dyn_smem(kern, smem, configured)) return e;
+  kern<<<dim3((unsigned)((p.N + MI * 64 - 1) / (MI * 64)), (unsigned)n_tiles), XP_THREADS, smem, s>>>(p, maps);
+  return check_launch("wgmma_xprop2_bs32");
 }
 
-// Variants (blocks per tile, CTAs per SM, W slots per stage, stages, pipelines, staging buffers, epilogue warps):
-//   V_SPARSE  <= ~12 % density: ~2 W blocks per pair-group; deep ring, the kernel is bound by the TMA round trip
-//   V_MID     12..45 %: ~4-7 W blocks per pair-group
-//   V_WIDE    one CTA per SM with 16-block tiles: the activation panel is re-read 8 instead of 16 times
-using Xp2Sparse = Xp2Cfg<8, 2, 4, 4, 2, 2, 4>;      // 4 x 24 KB + 16 KB = 112 KB
-using Xp2Mid    = Xp2Cfg<8, 2, 8, 3, 3, 2, 4>;      // 3 x 32 KB + 16 KB = 112 KB
-using Xp2Wide   = Xp2Cfg<16, 1, 12, 4, 2, 4, 8>;    // 4 x 40 KB + 32 KB = 192 KB
+template <int TB, int MI, bool BF16>
+int dispatch_tc_xprop2(const Xprop2Params& p, const XpropTmaps& maps, int n_tiles, bool axis0, bool bprop, cudaStream_t s) {
+  if (axis0) return bprop ? launch_tc_xprop2<TB, MI, BF16, true, true>(p, maps, n_tiles, s) : launch_tc_xprop2<TB, MI, BF16, true, false>(p, maps, n_tiles, s);
+  return bprop ? launch_tc_xprop2<TB, MI, BF16, false, true>(p, maps, n_tiles, s) : launch_tc_xprop2<TB, MI, BF16, false, false>(p, maps, n_tiles, s);
+}
 
-// sched_variant: 1 = sparse, 2 = mid, 3 = wide (chosen by the host from the layout density, matmul.py)
+// sched: lut.py:build_wide_schedule in device memory: tile offsets at int32 index 2, merged entries at ent_off.
 inline int tc_xprop2(int dtype, int axis, int bprop, int n_out, int n_in, int blocks, const void* x, const void* w, void* y,
-                     int N, const int32_t* sched, int sched_tiles, int variant, int groups_off, int list_off, int n_ctas,
-                     int sched_ntiles, cudaStream_t s) {
-  if (dtype != BSMM_F16 && dtype != BSMM_BF16) return fail(BSMM_E_ARG, "bsmm_xprop: the pair schedule needs a 16-bit dtype");
+                     int N, const int32_t* sched, int n_tiles, int variant, int ent_off, cudaStream_t s) {
+  if (dtype != BSMM_F16 && dtype != BSMM_BF16) return fail(BSMM_E_ARG, "bsmm_xprop: the wide-tile schedule needs a 16-bit dtype");
+  if (variant < 1 || variant > 3) return fail(BSMM_E_ARG, "bsmm_xprop: wide-tile variant %d (1..3)", variant);
+  const int tb = variant == 3 ? 4 : 2;
+  if (sched == nullptr || n_tiles <= 0 || (long long)n_tiles * tb < n_out || ent_off < n_tiles + 3)
+    return fail(BSMM_E_ARG, "bsmm_xprop: inconsistent wide-tile schedule (tiles=%d variant=%d entries at %d)", n_tiles, variant, ent_off);
   if (axis == 0 && (N & 7)) { fail(0, "feature_axis 0 needs N %% 8 == 0 for TMA (row pitch multiple of 16 bytes)"); return TC_NOT_APPLICABLE; }
   if (((uintptr_t)x | (uintptr_t)w | (uintptr_t)y) & 15) { fail(0, "pointers must be 16-byte aligned for TMA"); return TC_NOT_APPLICABLE; }
-  const DeviceInfo& dev = device_info();
-  if (!dev.ok || dev.cc_major != 10) { fail(0, "tcgen05 needs an sm_100 device"); return TC_NOT_APPLICABLE; }
-  const int tb = variant == 3 ? 16 : 8;
-  if (sched == nullptr || sched_tiles <= 0 || (long long)sched_tiles * tb < n_out || groups_off < 4 + 4 * sched_tiles ||
-      (groups_off & 31) || list_off <= groups_off || n_ctas <= 0 || variant < 1 || variant > 3)
-    return fail(BSMM_E_ARG, "bsmm_xprop: inconsistent pair schedule (tiles=%d variant=%d groups_off=%d list_off=%d ctas=%d)",
-                sched_tiles, variant, groups_off, list_off, n_ctas);
-  if (sched_ntiles != (N + 127) / 128)
-    return fail(BSMM_E_ARG, "bsmm_xprop: tile lists were built for %d minibatch tiles, N=%d needs %d", sched_ntiles, N, (N + 127) / 128);
-  const int occ = variant == 3 ? 1 : 2;
-  if (n_ctas > dev.sm_count * occ)
-    return fail(BSMM_E_ARG, "bsmm_xprop: tile lists built for %d CTAs, the device runs %d at once", n_ctas, dev.sm_count * occ);
+  if (!wgmma_device()) return TC_NOT_APPLICABLE;
 
-  static thread_local bool ctx_bound = false;
-  if (!ctx_bound) { cudaFree(nullptr); ctx_bound = true; }
+  const int rows = variant == 1 ? 64 : 128;
   const uint64_t Cin = (uint64_t)n_in * 32, Cout = (uint64_t)n_out * 32;
   XpropTmaps maps;
   if (axis == 1) {
-    if (int e = cached_tmap_2d(&maps.x, dtype, x, Cin, (uint64_t)N, Cin, 64, 128, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
-  } else {       // (C, N): inner dim = minibatch; box = 64 columns x 64 feature rows, 128-byte rows
-    if (int e = cached_tmap_2d(&maps.x, dtype, x, (uint64_t)N, Cin, (uint64_t)N, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
+    if (int e = cached_tmap_2d(&maps.x, dtype, x, Cin, (uint64_t)N, Cin, 32, rows, CU_TENSOR_MAP_SWIZZLE_64B)) return e;
+  } else {
+    if (int e = cached_tmap_2d(&maps.x, dtype, x, (uint64_t)N, Cin, (uint64_t)N, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   }
   if (int e = cached_tmap_2d(&maps.w, dtype, w, 32, (uint64_t)blocks * 32, 32, 32, 32, CU_TENSOR_MAP_SWIZZLE_64B)) return e;
-  if (int e = cached_tmap_2d(&maps.y, dtype, y, Cout, (uint64_t)N, Cout, 32, 128, CU_TENSOR_MAP_SWIZZLE_64B)) return e;
-
   Xprop2Params p;
-  p.sched = sched; p.groups_off = groups_off; p.list_off = list_off; p.n_ktiles = sched_tiles;
-  p.bprop = bprop; p.axis0 = axis == 0;
+  p.tile_off = sched + 2; p.ent = sched + ent_off; p.n_out = n_out; p.w_absent = blocks;
   p.y = y; p.y_pitch = axis == 0 ? (long long)N : (long long)Cout; p.N = N;
-  static const int ablate = [] { const char* e = getenv("BSMM_ABLATE"); return e ? atoi(e) : 0; }();
-  p.ablate = ablate;
-  p.trace = xprop2_trace_buffer();
-  const bool bf = dtype == BSMM_BF16;
+  const bool bf = dtype == BSMM_BF16, a0 = axis == 0, bp = bprop != 0;
   switch (variant) {
-    case 1: return bf ? launch_tc_xprop2<Xp2Sparse, true>(p, maps, n_ctas, s) : launch_tc_xprop2<Xp2Sparse, false>(p, maps, n_ctas, s);
-    case 2: return bf ? launch_tc_xprop2<Xp2Mid, true>(p, maps, n_ctas, s) : launch_tc_xprop2<Xp2Mid, false>(p, maps, n_ctas, s);
-    default: return bf ? launch_tc_xprop2<Xp2Wide, true>(p, maps, n_ctas, s) : launch_tc_xprop2<Xp2Wide, false>(p, maps, n_ctas, s);
+    case 1: return bf ? dispatch_tc_xprop2<2, 1, true>(p, maps, n_tiles, a0, bp, s) : dispatch_tc_xprop2<2, 1, false>(p, maps, n_tiles, a0, bp, s);
+    case 2: return bf ? dispatch_tc_xprop2<2, 2, true>(p, maps, n_tiles, a0, bp, s) : dispatch_tc_xprop2<2, 2, false>(p, maps, n_tiles, a0, bp, s);
+    default: return bf ? dispatch_tc_xprop2<4, 2, true>(p, maps, n_tiles, a0, bp, s) : dispatch_tc_xprop2<4, 2, false>(p, maps, n_tiles, a0, bp, s);
   }
 }
 

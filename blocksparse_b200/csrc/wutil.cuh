@@ -1,4 +1,4 @@
-// Utilities on the block-sparse weight format (blocks, bs, bs) and its neighbours on the hot path -- SURVEY.md 8(f) rows 2-4.
+// Utilities on the block-sparse weight format (blocks, bs, bs) and its neighbours on the hot path.
 // All of them are HBM-bound passes over W (or over the activations), so the kernels are built around wide coalesced
 // accesses and warp-shuffle reductions, one warp (or one small CTA) per block / block column, no atomics.
 //
@@ -242,11 +242,11 @@ __global__ void gather_rows_kernel(const T* __restrict__ x, const T* __restrict_
 }
 
 // ---- 8 x 8 blocks on the tensor cores: pad 2 x 2 neighbourhoods into 16 x 16 blocks ---------------------------------
-// tcgen05.mma needs N >= 16, so an 8 x 8 block cannot be a B operand on its own.  The host layer builds a SHADOW layout of
+// wgmma needs K = 16 per step, so an 8 x 8 block cannot be an operand on its own.  The host layer builds a SHADOW layout of
 // 16 x 16 super-blocks (one per 2 x 2 neighbourhood that holds at least one 8 x 8 block), these kernels scatter the weights
 // into it (absent sub-blocks are zero, the optional gate is folded in) and gather the weight gradient back out.  The padded
-// product multiplies zeros -- at 20 % density about a third of the super-block is real -- but runs ~10x faster than the
-// CUDA-core FMA kernels (profiles/r2_bench_cfg4.jsonl).
+// product multiplies zeros -- at 20 % density about a third of the super-block is real -- but runs on the tensor cores
+// instead of the CUDA-core FMA kernels.
 template <typename T>
 __global__ void pad_blocks_kernel(const T* __restrict__ w_small, const int32_t* __restrict__ sub_map, const float* __restrict__ gate,
                                   T* __restrict__ w_big, int blocks_big, int bs) {

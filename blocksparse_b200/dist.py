@@ -2,7 +2,7 @@
 
 fprop and bprop are independent per minibatch column, so they need no communication.  updat reduces over
 the minibatch: each rank produces the partial dW of its shard and the true dW is the SUM over ranks -- one
-all-reduce per weight tensor (SURVEY.md section 8e; the reference leaves this to user code through its
+all-reduce per weight tensor (the reference leaves this to user code through its
 AllreduceNccl op, examples/transformer/enwik8.py:220-231).  One process per GPU, torch.distributed (NCCL on
 GPUs; the same code runs on gloo for the CPU tests of the host logic).
 """
@@ -39,13 +39,11 @@ def allreduce_dw(dw, group=None, average=False, async_op=False):
 
 
 def reserve_sms_for_nccl(n_sms=8, nccl_ctas=None):
-    """Leave `n_sms` SMs free of persistent tcgen05 CTAs so that a concurrent NCCL kernel has somewhere to run.
+    """Leave `n_sms` SMs to a concurrent NCCL kernel.
 
-    The block-sparse kernels are persistent grids sized to the whole GPU (one or two CTAs per SM, host-built tile lists).
-    An all-reduce issued on a side stream cannot start while such a grid owns every SM, and a compute kernel launched
-    while NCCL holds SMs runs its displaced CTAs as a second wave (profiles/r1_dist_diag.txt: zero overlap).  With a
-    margin, every persistent grid and its schedules are built for sm_count - n_sms SMs (csrc/common.cuh:sm_margin,
-    _lib.grid_sms) and NCCL is capped to as many CTAs (NCCL_MAX_CTAS), so both run side by side.
+    NCCL is capped to that many CTAs (NCCL_MAX_CTAS) and the host-built updat schedule balances its tiles over
+    sm_count - n_sms SMs (csrc/common.cuh:sm_margin, _lib.grid_sms), so a dW all-reduce on a side stream and the next
+    block-sparse kernels can run side by side.
     Must be called before the first block-sparse op and before the process group is created; explicit environment
     settings win.  Returns the margin in effect.
     """
@@ -54,17 +52,13 @@ def reserve_sms_for_nccl(n_sms=8, nccl_ctas=None):
     margin = int(os.environ["BSMM_SM_MARGIN"])
     if margin > 0:
         os.environ.setdefault("NCCL_MAX_CTAS", str(int(nccl_ctas or margin)))
-        # (BSMM_TILE_QUEUE=dynamic lets late-starting CTAs pull tiles from a global counter instead of owning a fixed
-        # share; with a margin that NCCL respects it measured the same as the static deal, profiles/r2_scaling.txt)
     return margin
 
 
 def nccl_options():
-    """ProcessGroupNCCL options for runs that overlap the dW all-reduce with the persistent kernels: the collective runs on
-    a HIGH-PRIORITY stream.  The next compute kernel and the NCCL kernel become runnable at the same moment (when updat
-    retires); if the compute grid is placed first it spreads over all SMs and the NCCL CTAs -- which need most of an SM
-    each -- wait for a whole kernel (measured: 0.70 instead of 0.23 ms per step at 2 GPUs, profiles/r2_scaling.txt).  With
-    priority the NCCL CTAs are placed first and the compute grid, sized for sm_count - margin SMs, fits beside them."""
+    """ProcessGroupNCCL options for runs that overlap the dW all-reduce with the block-sparse kernels: the collective runs
+    on a HIGH-PRIORITY stream.  The next compute kernel and the NCCL kernel become runnable at the same moment (when updat
+    retires); with priority the NCCL CTAs are placed first instead of waiting for a whole compute grid to drain."""
     opts = dist.ProcessGroupNCCL.Options()
     opts.is_high_priority_stream = True
     return opts

@@ -1,6 +1,6 @@
 """Synthetic block layouts of the reference's tests and benchmarks (host-side helpers, NumPy only).
 
-  bernoulli_layout        i.i.d. Bernoulli(density) with the diagonal forced on (SURVEY.md 8d)
+  bernoulli_layout        i.i.d. Bernoulli(density) with the diagonal forced on
   barabasi_albert_layout  the skewed layout of test/blocksparse_matmul_bench.py:53-68: Barabasi-Albert adjacency
                           + identity + a dense m x m corner (networkx is not needed: the preferential-attachment
                           process is restated here)

@@ -166,6 +166,11 @@ class MatmulLuts(object):
     def updat_schedule(self, bsize, k_per_tile=None, n_cta=None):
         return build_updat_schedule(self.updat_lut, self.CB, self.KB, bsize, k_per_tile, n_cta)
 
+    def wide_schedule(self, bprop, blocks_per_tile):
+        outs, ins, wids = self._b if bprop else self._f
+        n_out = self.CB if bprop else self.KB
+        return build_wide_schedule(outs, ins, wids, n_out, blocks_per_tile)
+
     def pair_schedule(self, bprop, blocks_per_tile, w_per_group, n_tiles, n_ntiles, n_ctas, bsize=32):
         outs, ins, wids = self._b if bprop else self._f
         n_out = self.CB if bprop else self.KB
@@ -180,6 +185,41 @@ class MatmulLuts(object):
         outs, ins, wids = self._b if bprop else self._f
         n_out = self.CB if bprop else self.KB
         return build_tile_schedule(outs, ins, wids, n_out, blocks_per_tile, bsize, w_per_group, n_tiles, n_ntiles)
+
+
+WIDE_REC = 8             # ints per merged entry of build_wide_schedule (csrc/tc_xprop2.cuh XP2_REC)
+
+
+def build_wide_schedule(outs, ins, wids, n_out, blocks_per_tile):
+    """Merged LUT rows for the wide-tile xprop kernel (csrc/tc_xprop2.cuh).
+
+    Tile t covers output blocks [t*T, (t+1)*T), T = blocks_per_tile <= 4.  Its entries are the distinct input blocks
+    consumed by any of them, in ascending order, each with the W block of every output block of the tile (-1: none).
+
+    int32 layout:
+      [0] n_tiles  [1] T  [2 .. 2+n_tiles]  first entry of every tile (n_tiles + 1 offsets)
+      entries from `entry_offset` (a multiple of WIDE_REC): [in_block, w_0 .. w_{T-1}, -1 ...] (WIDE_REC ints each)
+    Returns (schedule, n_tiles, entry_offset).
+    """
+    T = int(blocks_per_tile)
+    assert 1 <= T <= WIDE_REC - 1
+    outs = np.asarray(outs, dtype=np.int64)
+    ins = np.asarray(ins, dtype=np.int64)
+    wids = np.asarray(wids, dtype=np.int64)
+    n_tiles = max(1, ceil_div(n_out, T))
+    n_in = int(ins.max()) + 1 if len(ins) else 1
+    key = (outs // T) * n_in + ins                       # (tile, input block)
+    uniq, inv = np.unique(key, return_inverse=True)
+    tile_of = uniq // n_in
+    offsets = np.searchsorted(tile_of, np.arange(n_tiles + 1))
+    ent_off = ceil_div(3 + n_tiles, WIDE_REC) * WIDE_REC
+    sched = np.full(ent_off + WIDE_REC * len(uniq), -1, dtype=np.int32)
+    sched[0:2] = (n_tiles, T)
+    sched[2:3 + n_tiles] = offsets
+    ent = sched[ent_off:].reshape(len(uniq), WIDE_REC)
+    ent[:, 0] = uniq % n_in
+    ent[inv, 1 + outs % T] = wids
+    return sched, n_tiles, ent_off
 
 
 GROUP_INTS = 32          # one 128-byte record per schedule group (one coalesced warp load)
@@ -224,10 +264,11 @@ def tile_order(tile_cost, n_ntiles):
 
 
 def build_tile_schedule(outs, ins, wids, n_out, blocks_per_tile, bsize=32, w_per_group=8, n_tiles=None, n_ntiles=None):
-    """Schedule for the tcgen05 xprop kernel (csrc/tc.cuh).
+    """Tile schedule for a tile-grouped xprop formulation (the wgmma xprop kernel of csrc/tc.cuh walks the row
+    LUTs instead and does not use it).
 
     An output tile covers `blocks_per_tile` consecutive output blocks (their fp32 accumulators live
-    side by side in tensor memory, block s of the tile at columns [s*bsize, (s+1)*bsize)).  For every
+    side by side, block s of the tile at columns [s*bsize, (s+1)*bsize)).  For every
     tile the LUT is regrouped by INPUT block: a *group* is one activation tile plus the <= w_per_group
     W blocks of the tile that consume it (an input block with more consumers is split into several
     groups).  Everything the device loops would otherwise derive per block is precomputed here:
@@ -437,12 +478,10 @@ def lpt_tile_lists(tile_cost, n_ntiles, n_ctas):
 
 
 def build_pair_schedule(outs, ins, wids, n_out, blocks_per_tile, w_per_group, n_tiles, n_ntiles, n_ctas, bsize=32):
-    """Schedule for the wide-activation-tile tcgen05 xprop kernel (csrc/tc_xprop2.cuh, 32 x 32 blocks).
+    """Schedule for a wide-activation-tile xprop formulation (32 x 32 blocks; not used by the wgmma kernels).
 
     Same idea as build_tile_schedule, but a group is an input-block PAIR (2p, 2p+1): its activation tile is
-    128 rows x 64 features = 128-byte rows, so every TMA row request moves a full 128-byte line (the 64-byte rows of
-    the single-block tile left the SM's L1->crossbar request port -- one request per cycle -- 67 % busy at 45 B/clk,
-    profiles/r1_ncu_tc_kernels.txt), and ~2x the W blocks consume each staged tile.  W blocks are listed half 0
+    128 rows x 64 features = 128-byte rows, so every TMA row request moves a full 128-byte line, and ~2x the W blocks consume each staged tile.  W blocks are listed half 0
     (input block 2p) first, then half 1, each in accumulator order, so that the runs of one half are issued back to
     back against the same K slices of the tile (A-collector reuse).
 
@@ -578,7 +617,7 @@ def _balance_windows(g_cnt, g_nwin, KT, n_cta):
 
 
 def build_updat_schedule(updat_lut, CB, KB, bsize, k_per_tile=None, n_cta=None):
-    """Schedule for the tcgen05 updat kernel (csrc/tc_updat.cuh): a "gathered dense GEMM".
+    """Schedule for the wgmma updat kernel (csrc/tc_updat.cuh): a "gathered dense GEMM".
 
     A tile pairs a GROUP of 128/bsize consecutive input blocks (128 features = the MMA M axis) with up
     to `k_per_tile` output blocks taken from a window of consecutive output blocks, keeping only those
@@ -672,7 +711,8 @@ def xn_lut(outs, ins, n_out):
 
 
 def build_nt_items(tn_rows_per_head):
-    """Schedule for the tcgen05 NT kernel (csrc/tc_bst.cuh): blocks that share a key block, two at a time.
+    """Pairing of the blocks that share a key block, two at a time (an NT schedule; the wgmma NT kernel of
+    csrc/tc_bst.cuh takes one block per CTA from the NT LUT and does not use it).
 
     tn_rows_per_head[h][k] = [(block_id, q_block), ...] (the reference's tn_list).  Returns int32
     [lut_heads][n_items][8] = (k_blk, n_valid, blk0, q0, blk1, q1, 0, 0); heads with fewer pairs are padded with

@@ -1,8 +1,8 @@
-"""BlocksparseMatMul for B200 -- host side.
+"""BlocksparseMatMul for H100 -- host side.
 
 Keeps the Python op surface of the reference's blocksparse/matmul.py (class
 BlocksparseMatMul :74-483, gradient wiring :485-527, group_param_grads :612-731) but
-operates on torch tensors and calls the sm_100a kernels through the C ABI in
+operates on torch tensors and calls the sm_90a kernels through the C ABI in
 include/bsmm_b200.h.  There is no CPU path: tensors must live on a CUDA device.
 """
 import ctypes
@@ -13,28 +13,16 @@ import torch
 
 from . import _lib
 from .checkers import MatmulCheckers
-from .lut import MatmulLuts, pick_tile_count
+from .lut import MatmulLuts
 
-# Output blocks per xprop tile and CTAs per SM (csrc/tc.cuh XpropCfg<BS, OCC>), picked from B200 timings
-# (profiles/r1_xprop_tuning.txt): 32x32 blocks run best as half-width tiles (8 blocks = 256 TMEM columns) with two
-# CTAs per SM, 64x64 blocks as full-width tiles (8 blocks = 512 columns) with one.  BSMM_XPROP_OCC=1|2 forces one.
-_OCC_ENV = os.environ.get("BSMM_XPROP_OCC", "")
-_OCC = {16: 2, 32: 2, 64: 1} if _OCC_ENV not in ("1", "2") else {16: 2, 32: int(_OCC_ENV), 64: int(_OCC_ENV)}
-_WPG_OVERRIDE = int(os.environ.get("BSMM_XPROP_WPG", "0"))     # tuning aid: force the W-slots-per-stage variant (2 or 4)
-_TILE_BLOCKS = {bs: (256 if occ == 2 else 512) // bs for bs, occ in _OCC.items()}
-# W blocks per schedule group == W slots per pipeline stage of the kernel (XpropCfg::WPS)
-_SCHED_CACHE_MAX = 16
-# csrc/tc_xprop2.cuh variants: id -> (output blocks per tile, CTAs per SM, W slots per stage).  The family is OPT-IN
-# (BSMM_XPROP2=1..3 forces a variant, -1 picks by density): on B200 it measured 5-10 % slower than the single-block kernel
-# of csrc/tc.cuh at every density (profiles/r2_xprop2_study.txt has the timings, the ablations and the pipeline trace that
-# explain why), so 0 -- the default -- keeps csrc/tc.cuh.
-_X2_VARIANTS = {1: (8, 2, 4), 2: (8, 2, 8), 3: (16, 1, 12)}
+# Opt-in xprop variants for 32 x 32 blocks and 16-bit dtypes (the default is csrc/tc.cuh, one output block per CTA):
+# BSMM_XPROP2=1..3 selects a wide-tile kernel (csrc/tc_xprop2.cuh: 2 / 2 / 4 output blocks per CTA, 64 / 128 / 128
+# minibatch rows), BSMM_PAIR_TILES=1 runs csrc/tc.cuh as 2-CTA clusters that share every W block by TMA multicast.
+_X2_VARIANTS = {1: 2, 2: 2, 3: 4}          # variant -> output blocks per tile
 _X2_FORCE = int(os.environ.get("BSMM_XPROP2", "0"))
-# BSMM_PAIR_TILES=1: 32 x 32 blocks at <= ~37 % density run as 2-CTA clusters that multicast the activation tiles
 _PAIR_TILES = int(os.environ.get("BSMM_PAIR_TILES", "0"))
-# BSMM_PAD8=0: keep 8 x 8 blocks on the CUDA-core FMA kernels instead of the padded 16 x 16 tcgen05 path
+# BSMM_PAD8=0: keep 8 x 8 blocks on the CUDA-core FMA kernels instead of the padded 16 x 16 wgmma path
 _PAD8 = int(os.environ.get("BSMM_PAD8", "1"))
-_W_PER_GROUP = {16: 8, 32: 8, 64: 2 if _OCC[64] == 2 else 4}
 
 
 def _as_2d(t, axis, feat):
@@ -85,7 +73,7 @@ class BlocksparseMatMul(MatmulCheckers):
         self.sparsity = round(float(self.blocks) / float(self.CB * self.KB), 3)
         self.layout = layout != 0
         self._dev = {}          # device -> dict of LUT tensors (uploaded once, matmul.py:33-53)
-        # 8 x 8 blocks: tcgen05.mma needs N >= 16, so 16-bit dtypes run on a SHADOW op over 16 x 16 super-blocks (2 x 2
+        # 8 x 8 blocks: the wgmma kernels need K >= 16, so 16-bit dtypes run on a SHADOW op over 16 x 16 super-blocks (2 x 2
         # neighbourhoods, absent sub-blocks zero) fed through bsmm_pad_blocks / bsmm_unpad_blocks (csrc/wutil.cuh)
         self._shadow = None
         if block_size == 8 and _PAD8 and self.CB % 2 == 0 and self.KB % 2 == 0:
@@ -183,92 +171,16 @@ class BlocksparseMatMul(MatmulCheckers):
         d = self._dev.get(key)
         if d is None:
             d = {
-                "plans": {},
                 "fprop": torch.as_tensor(self._luts.fprop_rows, device=device),
                 "bprop": torch.as_tensor(self._luts.bprop_rows, device=device),
                 "updat": torch.as_tensor(self.updat_lut, device=device),
             }
-            tb = _TILE_BLOCKS.get(self.bsize)
-            if tb:
-                d["xprop_sched"] = {}          # (bprop, n_tiles) -> (tensor, n_tiles, groups_off), built on demand
-                d["cta_slots"] = _lib.grid_sms(device) * _OCC[self.bsize]
+            if self.bsize in (16, 32, 64):
                 us, uoff = self._luts.updat_schedule(self.bsize, n_cta=_lib.grid_sms(device))
                 d["updat_sched"] = torch.as_tensor(us, device=device)
                 d["updat_tiles"], d["updat_kt"] = int(us[0]), int(us[2])
             self._dev[key] = d
         return d
-
-    def _xprop2_variant(self, dtype, gate):
-        """Which csrc/tc_xprop2.cuh variant serves this layout (0 = none: 64 x 64 blocks, fp32, dense layouts)."""
-        if self.bsize != 32 or dtype == torch.float32 or _X2_FORCE == 0:
-            return 0
-        if _X2_FORCE in _X2_VARIANTS:
-            return _X2_FORCE
-        density = self.blocks / float(self.CB * self.KB)
-        if density <= 0.12:
-            return 1
-        return 2 if density <= 0.45 else 0
-
-    def _xprop_plan(self, d, device, bprop, N, dtype):
-        """(lut ptr, n_out, n_in, sched ptr | None, sched_tiles, tile_arg, groups_off, list_off, n_ctas, n_ntiles, keepalive)."""
-        n_in, n_out = (self.KB, self.CB) if bprop else (self.CB, self.KB)
-        lut = d["bprop" if bprop else "fprop"]
-
-        sched, sched_tiles, sched_off = None, 0, 0
-        list_off = n_ctas = n_nt = 0
-        variant = self._xprop2_variant(dtype, None) if "xprop_sched" in d else 0
-        if variant:
-            # pair schedule (csrc/tc_xprop2.cuh): wide activation tiles + host-built per-CTA tile lists
-            key = ("pair", bool(bprop), variant, N)
-            plan = d["xprop_sched"].get(key)
-            if plan is None:
-                tb, occ, wps = _X2_VARIANTS[variant]
-                n_nt = -(-N // 128)
-                n_ctas = _lib.grid_sms(device) * occ
-                n_kt = pick_tile_count(n_out, n_nt, n_ctas, tb)
-                arr, off, loff = self._luts.pair_schedule(bprop, tb, wps, n_kt, n_nt, n_ctas)
-                while len(d["xprop_sched"]) >= _SCHED_CACHE_MAX:
-                    d["xprop_sched"].pop(next(iter(d["xprop_sched"])))
-                plan = d["xprop_sched"][key] = (torch.as_tensor(arr, device=device), n_kt, off, loff, n_ctas, n_nt, tb | (variant << 8) | (1 << 16))
-            sched, sched_tiles, sched_off, list_off, n_ctas, n_nt, tile_arg = plan
-        elif "xprop_sched" in d:
-            # tile count chosen so that (minibatch tiles) x (feature tiles) fills whole waves of the persistent grid
-            tb = _TILE_BLOCKS[self.bsize]
-            n_kt = pick_tile_count(n_out, -(-N // 128), d["cta_slots"], tb)
-            # sparse layouts (about one W block per group) use 2 W slots per stage => twice the stages in flight
-            wpg = _W_PER_GROUP[self.bsize]
-            sparse = _OCC[32] == 2 and self.bsize == 32 and self.blocks * tb <= 1.0 * self.CB * self.KB
-            if sparse:
-                wpg = 2
-            elif _OCC[32] == 2 and self.bsize == 32 and _WPG_OVERRIDE:
-                wpg, sparse = _WPG_OVERRIDE, True
-            elif _OCC[32] == 2 and self.bsize == 32 and self.blocks * tb <= 3.0 * self.CB * self.KB:
-                # 1..3 W blocks per group on average (density <= 37.5 %): 4 W slots per stage, 6 stages in flight
-                wpg, sparse = 4, True
-            n_nt = -(-N // 128)
-            if sparse and self.bsize == 32 and _PAIR_TILES and dtype != torch.float32:
-                # 2-CTA clusters over neighbouring output tiles sharing every activation tile by TMA multicast (csrc/tc.cuh, CL = 2)
-                key = ("pairtile", bool(bprop), n_kt, wpg)
-                if key not in d["xprop_sched"]:
-                    arr, off = self._luts.pair_tile_schedule(bprop, tb, self.bsize, wpg, n_kt)
-                    while len(d["xprop_sched"]) >= _SCHED_CACHE_MAX:
-                        d["xprop_sched"].pop(next(iter(d["xprop_sched"])))
-                    d["xprop_sched"][key] = (torch.as_tensor(arr, device=device), int(arr[0]), off, 0)
-                sched, sched_tiles, sched_off, list_off = d["xprop_sched"][key]
-                tile_arg = tb | (wpg << 8) | (1 << 12)
-                key = None
-            else:
-                key = (bool(bprop), n_kt, wpg, n_nt)
-            if key is not None and key not in d["xprop_sched"]:
-                arr, off, ooff = self._luts.tile_schedule(bprop, tb, self.bsize, wpg, n_tiles=n_kt, n_ntiles=n_nt)
-                while len(d["xprop_sched"]) >= _SCHED_CACHE_MAX:       # bounded: one entry per distinct minibatch tile count
-                    d["xprop_sched"].pop(next(iter(d["xprop_sched"])))
-                d["xprop_sched"][key] = (torch.as_tensor(arr, device=device), int(arr[0]), off, ooff)
-            if key is not None:
-                sched, sched_tiles, sched_off, list_off = d["xprop_sched"][key]
-                tile_arg = tb | ((wpg << 8) if sparse else 0)
-        return (lut.data_ptr(), n_out, n_in, None if sched is None else sched.data_ptr(), sched_tiles,
-                tile_arg if sched is not None else 0, sched_off, list_off, n_ctas, n_nt, (lut, sched))
 
     # ------------------------------------------------------------------ raw ops
     def fprop(self, x, w, gate=None, flags=0):
@@ -312,32 +224,35 @@ class BlocksparseMatMul(MatmulCheckers):
         if w.dtype != x.dtype:
             raise ValueError("x and w must have the same dtype")
         N = x2.shape[1] if self.axis == 0 else x2.shape[0]
-        # everything that depends only on (op, minibatch size, dtype class, device) is planned once: LUT / schedule pointers,
-        # tile counts, kernel variant (the per-call Python used to cost ~30 us per launch, tools/host_cost.py)
         d = self._device_luts(x.device)
-        pkey = (bprop, N, x.dtype == torch.float32, _X2_FORCE, _PAIR_TILES)
-        plan = d["plans"].get(pkey)
-        if plan is None:
-            if len(d["plans"]) >= 4 * _SCHED_CACHE_MAX:
-                d["plans"].clear()
-            plan = d["plans"][pkey] = self._xprop_plan(d, x.device, bprop, N, x.dtype)
-        lut_ptr, n_out, n_in, sched_ptr, sched_tiles, tile_arg, sched_off, list_off, n_ctas, n_nt, _keep = plan
+        lut = d["bprop" if bprop else "fprop"]
+        n_in, n_out = (self.KB, self.CB) if bprop else (self.CB, self.KB)
+        sched, sched_tiles, tile_arg, sched_off = None, 0, 0, 0
+        if self.bsize == 32 and x.dtype != torch.float32:
+            if _X2_FORCE in _X2_VARIANTS:
+                key = ("wide", bool(bprop), _X2_VARIANTS[_X2_FORCE])
+                if key not in d:
+                    arr, n_tiles, off = self._luts.wide_schedule(bprop, _X2_VARIANTS[_X2_FORCE])
+                    d[key] = (torch.as_tensor(arr, device=x.device), n_tiles, off)
+                sched, sched_tiles, sched_off = d[key]
+                tile_arg = (1 << 16) | (_X2_FORCE << 8)
+            elif _PAIR_TILES:
+                tile_arg = 1 << 12
         y2 = torch.empty((feat_out, N) if self.axis == 0 else (N, feat_out), dtype=x.dtype, device=x.device)
         if gate is not None:
             gate = gate.to(torch.float32).contiguous()
-            if sched_ptr is not None and x.dtype != torch.float32 and not (flags & _lib.FLAG_FORCE_GENERIC):
-                # gated product on the tcgen05 kernel: fold the gate into a scaled copy of the (small) weight tensor,
+            if self.bsize in (16, 32, 64) and x.dtype != torch.float32 and not (flags & _lib.FLAG_FORCE_GENERIC):
+                # gated product on the wgmma kernel: fold the gate into a scaled copy of the (small) weight tensor,
                 # as the reference's gated kernels do with the loaded weights (cn_64.cu:96-98)
                 wg = torch.empty_like(w)
                 _lib.check(lib.bsmm_gate_weights(_lib.dtype_code(w.dtype), self.bsize, self.blocks, w.data_ptr(),
                                                  gate.data_ptr(), wg.data_ptr(), _lib.stream_ptr()), "bsmm_gate_weights")
                 w, gate = wg, None
         rc = lib.bsmm_xprop(_lib.dtype_code(x.dtype), self.axis, self.bsize, int(bprop),
-                            lut_ptr, n_out, n_in, self.blocks,
+                            lut.data_ptr(), n_out, n_in, self.blocks,
                             x2.data_ptr(), w.data_ptr(), y2.data_ptr(), N,
                             _lib.ptr(gate),
-                            sched_ptr, sched_tiles, tile_arg, sched_off,
-                            list_off, n_ctas, n_nt,
+                            _lib.ptr(sched), sched_tiles, tile_arg, sched_off, 0, 0, 0,
                             flags, _lib.stream_ptr())
         _lib.check(rc, "bsmm_xprop")
         if self.axis == 0:

@@ -1,8 +1,8 @@
-"""BlocksparseTransformer for B200 -- host side.
+"""BlocksparseTransformer for H100 -- host side.
 
 Keeps the Python op surface of the reference's blocksparse/transformer.py (class
 BlocksparseTransformer :51-383, gradient wiring :391-480) on torch tensors, calling the
-sm_100a kernels through the C ABI in include/bsmm_b200.h.
+sm_90a kernels through the C ABI in include/bsmm_b200.h.
 
 Tensor conventions (reference transformer.py:186-203):
   dense  q/k/v : (batch, ctx, heads*head_state), heads-major state

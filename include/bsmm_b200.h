@@ -1,7 +1,7 @@
 /*
  * bsmm_b200.h -- C ABI of libbsmm_b200.so: block-sparse matmul (fprop / bprop / updat)
  * and block-sparse transformer ops (NT / NN / TN, masked softmax, softmax grad,
- * partial autoregressive mask) for NVIDIA B200 (sm_100a).
+ * partial autoregressive mask) for NVIDIA H100 (sm_90a).
  *
  * This is the drop-in boundary for the hot path of openai/blocksparse.  Each entry
  * point replaces one host launcher that the reference's TensorFlow OpKernels call
@@ -64,13 +64,13 @@ enum {
   BSMM_E_BSIZE   = -2,   /* unsupported block size / axis combination  */
   BSMM_E_ARG     = -3,   /* null pointer, negative size, pcount > 8 …  */
   BSMM_E_LIMIT   = -4,   /* size limit exceeded (mirrors reference OP_REQUIRES) */
-  BSMM_E_NODEV   = -5,   /* no sm_100 device / driver entry point missing */
+  BSMM_E_NODEV   = -5,   /* no sm_90 device / driver entry point missing */
   BSMM_E_ALIGN   = -6    /* pointer or leading dimension not aligned as the tensor-core path needs */
 };
 
 /* flags for bsmm_xprop / bsmm_updat / bst_* */
 enum {
-  BSMM_FLAG_FORCE_GENERIC = 1,   /* use the CUDA-core kernels even where a tcgen05 kernel exists */
+  BSMM_FLAG_FORCE_GENERIC = 1,   /* use the CUDA-core kernels even where a wgmma kernel exists */
   BSMM_FLAG_FORCE_TC      = 2    /* fail (BSMM_E_ARG) instead of falling back to CUDA-core kernels */
 };
 
@@ -81,19 +81,17 @@ int         bsmm_version(void);                 /* 1000*major + minor */
 const char* bsmm_last_error(void);              /* thread-local, never NULL */
 int         bsmm_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* name of the kernel family the last successful call on this thread dispatched to
- * ("tcgen05_xprop_bs32", "fma_xprop", ...) -- used by tests to prove which path ran */
+ * ("wgmma_xprop_bs32", "fma_sdd_xn", ...) -- used by tests to prove which path ran */
 const char* bsmm_last_kernel(void);
 /* Debug aid: synchronises the current device, then returns and clears the sticky device-side error
  * word (non-zero if a tensor-core kernel's bounded barrier wait timed out since the last call). */
 int         bsmm_device_error(void);
-/* Every mbarrier wait inside the tcgen05 kernels is wall-clock bounded.  A wait that exceeds `ms` milliseconds
+/* Every mbarrier wait inside the wgmma kernels is wall-clock bounded.  A wait that exceeds `ms` milliseconds
  * (default 2000) records an error code and, when `trap` is non-zero (default), executes `trap`: the launch fails and
  * the next CUDA call of the host reports the fault, so a starved or mis-sequenced kernel can never return partially
  * written outputs with rc 0.  trap = 0 keeps the context alive (the kernel exits early; poll bsmm_device_error()). */
 int         bsmm_set_wait_timeout_ms(int ms, int trap);
-/* Tuning aid: with BSMM_TRACE set in the environment, CTA 0 of the pair-schedule xprop kernel records clock64() at five
- * pipeline events (producer: stage free, loads issued; issuer: stage full, turn taken, MMAs committed) of its first 256
- * groups; this copies n <= 2048 words (8 per group) of the last launch to `out`. */
+/* Kept for ABI compatibility: no kernel of this build records a pipeline trace, so this always fails (BSMM_E_ARG). */
 int         bsmm_debug_trace(unsigned long long* out, int n);
 
 /* ---- block-sparse matmul -------------------------------------------------------- */
@@ -108,19 +106,15 @@ int         bsmm_debug_trace(unsigned long long* out, int n);
  *    (blocksparse/matmul.py:360,369).
  * lut: row LUT grouped by output block (n_out headers).  Output blocks with no entries are
  *    zero-filled (reference behaviour, cn_64.cu:243-253).
- * sched: optional tile schedule for the tcgen05 kernels built by the host layer
- *    (blocksparse_b200/lut.py:build_tile_schedule, device memory) with its shape passed by value:
- *    sched_tiles output tiles of (sched_tile_blocks & 0xff) consecutive output blocks each (bits 8.. = W blocks
- *    per schedule group when it differs from the default: 2 or 4 select the deeper-pipeline variants used for
- *    layouts below ~12 % / ~37 % density), group records starting at int32 index sched_groups_off; NULL selects
+ * sched: NULL for the default wgmma kernel (it walks `lut`).  Opt-in variants for 32 x 32 blocks and 16-bit dtypes:
+ *    bit 12 of sched_tile_blocks: 2-CTA clusters sharing every W block by TMA multicast (same results, bit for bit);
+ *    bit 16: the wide-tile kernel -- sched = lut.py:build_wide_schedule in device memory with sched_tiles tiles, its
+ *    entries at int32 index sched_groups_off, bits 8..15 the variant (1, 2, 3).
+ * sched_list_off, sched_ctas, sched_ntiles: reserved (ABI compatibility); pass 0.
+ * 16-bit dtypes with block size 16 / 32 / 64 (and N % 8 == 0 for axis 0) run on the wgmma kernel; other calls run on
  *    the CUDA-core kernels.
- *    The persistent CTAs pull tiles from a global counter; sched_list_off > 0 gives the int32 index (inside sched) of an
- *    optional tile ORDER table (tile ids, heaviest first, built for sched_ntiles = ceil(N/128) minibatch tiles).
- *    Pair schedule (32 x 32 blocks, lut.py:build_pair_schedule, opt-in): bit 16 of sched_tile_blocks set; then
- *    sched_list_off indexes the per-CTA tile lists (built for sched_ctas CTAs and sched_ntiles minibatch tiles) and
- *    bits 8..15 select the kernel variant (1 sparse, 2 mid, 3 wide tiles).
  * gate: optional float[blocks]; a zero gate skips the block (cn_64.cu:96-98).  With a gate the call runs on the
- *    CUDA-core kernels; for 16-bit weights call bsmm_gate_weights first and pass gate = NULL to stay on tcgen05.
+ *    CUDA-core kernels; for 16-bit weights call bsmm_gate_weights first and pass gate = NULL to stay on wgmma.
  */
 int bsmm_xprop(int dtype, int axis, int bsize, int bprop,
                const int32_t* lut, int n_out, int n_in, int blocks,
@@ -153,7 +147,7 @@ int bsmm_gate_grad(int dtype, int bsize, int blocks, const void* dw, const void*
                    float* dg, void* stream);
 
 /* w_out[w] = gate[w] * w[w] (zero gate => exact zero block).  Host layers call it before a gated bsmm_xprop of 16-bit
- * weights so that the gated product runs on the tcgen05 kernel: the reference's gated kernels apply the gate to the
+ * weights so that the gated product runs on the wgmma kernel: the reference's gated kernels apply the gate to the
  * loaded weights the same way (cn_64.cu:96-98, blocksparse_hgemm_nc_op_gpu.cu gate handling). */
 int bsmm_gate_weights(int dtype, int bsize, int blocks, const void* w, const float* gate,
                       void* w_out, void* stream);
@@ -165,9 +159,7 @@ int bsmm_gate_weights(int dtype, int bsize, int blocks, const void* w, const flo
  *   a: (batch, ctx_blks_a*bsize, heads*head_state), b: (batch, ctx_blks_b*bsize, heads*head_state)
  *   c: (batch, heads, blocks, bsize, bsize) of c_dtype.
  *   nt_lut: int32 [lut_heads][blocks][2]; lut_heads in {1, heads}.
- *   nt_items / n_items: optional schedule for the tcgen05 kernel (blocksparse_b200/lut.py:build_nt_items, device
- *     int32 [lut_heads][n_items][8] = (k_blk, n_valid, blk0, q0, blk1, q1, 0, 0): blocks sharing a key block, two
- *     at a time); NULL selects the CUDA-core kernel.
+ *   nt_items / n_items: reserved (ABI compatibility, ignored): the wgmma kernel reads nt_lut.
  */
 int bst_nt(int dtype, int c_dtype, int bsize,
            const int32_t* nt_lut, int lut_heads, int blocks,
@@ -180,8 +172,7 @@ int bst_nt(int dtype, int c_dtype, int bsize,
  * XN: transpose_a=0 (NN): C[b, q-blk, h, :] = sum_{(blk,k) in lut[q]} A[b,h,blk]   . B[b, k-blk, h, :]
  *     transpose_a=1 (TN): C[b, k-blk, h, :] = sum_{(blk,q) in lut[k]} A[b,h,blk]^T . B[b, q-blk, h, :]
  *   lut: int32 [lut_heads][ctx_blks_c + blocks][2] -- the reference's nn_lut / tn_lut verbatim.
- *   out_order: optional int32 [lut_heads][ctx_blks_c], output blocks sorted by decreasing LUT row length; the
- *     persistent tcgen05 kernel walks it so that long rows (e.g. strided attention columns) start first.
+ *   out_order: reserved (ABI compatibility, ignored).
  */
 int bst_xn(int a_dtype, int dtype, int bsize, int transpose_a,
            const int32_t* lut, const int32_t* out_order, int lut_heads, int blocks, int max_lut,
@@ -216,7 +207,7 @@ int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int
                             const void* mask_in, void* mask_out, int autoregress_at_key,
                             void* stream);
 
-/* ---- utilities on the (blocks, bsize, bsize) weight format (SURVEY.md 8f) -------------------------------------- */
+/* ---- utilities on the (blocks, bsize, bsize) weight format -------------------------------------- */
 
 /* norm[b] = max|w| (norm_type 0) or sqrt(sum w^2) (norm_type 1) of block b; norm is float[blocks]. */
 int bsmm_block_norm(int dtype, int bsize, int blocks, const void* w, float* norm, int norm_type, void* stream);
@@ -249,7 +240,7 @@ int bsmm_reduced_dw(int dtype, int axis, int bsize, const void* const* xs, const
  * op 1: out[r] = x[r] + (idx[r] >= 0 ? y[idx[r]] : 0);  op 2: out[r] = x[r] * (idx[r] >= 0 ? y[idx[r]] : 1). */
 int bsmm_gather_rows(int dtype, const void* x, const void* y, const int32_t* idx, void* out, int rows, long long N, int op, void* stream);
 
-/* 8 x 8 blocks on tcgen05 (N >= 16 per MMA): scatter a (blocks_small, bs, bs) weight tensor into (blocks_big, 2bs, 2bs)
+/* 8 x 8 blocks on wgmma (K = 16 per MMA step): scatter a (blocks_small, bs, bs) weight tensor into (blocks_big, 2bs, 2bs)
  * super-blocks -- sub_map[4*b + 2*(row half) + (col half)] = small block id or -1 (zero fill), optional per-small-block gate
  * folded in -- and gather the weight gradient back: inv_map[w] = 4 * super-block + sub-position, optional per-block gate
  * (gated dW), accumulate adds to dw_small. */

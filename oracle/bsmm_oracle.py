@@ -9,7 +9,7 @@ Parity status: PINNED.  tests/test_oracle_golden.py checks every function here
 against fixtures in tests/golden/ that were produced by importing the reference's
 own blocksparse/matmul.py (TensorFlow mocked, see tests/golden/make_golden.py).
 
-Reference anchors (relative to /root/reference):
+Reference anchors (relative to the openai/blocksparse source tree):
   blocksparse/utils.py:95-103     z_order_2d
   blocksparse/matmul.py:82-162    BlocksparseMatMul.__init__ (block order, lists)
   blocksparse/matmul.py:172-270   xprop_lut (segments, locks, wire format)
@@ -104,8 +104,8 @@ class MatmulOracle(object):
     """Restatement of BlocksparseMatMul's host state and NumPy checkers.
 
     Block enumeration follows the *intended* behaviour of matmul.py:113-117
-    (blocks discovered in column-major order: sorted by k then c); see
-    SURVEY.md section 3.1 for why modern SciPy needs the explicit sort.
+    (blocks discovered in column-major order: sorted by k then c); modern SciPy's
+    sparse.find no longer returns them in that order, hence the explicit sort.
     """
 
     def __init__(self, layout, block_size=32, feature_axis=0, z_order=True):

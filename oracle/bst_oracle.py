@@ -8,7 +8,7 @@ baseline legs; the product package never imports it.
 Parity status: PINNED against tests/golden/bst_*.npz, produced by importing the
 reference's blocksparse/transformer.py (see tests/golden/make_golden.py).
 
-Reference anchors (relative to /root/reference):
+Reference anchors (relative to the openai/blocksparse source tree):
   blocksparse/transformer.py:61-133    __init__ (nt/nn/tn lists and LUTs)
   blocksparse/transformer.py:135-159   init_softmax_mask (bit packing)
   blocksparse/transformer.py:161-181   xn_lut

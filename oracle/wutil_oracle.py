@@ -1,7 +1,7 @@
 """CPU restatement of the reference's block-sparse weight utilities -- TEST INFRASTRUCTURE ONLY (see oracle/__init__.py:
 only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may import this package).
 
-Each function follows the reference line by line (file:line relative to /root/reference):
+Each function follows the reference line by line (file:line relative to the openai/blocksparse source tree):
   l2_normalize / l2_normalize_grad   blocksparse/matmul.py:421-443 (l2_normalize_test, l2_normalize_grad_test); the gain
                                      variant follows the kernel comment src/blocksparse_l2_norm_op_gpu.cu:704-708
   block_norm / l2_decay / threshold_prune / prune_topk

@@ -1,11 +1,10 @@
 """Generate the golden fixtures in this directory from the REFERENCE implementation.
 
-Run in the build container only (needs /root/reference; it does not exist on the
-GPU box, which consumes the committed .npz files):
+Needs a checkout of openai/blocksparse (the tests only read the committed .npz files):
 
-    python tests/golden/make_golden.py
+    BLOCKSPARSE_REFERENCE=/path/to/blocksparse python tests/golden/make_golden.py
 
-How the reference is imported without TensorFlow (SURVEY.md appendix C.4): a
+How the reference is imported without TensorFlow: a
 MagicMock stands in for `tensorflow` (only graph-building code touches it, none of
 which runs here), and the package __init__ is bypassed so that only
 blocksparse/matmul.py, transformer.py and utils.py are loaded.  Everything the
@@ -34,7 +33,7 @@ from unittest import mock
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference"
+REF = os.environ.get("BLOCKSPARSE_REFERENCE", "")
 
 
 def import_reference():

@@ -66,12 +66,12 @@ def test_cfg2_every_density_bf16(density, axis):
     """BASELINE configs[1]: 4096 x 4096, bs 32, N 4096, bf16, all five densities, both feature axes."""
     rng = np.random.default_rng(1236)
     lay = bernoulli_layout(rng, 128, 128, density)
-    _case(lay, 32, axis, 4096, torch.bfloat16, seed=int(density * 100) + axis, expect="tcgen05_")
+    _case(lay, 32, axis, 4096, torch.bfloat16, seed=int(density * 100) + axis, expect="wgmma_")
 
 
 def test_cfg2_fp16_headline_density():
     rng = np.random.default_rng(1236)
-    _case(bernoulli_layout(rng, 128, 128, 0.25), 32, 1, 4096, torch.float16, seed=7, expect="tcgen05_", tol=(1e-2, 1e-2))
+    _case(bernoulli_layout(rng, 128, 128, 0.25), 32, 1, 4096, torch.float16, seed=7, expect="wgmma_", tol=(1e-2, 1e-2))
 
 
 @pytest.mark.parametrize("density", [0.10, 0.25])
@@ -81,12 +81,12 @@ def test_cfg2_skewed_barabasi_albert(density):
     rng = np.random.default_rng(1237)
     lay = barabasi_albert_layout(128, density, rng)
     assert lay.sum(axis=0).max() >= 3 * lay.sum(axis=0).mean() * 0.6
-    _case(lay, 32, 1, 4096, torch.bfloat16, seed=11, expect="tcgen05_")
+    _case(lay, 32, 1, 4096, torch.bfloat16, seed=11, expect="wgmma_")
 
 
 @pytest.mark.parametrize("bs,axis", [(8, 0), (16, 0), (32, 0), (32, 1), (64, 1)])
 def test_cfg4_block_size_sweep(bs, axis):
-    """BASELINE configs[3]: 4096 x 4096, 20 % density, N 2048, block size 8 / 16 / 32 / 64 (SURVEY 8d axes)."""
+    """BASELINE configs[3]: 4096 x 4096, 20 % density, N 2048, block size 8 / 16 / 32 / 64."""
     rng = np.random.default_rng(1238)
     nb = 4096 // bs
     _case(bernoulli_layout(rng, nb, nb, 0.20), bs, axis, 2048, torch.bfloat16, seed=bs + axis, n_blocks=64)
@@ -117,7 +117,7 @@ def test_cfg3_full_heads_and_batch():
     k_nn = _lib.last_kernel()
     y.backward(E)
     assert _lib.device_error() == 0, _lib.device_error_text()
-    assert k_nt.startswith("tcgen05_bst") and k_nn.startswith("tcgen05_bst")
+    assert k_nt.startswith("wgmma_bst") and k_nn.startswith("wgmma_bst")
     b = batch - 1
     for h in (0, heads - 1):
         sl = slice(h * hs, (h + 1) * hs)

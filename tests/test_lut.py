@@ -241,7 +241,7 @@ def test_updat_schedule_balances_whole_waves():
 
 def test_pick_tile_count_fills_whole_waves():
     from blocksparse_b200.lut import pick_tile_count
-    # BASELINE cfg 2 on a B200 with two CTAs per SM: 32 minibatch tiles, 128 output blocks, 296 CTA slots
+    # BASELINE cfg 2 with 296 CTA slots: 32 minibatch tiles, 128 output blocks
     n_kt = pick_tile_count(128, 32, 296, 8)
     assert n_kt == 18 and 32 * n_kt <= 2 * 296            # 576 tiles: two full waves instead of 512 in 1.73
     assert pick_tile_count(8, 1, 296, 8) == 2             # idle slots: narrower tiles spread a small problem over more CTAs

@@ -115,3 +115,29 @@ def test_pair_tile_schedule_pairs_walk_one_group_list(shape, density, n_kt, wpg,
             assert covered == n_w
     outs, ins, wids = luts._b if bprop else luts._f
     assert sorted(triples) == sorted(zip(outs.tolist(), ins.tolist(), wids.tolist()))
+
+
+@pytest.mark.parametrize("bprop", [0, 1])
+@pytest.mark.parametrize("T", [2, 4])
+def test_wide_schedule_lists_every_block_once_in_input_order(bprop, T):
+    """lut.build_wide_schedule (csrc/tc_xprop2.cuh): every (output block, input block) -> W block of the layout appears in
+    exactly one merged entry of its tile, entries ascend by input block, and nothing else is listed."""
+    from blocksparse_b200.lut import MatmulLuts, WIDE_REC
+    rng = np.random.default_rng(5 + T)
+    lay = (rng.random((9, 37)) < 0.4).astype(np.int32)
+    lay[2, :] = 0
+    L = MatmulLuts(lay)
+    sched, n_tiles, off = L.wide_schedule(bprop, T)
+    outs, ins, wids = L._b if bprop else L._f
+    n_out = lay.shape[0] if bprop else lay.shape[1]
+    assert n_tiles == -(-n_out // T) and off % WIDE_REC == 0 and int(sched[0]) == n_tiles and int(sched[1]) == T
+    got = {}
+    for t in range(n_tiles):
+        rows = [sched[off + WIDE_REC * e: off + WIDE_REC * (e + 1)] for e in range(sched[2 + t], sched[3 + t])]
+        assert [int(r[0]) for r in rows] == sorted({int(r[0]) for r in rows})
+        for r in rows:
+            assert any(r[1:1 + T] >= 0) and all(r[1 + T:] == -1)
+            for j in range(T):
+                if r[1 + j] >= 0:
+                    got[(t * T + j, int(r[0]))] = int(r[1 + j])
+    assert got == {(int(o), int(i)): int(w) for o, i, w in zip(outs, ins, wids)}

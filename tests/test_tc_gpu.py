@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 kernel families (forced with BSMM_FLAG_FORCE_TC so a silent fall-back to the
+"""GPU parity of the wgmma kernel families (forced with BSMM_FLAG_FORCE_TC so a silent fall-back to the
 CUDA-core kernels cannot pass) against the oracle, at sizes the NumPy loops finish in seconds."""
 import numpy as np
 import pytest
@@ -58,8 +58,8 @@ def test_tc_xprop_matches_oracle(case, dtype, axis):
     for name, got_fn, ref in [("fprop", lambda: bsmm.fprop(X.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_TC), orc.fprop_dense(Xn, Wn)),
                               ("bprop", lambda: bsmm.bprop(E.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_TC), orc.bprop_dense(En, Wn))]:
         got = got_fn()
-        assert _lib.device_error() == 0, "a tcgen05 kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
-        assert _lib.last_kernel().startswith("tcgen05_xprop"), _lib.last_kernel()
+        assert _lib.device_error() == 0, "a wgmma kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
+        assert _lib.last_kernel().startswith("wgmma_xprop"), _lib.last_kernel()
         mx, l2 = ref_errors(got.float().cpu().numpy(), ref)
         assert l2 <= (4e-3 if dtype == torch.bfloat16 else 1e-3), "%s l2 %.3e max %.3e" % (name, l2, mx)
         assert mx <= (4e-2 if dtype == torch.bfloat16 else 1e-2), "%s l2 %.3e max %.3e" % (name, l2, mx)
@@ -68,7 +68,7 @@ def test_tc_xprop_matches_oracle(case, dtype, axis):
             bsmm.bprop(E.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_GENERIC)
         diff = (got.float() - gen.float()).abs().max().item()
         scale = gen.float().abs().max().item()
-        assert diff <= scale * 2.0 ** -7, "tcgen05 vs FMA path differ by %g (scale %g)" % (diff, scale)
+        assert diff <= scale * 2.0 ** -7, "wgmma vs FMA path differ by %g (scale %g)" % (diff, scale)
 
 
 def test_tc_xprop_repeatable_and_stream_ordered():
@@ -85,7 +85,7 @@ def test_tc_xprop_repeatable_and_stream_ordered():
 
 @pytest.mark.parametrize("bs", [32, 64])
 def test_gated_xprop_runs_on_tcgen05(bs):
-    """gate folded into a scaled weight copy (bsmm_gate_weights) + tcgen05 kernel == oracle's gated product;
+    """gate folded into a scaled weight copy (bsmm_gate_weights) + wgmma kernel == oracle's gated product;
     zero gates drop their blocks exactly."""
     rng = np.random.default_rng(11)
     lay = layout(rng, 12, 10, 0.4)
@@ -101,9 +101,9 @@ def test_gated_xprop_runs_on_tcgen05(bs):
     Wg = (W.float().numpy() * gate[:, None, None])
     g = torch.as_tensor(gate).cuda()
     y = bsmm.fprop(X.cuda(), W.cuda(), gate=g)
-    assert _lib.last_kernel().startswith("tcgen05_xprop")
+    assert _lib.last_kernel().startswith("wgmma_xprop")
     dx = bsmm.bprop(E.cuda(), W.cuda(), gate=g)
-    assert _lib.last_kernel().startswith("tcgen05_xprop") and _lib.device_error() == 0
+    assert _lib.last_kernel().startswith("wgmma_xprop") and _lib.device_error() == 0
     for got, ref in [(y, orc.fprop_dense(X.float().numpy(), Wg)), (dx, orc.bprop_dense(E.float().numpy(), Wg))]:
         err = np.abs(got.float().cpu().numpy() - ref)
         assert err.max() <= 4e-2 * np.abs(ref).max() and np.sqrt((err ** 2).sum() / (ref ** 2).sum()) <= 1e-2
@@ -147,8 +147,8 @@ def test_tc_updat_matches_oracle(case, dtype, axis):
         ref += orc.updat_dense(X.float().numpy(), E.float().numpy())
     # fp32 output: only the 16-bit INPUT rounding separates us from the oracle (which sees the same rounded inputs)
     dw32 = bsmm.updat(xs, es, dw_dtype=torch.float32, flags=_lib.FLAG_FORCE_TC)
-    assert _lib.device_error() == 0, "a tcgen05 kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
-    assert _lib.last_kernel().startswith("tcgen05_updat"), _lib.last_kernel()
+    assert _lib.device_error() == 0, "a wgmma kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
+    assert _lib.last_kernel().startswith("wgmma_updat"), _lib.last_kernel()
     mx, l2 = ref_errors(dw32.cpu().numpy(), ref)
     assert l2 <= 1e-5 and mx <= 1e-4, "fp32-out updat l2 %.3e max %.3e" % (l2, mx)
     # native-dtype output, alpha, and in-place accumulation (beta = 1)
@@ -168,7 +168,7 @@ def test_tc_updat_matches_oracle(case, dtype, axis):
 
 
 # ------------------------------------------------------------------------------------------------------------
-# block-sparse transformer GEMMs on tcgen05 (block size 64)
+# block-sparse transformer GEMMs on wgmma (block size 64)
 from blocksparse_b200 import BlocksparseTransformer          # noqa: E402
 from oracle.bst_oracle import TransformerOracle               # noqa: E402
 
@@ -215,21 +215,21 @@ def test_tc_bst_gemms_match_oracle(case, dtype):
     tol = 4e-3 if dtype == torch.bfloat16 else 1e-3
     for c_dtype in (torch.float32, torch.bfloat16):
         got = bst._nt(Q.cuda(), K.cuda(), c_dtype, flags=F)
-        assert _lib.device_error() == 0 and _lib.last_kernel() == "tcgen05_bst_nt"
+        assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_nt"
         mx, l2 = ref_errors(got.float().cpu().numpy(), orc.nt(Qn, Kn))
         assert l2 <= (1e-5 if c_dtype == torch.float32 else 4e-3), "nt l2 %.3e" % l2
     got = bst._xn(P.cuda(), V.cuda(), False, flags=F)
-    assert _lib.device_error() == 0 and _lib.last_kernel() == "tcgen05_bst_nn"
+    assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_nn"
     mx, l2 = ref_errors(got.float().cpu().numpy(), orc.nn(Pn, Vn))
     assert l2 <= tol, "nn l2 %.3e" % l2
     got = bst._xn(P.cuda(), DY.cuda(), True, flags=F)
-    assert _lib.device_error() == 0 and _lib.last_kernel() == "tcgen05_bst_tn"
+    assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_tn"
     mx, l2 = ref_errors(got.float().cpu().numpy(), orc.tn(Pn, DYn))
     assert l2 <= tol, "tn l2 %.3e" % l2
 
 
 X2_CASES = [
-    # CB, KB, density, N            (32 x 32 blocks; csrc/tc_xprop2.cuh)
+    # CB, KB, density, N            (32 x 32 blocks; csrc/tc_xprop2.cuh wide tiles)
     (8, 8, 0.3, 128),
     (5, 37, 0.5, 200),            # odd number of input blocks (last pair is half out of range), ragged N
     (7, 20, 1.0, 257),            # dense: every pair-group overflows its W slots and is split
@@ -264,7 +264,7 @@ def test_tc_xprop2_variants_match_oracle(case, dtype, axis, variant, monkeypatch
     for name, fn, inp, ref in [("fprop", bsmm.fprop, X, orc.fprop_dense(Xn, Wn)), ("bprop", bsmm.bprop, E, orc.bprop_dense(En, Wn))]:
         got = fn(inp.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_TC)
         assert _lib.device_error() == 0, _lib.device_error_text()
-        assert _lib.last_kernel() == "tcgen05_xprop2_bs32", _lib.last_kernel()
+        assert _lib.last_kernel() == "wgmma_xprop2_bs32", _lib.last_kernel()
         mx, l2 = ref_errors(got.float().cpu().numpy(), ref)
         # max metric = worst element over MEAN magnitude: the bf16 output rounding alone (2^-9 of the largest element,
         # max/mean ~ 20 for these N(0,1) inputs at 4-10 terms per sum) reaches ~4e-2; the l2 bound is the meaningful one
@@ -314,8 +314,8 @@ def test_cuda_graph_capture_and_replay():
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("case", [(8, 8, 0.3, 128), (40, 33, 0.08, 1), (64, 64, 0.2, 640), (9, 47, 0.3, 200), (128, 128, 0.25, 1024)])
 def test_tc_xprop_pair_tiles_match_oracle(case, dtype, axis, monkeypatch):
-    """2-CTA clusters sharing every activation tile by TMA multicast (BSMM_PAIR_TILES, csrc/tc.cuh CL = 2): same results, bit for
-    bit, as the single-CTA kernel (each output tile still sees its MMAs in ascending input-block order)."""
+    """2-CTA clusters sharing every W block by TMA multicast (BSMM_PAIR_TILES, csrc/tc.cuh CL = 2): same results, bit for
+    bit, as the single-CTA kernel (each output block still sees its MMAs in LUT order)."""
     import blocksparse_b200.matmul as mm
     CB, KB, density, N = case
     if axis == 0:
@@ -332,7 +332,7 @@ def test_tc_xprop_pair_tiles_match_oracle(case, dtype, axis, monkeypatch):
         y = bsmm.fprop(X, W, flags=_lib.FLAG_FORCE_TC); k1 = _lib.last_kernel()
         dx = bsmm.bprop(E, W, flags=_lib.FLAG_FORCE_TC); k2 = _lib.last_kernel()
         assert _lib.device_error() == 0, _lib.device_error_text()
-        assert k1 == k2 == ("tcgen05_xprop_bs32_pair" if pair else "tcgen05_xprop_bs32"), (k1, k2)
+        assert k1 == k2 == ("wgmma_xprop_bs32_pair" if pair else "wgmma_xprop_bs32"), (k1, k2)
         res[pair] = (y, dx)
     assert torch.equal(res[0][0], res[1][0]) and torch.equal(res[0][1], res[1][1])
     orc = MatmulOracle(lay, 32, axis)
@@ -343,7 +343,7 @@ def test_tc_xprop_pair_tiles_match_oracle(case, dtype, axis, monkeypatch):
 @pytest.mark.parametrize("axis", [0, 1])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 def test_bs8_runs_padded_on_tcgen05(dtype, axis):
-    """8 x 8 blocks: 2 x 2 neighbourhoods padded into 16 x 16 super-blocks (csrc/wutil.cuh pad/unpad) and run by the tcgen05
+    """8 x 8 blocks: 2 x 2 neighbourhoods padded into 16 x 16 super-blocks (csrc/wutil.cuh pad/unpad) and run by the wgmma
     kernels; fprop / bprop / updat (alpha, accumulate, gate) against the oracle and against the CUDA-core path."""
     rng = np.random.default_rng(8 + axis)
     lay = layout(rng, 20, 14, 0.3, empty_col=3, empty_row=5)
@@ -362,7 +362,7 @@ def test_bs8_runs_padded_on_tcgen05(dtype, axis):
     for name, got, ref in [("fprop", bsmm.fprop(X.cuda(), W.cuda()), orc.fprop_dense(Xn, Wn)),
                            ("bprop", bsmm.bprop(E.cuda(), W.cuda()), orc.bprop_dense(En, Wn)),
                            ("fprop gated", bsmm.fprop(X.cuda(), W.cuda(), gate=g), orc.fprop_dense(Xn, Wn * gate[:, None, None]))]:
-        assert _lib.last_kernel() == "tcgen05_xprop_bs16", _lib.last_kernel()
+        assert _lib.last_kernel() == "wgmma_xprop_bs16", _lib.last_kernel()
         mx, l2 = ref_errors(got.float().cpu().numpy(), ref)
         assert l2 <= tol, "%s l2 %.3e" % (name, l2)
     ref_dw = orc.updat_dense(Xn, En)

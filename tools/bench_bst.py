@@ -1,6 +1,6 @@
 """BASELINE cfg 3: block-sparse attention ops, heads 16, ctx 4096, bs 64, local+strided causal layout, batch 4.
 
-Prints one JSON line per op with CUDA-event time, algorithmic bytes/flops (SURVEY section 8d) and the fraction of
+Prints one JSON line per op with CUDA-event time, algorithmic bytes/flops and the fraction of
 the measured HBM / tensor peaks (MEASURED_PEAKS.json)."""
 import json
 import sys

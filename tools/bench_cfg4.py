@@ -1,5 +1,5 @@
 """BASELINE cfg 4: block-size sweep {8,16,32,64} at 4096x4096, density 20 %, N=2048, bf16 -- which kernel family runs
-each (axis, block size) and how fast (CUDA-core FMA vs tcgen05 crossover)."""
+each (axis, block size) and how fast (CUDA-core FMA vs wgmma crossover)."""
 import json
 import sys
 

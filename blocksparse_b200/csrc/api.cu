@@ -275,6 +275,8 @@ int bst_softmax(int x_dtype, int y_dtype, int bsize,
                 int batch, int heads, int ctx_blks_q, void* stream) {
   if (int e = check_bst(bsize, lut_heads, heads, 8, batch, blocks)) return e;
   if (!nn_lut || !x || !y) return fail(BSMM_E_ARG, "bst_softmax: null pointer");
+  // the register kernel loads up to 16 bytes per lane (uint4 of 16-bit data at bs 32/64), the staged one bulk-copies
+  if (((uintptr_t)x | (uintptr_t)y) & 15) return fail(BSMM_E_ARG, "bst_softmax: x and y must be 16-byte aligned");
   if ((long long)max_lut * bsize > 32768) return fail(BSMM_E_LIMIT, "bst_softmax: max_lut*bsize > 32768 (bst_op.cc:383)");
   if (autoregress_at_key >= 0 && (!mask || !nt_lut))
     return fail(BSMM_E_ARG, "bst_softmax: autoregress_at_key needs a mask and nt_lut");
@@ -291,7 +293,7 @@ int bst_softmax(int x_dtype, int y_dtype, int bsize,
   // TMA-staged kernel: 16-bit tensors, 32 x 32 / 64 x 64 blocks, every row's blocks fit shared memory (<= 16 of them)
   static const bool no_staged = [] { const char* e = getenv("BSMM_SOFTMAX_STAGED"); return e && atoi(e) == 0; }();
   if (!no_staged && x_dtype != BSMM_F32 && y_dtype != BSMM_F32 && (bsize == 32 || bsize == 64) && max_lut >= 1 && max_lut <= 16 &&
-      (((uintptr_t)x | (uintptr_t)y) & 15) == 0 && device_info().ok && device_info().cc_major >= 9) {
+      device_info().ok && device_info().cc_major >= 9) {
 #define BSMM_SM_STAGED(TXT, TYT)                                                                              \
     return bsize == 64 ? launch_softmax_staged<TXT, TYT, 64>(p, max_lut, s) : launch_softmax_staged<TXT, TYT, 32>(p, max_lut, s);
     if (x_dtype == BSMM_BF16 && y_dtype == BSMM_BF16) { BSMM_SM_STAGED(__nv_bfloat16, __nv_bfloat16) }
@@ -318,6 +320,8 @@ int bst_softmax_grad(int dtype, int dx_dtype, int bsize,
                      int batch, int heads, int ctx_blks_q, void* stream) {
   if (int e = check_bst(bsize, lut_heads, heads, 8, batch, blocks)) return e;
   if (!nn_lut || !dy || !y || !dx) return fail(BSMM_E_ARG, "bst_softmax_grad: null pointer");
+  if (((uintptr_t)dy | (uintptr_t)y | (uintptr_t)dx) & 15)
+    return fail(BSMM_E_ARG, "bst_softmax_grad: dy, y and dx must be 16-byte aligned");
   if ((long long)max_lut * bsize > 32768) return fail(BSMM_E_LIMIT, "bst_softmax_grad: max_lut*bsize > 32768");
   cudaStream_t s = (cudaStream_t)stream;
   SoftmaxParams p = {};
@@ -327,7 +331,7 @@ int bst_softmax_grad(int dtype, int dx_dtype, int bsize,
   p.batch = batch; p.heads = heads; p.blocks = blocks; p.ctx_blks_q = ctx_blks_q;
   static const bool no_staged = [] { const char* e = getenv("BSMM_SOFTMAX_STAGED"); return e && atoi(e) == 0; }();
   if (!no_staged && dtype != BSMM_F32 && dx_dtype != BSMM_F32 && (bsize == 32 || bsize == 64) && max_lut >= 1 && max_lut <= 16 &&
-      (((uintptr_t)dy | (uintptr_t)y | (uintptr_t)dx) & 15) == 0 && device_info().ok && device_info().cc_major >= 9) {
+      device_info().ok && device_info().cc_major >= 9) {
 #define BSMM_SG_STAGED(TT, TDT)                                                                               \
     return bsize == 64 ? launch_softmax_grad_staged<TT, TDT, 64>(p, max_lut, s) : launch_softmax_grad_staged<TT, TDT, 32>(p, max_lut, s);
     if (dtype == BSMM_BF16 && dx_dtype == BSMM_BF16) { BSMM_SG_STAGED(__nv_bfloat16, __nv_bfloat16) }

@@ -16,6 +16,13 @@ from .checkers import TransformerCheckers
 from .lut import TransformerLuts
 
 
+def _aligned(t):
+    """Contiguous `t` starting on a 16-byte boundary, which the softmax kernels' vector loads need. A view at an odd
+    offset into a larger buffer is legal torch; it gets a fresh copy."""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
 class BlocksparseTransformer(TransformerCheckers):
     """Drop-in for blocksparse.transformer.BlocksparseTransformer (reference transformer.py:51)."""
 
@@ -123,7 +130,7 @@ class BlocksparseTransformer(TransformerCheckers):
     @_lib.guarded
     def _softmax(self, x, scale, use_mask, autoregress_at_key, dtype):
         lib = _lib.load()
-        x = x.contiguous()
+        x = _aligned(x)
         batch = x.shape[0]
         y = torch.empty(x.shape, dtype=dtype, device=x.device)
         d = self._device_luts(x.device)
@@ -140,8 +147,8 @@ class BlocksparseTransformer(TransformerCheckers):
     @_lib.guarded
     def _softmax_grad(self, dy, y, scale):
         lib = _lib.load()
-        dy = dy.to(y.dtype).contiguous()
-        y = y.contiguous()
+        dy = _aligned(dy.to(y.dtype))
+        y = _aligned(y)
         dx = torch.empty_like(dy)
         d = self._device_luts(y.device)
         rc = lib.bst_softmax_grad(_lib.dtype_code(y.dtype), _lib.dtype_code(dx.dtype), self.blk_size,

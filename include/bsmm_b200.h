@@ -189,6 +189,7 @@ int bst_xn(int a_dtype, int dtype, int bsize, int transpose_a,
  *   autoregress_at_key >= 0 applies the partial-autoregressive rewrite on the fly
  *         (blocksparse/transformer.py:264-274); nt_lut is then required.
  * Limit: max_lut * bsize <= 32768 (bst_op.cc:383).
+ * x and y must be 16-byte aligned (BSMM_E_ARG otherwise); so must dy, y and dx of bst_softmax_grad.
  */
 int bst_softmax(int x_dtype, int y_dtype, int bsize,
                 const int32_t* nn_lut, const int32_t* nt_lut, int lut_heads, int blocks, int max_lut,

@@ -47,3 +47,18 @@ def test_argument_errors_are_reported_without_a_gpu():
     assert rc == -3
     with pytest.raises(ValueError):
         _lib.check(rc, "bsmm_xprop")
+
+
+def test_softmax_refuses_misaligned_pointers_before_any_launch():
+    """Both softmax kernels load 16-byte vectors, so any operand that does not start on a 16-byte boundary is refused
+    on the host. The pointers below are never dereferenced: the call must fail before touching the device."""
+    lib = _lib.load()
+    before = _lib.last_kernel()
+    lut, a, b, c = 0x1000, 0x10000, 0x20000, 0x30000
+    for dt, x, y in [(_lib.BF16, a + 2, b), (_lib.F16, a, b + 2), (_lib.F32, a + 8, b), (_lib.BF16, a + 14, b + 6)]:
+        rc = lib.bst_softmax(dt, dt, 64, lut, None, 1, 4, 2, None, 1, -1, x, y, 1.0, 1, 1, 2, None)
+        assert rc == -3 and b"16-byte aligned" in lib.bsmm_last_error(), (rc, lib.bsmm_last_error())
+    for dt, dy, y, dx in [(_lib.BF16, a + 2, b, c), (_lib.F16, a, b + 4, c), (_lib.F32, a, b, c + 8), (_lib.F16, a + 1, b, c)]:
+        rc = lib.bst_softmax_grad(dt, dt, 32, lut, 1, 4, 2, dy, y, dx, 1.0, 1, 1, 2, None)
+        assert rc == -3 and b"16-byte aligned" in lib.bsmm_last_error(), (rc, lib.bsmm_last_error())
+    assert _lib.last_kernel() == before          # nothing was launched

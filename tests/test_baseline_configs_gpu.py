@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests._util import ref_errors
+from tests._util import U_OUT, fma_gemm_bound, ref_errors, softmax_grad_bound, softmax_row_sums
 from blocksparse_b200 import BlocksparseMatMul, BlocksparseTransformer, _lib
 from blocksparse_b200.layouts import bernoulli_layout, barabasi_albert_layout, local_strided_layout
 from oracle.bsmm_oracle import MatmulOracle
@@ -94,7 +94,8 @@ def test_cfg4_block_size_sweep(bs, axis):
 
 def test_cfg3_full_heads_and_batch():
     """BASELINE configs[2]: heads 16, ctx 4096, bs 64, batch 4, head_state 64, fp16, causal local+strided layout.
-    Forward chain and both backward GEMMs against the oracle on (batch 3, heads 0 and 15)."""
+    Forward chain and the whole backward (dv, the softmax gradient, dq, dk) against the oracle on (batch 3, heads 0
+    and 15), and which kernel ran each backward op."""
     nb, bs, heads, hs, batch = 64, 64, 16, 64, 4
     lay = local_strided_layout(nb)
 
@@ -106,6 +107,15 @@ def test_cfg3_full_heads_and_batch():
 
     bst = BlocksparseTransformer(lay, bs, heads=heads, mask_callback=causal)
     assert (bst.blocks, bst.nn_max, bst.tn_max) == (453, 11, 57)
+    # record the kernel behind every raw op of the backward, with its operand dtypes
+    seen = []
+
+    def logged(fn, op):
+        def run(*args, **kw):
+            out = fn(*args, **kw)
+            seen.append((op, args[0].dtype, args[1].dtype, _lib.last_kernel()))
+            return out
+        return run
     gen = torch.Generator(device="cuda").manual_seed(5)
     Q, K, V, E = ((torch.rand((batch, nb * bs, heads * hs), generator=gen, device="cuda") * 2 - 1).half() for _ in range(4))
     scale = 1.0 / np.sqrt(hs)
@@ -113,11 +123,23 @@ def test_cfg3_full_heads_and_batch():
     w = bst.query_key_op(Q, K)
     k_nt = _lib.last_kernel()
     p = bst.masked_softmax(w, scale=scale)
+    k_sm = _lib.last_kernel()
     y = bst.weight_value_op(p, V)
     k_nn = _lib.last_kernel()
+    grads = {}
+    w.register_hook(lambda g: grads.__setitem__("ds", g))       # softmax grad, cast back to the scores' bf16
+    p.register_hook(lambda g: grads.__setitem__("dp", g))       # upstream gradient of the probabilities (fp16)
+    bst._xn, bst._softmax_grad = logged(bst._xn, "xn"), logged(bst._softmax_grad, "softmax_grad")
     y.backward(E)
     assert _lib.device_error() == 0, _lib.device_error_text()
     assert k_nt.startswith("wgmma_bst") and k_nn.startswith("wgmma_bst")
+    assert k_sm == "bst_softmax_staged"                                         # rows of <= 11 blocks: MAXE 12
+    assert grads["ds"].dtype == torch.bfloat16 and grads["dp"].dtype == torch.float16
+    # dv: fp16 x fp16 on wgmma; the softmax grad on the staged kernel (MAXE 12); dq / dk: bf16 dS x fp16 Q / K, which
+    # the wgmma kernels refuse, on the CUDA-core kernel
+    f16, b16 = torch.float16, torch.bfloat16
+    assert seen == [("xn", f16, f16, "wgmma_bst_tn"), ("softmax_grad", f16, f16, "bst_softmax_grad_staged"),
+                    ("xn", b16, f16, "fma_sdd_xn"), ("xn", b16, f16, "fma_sdd_xn")], seen
     b = batch - 1
     for h in (0, heads - 1):
         sl = slice(h * hs, (h + 1) * hs)
@@ -134,4 +156,31 @@ def test_cfg3_full_heads_and_batch():
                                     (y[b:b + 1, :, sl], Y, "y", (1.5e-1, 1e-2)),
                                     (V.grad[b:b + 1, :, sl], DV, "dv", (1.5e-1, 1e-2))]:
             mx, l2 = ref_errors(got.detach().float().cpu().numpy().reshape(ref.shape), ref)
+            assert mx <= tol[0] and l2 <= tol[1], "head %d %s: max %.3e l2 %.3e" % (h, what, mx, l2)
+
+        # backward through the softmax, elementwise, at the op's own intermediates of this slice
+        Pk = p[b:b + 1, h:h + 1].detach().double().cpu().numpy()
+        dPk = grads["dp"][b:b + 1, h:h + 1].double().cpu().numpy()
+        dSk = grads["ds"][b:b + 1, h:h + 1].double().cpu().numpy()
+        DSk = orc.masked_softmax_grad(dPk, Pk, scale=scale)                    # float64
+        bound = softmax_grad_bound(DSk, dPk, Pk, softmax_row_sums(np.abs(dPk * Pk), orc), "float16", scale, bst.nn_max)
+        bound += U_OUT["bfloat16"] * (np.abs(DSk) + bound)                     # fp16 result cast to bf16 for the NT backward
+        err = np.abs(dSk - DSk)
+        assert np.all(err <= bound), "head %d softmax grad: %d out of bound" % (h, int((err > bound).sum()))
+        dS32 = dSk.astype(np.float32)
+        for got, op, dense, k_terms, what in [(Q.grad, orc.nn, Kh, bst.nn_max * bs, "dq"), (K.grad, orc.tn, Qh, bst.tn_max * bs, "dk")]:
+            ref = op(dS32, dense)
+            g = got[b:b + 1, :, sl].double().cpu().numpy()
+            bound = fma_gemm_bound(ref.astype(np.float64), op(np.abs(dS32), np.abs(dense)).astype(np.float64), "float16", k_terms)
+            err = np.abs(g - ref)
+            assert np.all(err <= bound), "head %d %s: %d out of bound" % (h, what, int((err > bound).sum()))
+        # and the whole backward against the oracle chain on its own 16-bit-rounded intermediates
+        DP16 = torch.as_tensor(orc.nt(Eh, Vh)).half().float().numpy()
+        DS16 = torch.as_tensor(orc.masked_softmax_grad(DP16, P16, scale=scale)).to(torch.bfloat16).float().numpy()
+        # probabilities and their gradients are peaked per row, so the max metric (over the MEAN magnitude) says little
+        # about dS: its l2 only; dq / dk are three 16-bit roundings deep, as in the golden chain test
+        for got, ref, what, tol in [(grads["ds"][b:b + 1, h:h + 1], DS16, "ds", (np.inf, 1e-2)),
+                                    (Q.grad[b:b + 1, :, sl], orc.nn(DS16, Kh), "dq", (2e-1, 2e-2)),
+                                    (K.grad[b:b + 1, :, sl], orc.tn(DS16, Qh), "dk", (2e-1, 2e-2))]:
+            mx, l2 = ref_errors(got.float().cpu().numpy().reshape(ref.shape), ref)
             assert mx <= tol[0] and l2 <= tol[1], "head %d %s: max %.3e l2 %.3e" % (h, what, mx, l2)

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests._util import ref_errors
+from tests._util import fma_gemm_bound, ref_errors
 from blocksparse_b200 import BlocksparseMatMul, _lib
 from oracle.bsmm_oracle import MatmulOracle
 
@@ -173,37 +173,74 @@ from blocksparse_b200 import BlocksparseTransformer          # noqa: E402
 from oracle.bst_oracle import TransformerOracle               # noqa: E402
 
 
-def _bst_layout(rng, heads_l, qb, kb, density):
+def _bst_layout(rng, heads_l, qb, kb, density, empty_q=(), empty_k=()):
+    """Random per-head layouts with equal block counts (reference requirement); query blocks `empty_q` hold no key
+    block and key blocks `empty_k` no query block in any head."""
     lay = (rng.random((heads_l, qb, kb)) < density).astype(np.int32)
     for h in range(heads_l):
         for q in range(qb):
             lay[h, q, (q + h) % kb] = 1
-    # equal block count across heads (reference requirement): top up the sparser heads
+    lay[:, list(empty_q), :] = 0
+    lay[:, :, list(empty_k)] = 0
+    # equal block count across heads: top up the sparser heads, outside the empty rows and columns
     target = int(lay.reshape(heads_l, -1).sum(1).max())
     for h in range(heads_l):
         free = np.argwhere(lay[h] == 0)
+        free = free[~np.isin(free[:, 0], list(empty_q)) & ~np.isin(free[:, 1], list(empty_k))]
         rng.shuffle(free)
         for q, k in free[: target - int(lay[h].sum())]:
             lay[h, q, k] = 1
     return lay
 
 
+def _on_poisoned_output(fn, shape, dtype, tries=8):
+    """Run fn(), whose output is a fresh torch.empty(shape, dtype), on memory just filled with NaN: a tensor of that
+    size is filled and freed, and the caching allocator hands the block back to the next allocation of that size, so
+    an element the kernel never writes shows up as NaN. Should the allocator pick another free block instead (it
+    prefers the best fit, and the freed block may have merged with a neighbour), that output is kept alive, so the
+    next try cannot get it again."""
+    held = []
+    for _ in range(tries):
+        t = torch.full(shape, float("nan"), dtype=dtype, device="cuda")
+        ptr = t.data_ptr()
+        del t
+        c = fn()
+        if c.data_ptr() == ptr:
+            return c
+        held.append(c)
+    raise AssertionError("the output never landed on the NaN-filled block")
+
+
+def _assert_zero_blocks(c, empty, bs, what):
+    """rows of the dense output that belong to the given context blocks are exactly 0 (no NaN left from _poison_next)"""
+    for blk in empty:
+        v = c[:, blk * bs:(blk + 1) * bs]
+        assert bool((v == 0).all()), "%s: output block %d is not zero-filled (max %s)" % (what, blk, v.float().abs().max().item())
+
+
 BST_CASES = [
-    # lut_heads, heads, q_blks, k_blks, density, head_state, batch
-    (1, 2, 4, 4, 0.6, 64, 2),
-    (1, 3, 5, 7, 0.4, 64, 1),        # rectangular, odd number of blocks per key column
-    (2, 2, 6, 5, 0.5, 128, 2),       # per-head layouts, head_state 128 (two column atoms)
-    (1, 4, 16, 16, 0.3, 64, 1),
+    # lut_heads, heads, q_blks, k_blks, density, head_state, batch, (empty query blocks, empty key blocks)
+    (1, 2, 4, 4, 0.6, 64, 2, None),
+    (1, 3, 5, 7, 0.4, 64, 1, None),        # rectangular, odd number of blocks per key column
+    (2, 2, 6, 5, 0.5, 128, 2, None),       # per-head layouts, head_state 128 (two column atoms)
+    (1, 4, 16, 16, 0.3, 64, 1, None),
+    (4, 4, 6, 7, 0.4, 64, 2, None),        # a layout per head at head_state 64
+    (1, 2, 5, 6, 0.5, 128, 1, None),       # shared layout at head_state 128
+    (1, 2, 12, 12, 0.85, 64, 1, None),     # rows of 9+ blocks: the 4-stage ring wraps more than twice
+    (2, 2, 7, 6, 0.5, 64, 2, ((1, 4), (2,))),   # empty query rows (NN zero-fill) and an empty key column (TN zero-fill)
 ]
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("case", BST_CASES)
 def test_tc_bst_gemms_match_oracle(case, dtype):
-    lh, heads, qb, kb, density, hs, batch = case
+    lh, heads, qb, kb, density, hs, batch, holes = case
     rng = np.random.default_rng(lh * 100 + heads * 10 + qb)
-    lay = _bst_layout(rng, lh, qb, kb, density)
+    empty_q, empty_k = holes or ((), ())
+    lay = _bst_layout(rng, lh, qb, kb, density, empty_q, empty_k)
     bst = BlocksparseTransformer(lay if lh > 1 else lay[0], 64, heads=heads)
+    if density > 0.8:
+        assert bst.nn_max > 8 and bst.tn_max > 8
     orc = TransformerOracle(lay if lh > 1 else lay[0], 64, heads=heads)
     S = heads * hs
     mk = lambda *shape: torch.as_tensor(rng.uniform(-1, 1, shape).astype(np.float32)).to(dtype)
@@ -226,6 +263,70 @@ def test_tc_bst_gemms_match_oracle(case, dtype):
     assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_tn"
     mx, l2 = ref_errors(got.float().cpu().numpy(), orc.tn(Pn, DYn))
     assert l2 <= tol, "tn l2 %.3e" % l2
+    if holes:
+        Pd, Vd, DYd = P.cuda(), V.cuda(), DY.cuda()
+        for transpose, dense, empty, what in [(False, Vd, empty_q, "nn"), (True, DYd, empty_k, "tn")]:
+            shape = (batch, (kb if transpose else qb) * 64, S)
+            c = _on_poisoned_output(lambda: bst._xn(Pd, dense, transpose, flags=F), shape, dtype)
+            assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_" + what
+            _assert_zero_blocks(c, empty, 64, what)
+
+
+FMA_CASES = [
+    # bs, head_state, flags, sparse dtype, dense dtype: the CUDA-core NT / NN / TN kernels in 16-bit
+    (8, 32, 0, torch.bfloat16, torch.bfloat16),
+    (16, 64, 0, torch.float16, torch.float16),
+    (32, 64, 0, torch.bfloat16, torch.bfloat16),
+    (64, 32, 0, torch.float16, torch.float16),
+    (64, 96, 0, torch.bfloat16, torch.bfloat16),
+    (64, 256, 0, torch.float16, torch.float16),
+    (64, 64, _lib.FLAG_FORCE_GENERIC, torch.bfloat16, torch.bfloat16),
+    (64, 64, 0, torch.bfloat16, torch.float16),    # bf16 scores x fp16 Q / K: the fp16 attention backward's dq / dk
+]
+
+
+@pytest.mark.parametrize("case", FMA_CASES)
+def test_fma_bst_gemms_match_oracle(case):
+    """The CUDA-core attention GEMMs, elementwise against the oracle: NT (fma_dds_nt) and NN / TN (fma_sdd_xn),
+    with empty query rows and an empty key column whose output rows must be zero-filled."""
+    bs, hs, flags, a_dtype, dtype = case
+    heads, batch, qb, kb = 2, 2, 7, 6
+    rng = np.random.default_rng(bs * 1000 + hs)
+    empty_q, empty_k = (1, 4), (2,)
+    lay = _bst_layout(rng, 2, qb, kb, 0.5, empty_q, empty_k)
+    bst = BlocksparseTransformer(lay, bs, heads=heads)
+    orc = TransformerOracle(lay, bs, heads=heads)
+    S = heads * hs
+    mk = lambda dt, *shape: torch.as_tensor(rng.uniform(-1, 1, shape).astype(np.float32)).to(dt)
+    Q, K, DY = mk(dtype, batch, qb * bs, S), mk(dtype, batch, kb * bs, S), mk(dtype, batch, qb * bs, S)
+    P = mk(a_dtype, batch, heads, bst.blocks, bs, bs)
+    Qn, Kn, DYn, Pn = (t.float().numpy() for t in (Q, K, DY, P))
+    Qd, Kd, DYd, Pd = Q.cuda(), K.cuda(), DY.cuda(), P.cuda()
+    name = lambda dt: str(dt).replace("torch.", "")
+
+    def check(got, ref, ref_abs, k_terms, what):
+        g = got.double().cpu().numpy().reshape(ref.shape)
+        bound = fma_gemm_bound(ref.astype(np.float64), ref_abs.astype(np.float64), name(got.dtype), k_terms)
+        err = np.abs(g - ref)
+        assert np.all(err <= bound), "%s: %d elements out of bound, worst excess %.3e" % (
+            what, int((err > bound).sum()), float((err - bound).max()))
+
+    if a_dtype == dtype:            # NT takes one dtype for both dense operands
+        for c_dtype in (torch.float32, torch.bfloat16):
+            got = bst._nt(Qd, Kd, c_dtype, flags=flags)
+            assert _lib.device_error() == 0 and _lib.last_kernel() == "fma_dds_nt", _lib.last_kernel()
+            check(got, orc.nt(Qn, Kn), orc.nt(np.abs(Qn), np.abs(Kn)), hs, "nt")
+    for transpose, dense, dn, empty, lmax, what in [(False, Kd, Kn, empty_q, bst.nn_max, "nn"),
+                                                    (True, DYd, DYn, empty_k, bst.tn_max, "tn")]:
+        bst._xn(Pd, dense, transpose, flags=flags)              # first call builds the device LUTs
+        got = _on_poisoned_output(lambda: bst._xn(Pd, dense, transpose, flags=flags),
+                                  (batch, (kb if transpose else qb) * bs, S), dtype)
+        assert _lib.device_error() == 0 and _lib.last_kernel() == "fma_sdd_xn", _lib.last_kernel()
+        assert got.dtype == dtype
+        op = orc.tn if transpose else orc.nn
+        ref, ref_abs = op(Pn, dn), op(np.abs(Pn), np.abs(dn))
+        check(got, ref, ref_abs, lmax * bs, what)
+        _assert_zero_blocks(got, empty, bs, what)
 
 
 X2_CASES = [

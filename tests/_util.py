@@ -1,7 +1,9 @@
 """Shared helpers for the test-suite."""
+import json
 import os
 
 import numpy as np
+import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
@@ -36,6 +38,10 @@ def softmax_row_sums(a, orc):
     return out
 
 
+def dtype_name(dtype):
+    """"bfloat16" for torch.bfloat16: the keys of U_OUT."""
+    return str(dtype).replace("torch.", "")
+
 
 EPS32 = 2.0 ** -24                    # unit roundoff of fp32
 # unit roundoff of one round-to-nearest conversion to a storage dtype, by name: "bfloat16", "float16", "float32"
@@ -62,3 +68,120 @@ def fma_gemm_bound(ref, ref_abs, out_dtype, k_terms):
     computed value (relative u_out, applied to ref plus that error) and 2^-25 for fp16 subnormals."""
     u = U_OUT[out_dtype]
     return u * np.abs(ref) + k_terms * 2.0 ** -23 * (1 + u) * ref_abs + 2.0 ** -25
+
+
+# Units of eps32 * |a b| that one product of a wgmma GEMM may lose in its fp32 accumulation. Products of 16-bit values
+# are exact in fp32, but the tensor cores do not round each addition to nearest: published models of Hopper's MMA align
+# a group of products to the largest exponent and truncate. 4 allows two fp32 units per term; it is an assumption, not
+# a derivation, so the checks below can log the worst ratio they see (BSMM_BOUND_LOG) to keep it honest. Measured with
+# the GPU suite on an H100 80GB HBM3 (700 W power limit), the worst ratios were 0.11 for the fp32-output updat, where
+# the accumulation shows directly; 0.77 with its alpha / gate / beta roundings, which the unit leaves out; and <= 0.05
+# for the 16-bit outputs (xprop, xprop2, pair tiles, updat), whose own rounding hides most of it.
+MMA_C = 4
+
+
+def mma_gemm_bound(ref, ref_abs, out_dtype, k_terms, extra=0):
+    """Largest |got - ref| of a wgmma (tensor-core, fp32-accumulating) block-sparse GEMM, elementwise, built like
+    fma_gemm_bound: one output rounding, MMA_C eps32 per accumulated term (k_terms per output element: bs x the LUT
+    entries the kernel walks for its block, or the minibatch x pairs for updat), the fp16 subnormal floor. `extra`
+    counts the fp32 roundings of the epilogue (alpha, gate, beta: one each), each at most eps32 * ref_abs. For an
+    accumulating call, ref_abs includes |old value|."""
+    u = U_OUT[out_dtype]
+    return u * np.abs(ref) + (k_terms * MMA_C * EPS32 * (1 + u) + extra * EPS32) * ref_abs + 2.0 ** -25
+
+
+def assert_within(got, ref, bound, what, ref_abs=None, k_terms=None, out_dtype=None, family=None):
+    """Every element of got (tensor or array) lies within bound of the float64 ref.
+
+    With family, ref_abs, k_terms and out_dtype given and BSMM_BOUND_LOG naming a file, one JSON line is appended with
+    the worst accumulation error seen, in units of k_terms * eps32 * ref_abs: the part of |got - ref| that the output
+    rounding cannot explain. That is the number MMA_C has to stay above."""
+    if hasattr(got, "detach"):
+        got = got.detach().double().cpu().numpy()
+    g = np.asarray(got, dtype=np.float64).reshape(np.shape(ref))
+    err = np.abs(g - ref)
+    log = os.environ.get("BSMM_BOUND_LOG")
+    if log and family and ref_abs is not None:
+        excess = np.maximum(err - U_OUT[out_dtype] * np.abs(ref) - 2.0 ** -25, 0.0)
+        unit = np.broadcast_to(k_terms * EPS32 * ref_abs, err.shape)
+        ratio = float(np.max(np.where(unit > 0, excess / np.where(unit > 0, unit, 1.0), 0.0), initial=0.0))
+        with open(log, "a") as f:
+            f.write(json.dumps({"family": family, "what": what, "ratio": ratio}) + "\n")
+    bad = ~(err <= bound)
+    assert not bad.any(), "%s: %d of %d elements out of bound, worst excess %.3e (err %.3e)" % (
+        what, int(bad.sum()), bad.size, float(np.nanmax(np.where(bad, err - bound, -np.inf))), float(np.nanmax(err)))
+
+
+def oracle_dense(orc, op, a, b):
+    """MatmulOracle.fprop_dense / bprop_dense / updat_dense in float64 ("fprop" / "bprop": a = activations, b = W;
+    "updat": a = X, b = DY), the same dense restatement evaluated through BLAS instead of einsum loops."""
+    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
+    if op == "updat":
+        full = a.T @ b if orc.axis else a @ b.T
+        bs = orc.bsize
+        return full.reshape(orc.C // bs, bs, orc.K // bs, bs)[orc.updat_lut[:, 0], :, orc.updat_lut[:, 1], :]
+    D = orc.dense_weight(b)
+    if op == "fprop":
+        return a @ D if orc.axis else D.T @ a
+    return a @ D.T if orc.axis else D @ a
+
+
+def feature_terms(layout, bs, bprop, axis):
+    """k_terms of a single-block-per-CTA xprop, broadcastable against its (n_out*bs, N) or (N, n_out*bs) output:
+    bs x the LUT row length of every output block (column counts for fprop, row counts for bprop)."""
+    lay = np.asarray(layout) != 0
+    counts = lay.sum(axis=1 if bprop else 0)
+    kf = np.repeat(counts * bs, bs).astype(np.float64)
+    return kf[None, :] if axis else kf[:, None]
+
+
+def out_block(y, blk, bs, axis):
+    """Output feature block blk of a dense (features on `axis`) matmul result."""
+    return y[:, blk * bs:(blk + 1) * bs] if axis else y[blk * bs:(blk + 1) * bs]
+
+
+def assert_zero_filled(y, empty, bs, axis, what):
+    """A kernel wrote every element of y (fresh from _on_poisoned_output: no NaN is left) and the output blocks whose
+    LUT row is empty are exactly zero."""
+    assert not bool(torch.isnan(y).any()), "%s: %d elements never written" % (what, int(torch.isnan(y).sum()))
+    for blk in empty:
+        v = out_block(y, int(blk), bs, axis)
+        assert bool((v == 0).all()), "%s: output block %d is not zero-filled (max %s)" % (what, blk, v.float().abs().max().item())
+
+
+def record_kernels(monkeypatch, obj, names, seen):
+    """Wrap the methods `names` of obj so that every call appends (name, kernel it launched last) to seen. The library
+    keeps the last kernel's name per thread, and autograd runs the backward on a thread of its own, so the name is read
+    in the thread that made the call."""
+    from blocksparse_b200 import _lib
+
+    def wrap(name, fn):
+        def run(*a, **kw):
+            out = fn(*a, **kw)
+            seen.append((name, _lib.last_kernel()))
+            return out
+        return run
+    for name in names:
+        monkeypatch.setattr(obj, name, wrap(name, getattr(obj, name)))
+
+
+def _on_poisoned_output(fn):
+    """Run fn() with every floating-point tensor it allocates through torch.empty / torch.empty_like (its output and
+    any temporaries) filled with NaN first, so an element a kernel never writes shows up as NaN. The returned tensor
+    must be one of those: an output allocated any other way would make the NaN checks vacuous, so it fails here."""
+    empty, empty_like = torch.empty, torch.empty_like
+    ptrs = set()
+
+    def poisoned(t):
+        if t.is_floating_point():
+            t.fill_(float("nan"))
+            ptrs.add(t.data_ptr())
+        return t
+    torch.empty = lambda *a, **kw: poisoned(empty(*a, **kw))
+    torch.empty_like = lambda *a, **kw: poisoned(empty_like(*a, **kw))
+    try:
+        out = fn()
+    finally:
+        torch.empty, torch.empty_like = empty, empty_like
+    assert out.data_ptr() in ptrs, "the output was not allocated through torch.empty / torch.empty_like: nothing poisoned it"
+    return out

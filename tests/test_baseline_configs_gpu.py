@@ -5,13 +5,16 @@ The oracle's NumPy loops cannot run a 4096 x 4096 x 4096 problem in seconds, so 
     `fprop` / `bprop` restatement of matmul.py:353-399 evaluated on exactly those rows, all features;
   * updat on a SAMPLE of weight blocks over the FULL minibatch (`updat_blocks`, matmul.py:401-419);
 with the reference's two error metrics, and asserts which kernel family ran and that no bounded wait timed out.
-Each density of cfg 2 selects a different xprop kernel variant (matmul.py picks the stage shape from the density).
+The same samples are also checked elementwise against float64, with the error bound of the kernel that ran. Every
+density of cfg 2 runs the same wgmma kernels; what changes is the LUT row length, up to 128 entries (4096 accumulated
+terms) at density 1.0.
 """
 import numpy as np
 import pytest
 import torch
 
-from tests._util import U_OUT, fma_gemm_bound, ref_errors, softmax_grad_bound, softmax_row_sums
+from tests._util import (U_OUT, assert_within, dtype_name, fma_gemm_bound, mma_gemm_bound, ref_errors, softmax_grad_bound,
+                         softmax_row_sums)
 from blocksparse_b200 import BlocksparseMatMul, BlocksparseTransformer, _lib
 from blocksparse_b200.layouts import bernoulli_layout, barabasi_albert_layout, local_strided_layout
 from oracle.bsmm_oracle import MatmulOracle
@@ -52,6 +55,25 @@ def _case(layout, bs, axis, N, dtype, seed, n_rows=48, n_blocks=96, expect=None,
     errs["updat"] = ref_errors(dw.index_select(0, torch.as_tensor(blk, device="cuda")).float().cpu().numpy(), ref_dw)
     for op, (mx, l2) in errs.items():
         assert mx <= tol[0] and l2 <= tol[1], "%s: max_err %.3e l2_err %.3e (%s)" % (op, mx, l2, kernels[op])
+    # elementwise, against float64, with the bound of the kernel that ran: bs x the LUT row length terms per output
+    # block of the layout the kernel walks (the 16 x 16 super-blocks for padded 8 x 8 blocks), N per dw element
+    name = dtype_name(dtype)
+    walked = bsmm._shadow if bsmm._shadow is not None else bsmm
+    lay_w = walked.layout.astype(np.int64)
+    W64, rows_x, rows_e = Wh.astype(np.float64), sample(X).astype(np.float64), sample(E).astype(np.float64)
+    for op, got, a, fn in [("fprop", y, rows_x, orc.fprop), ("bprop", dx, rows_e, orc.bprop)]:
+        counts = lay_w.sum(axis=1 if op == "bprop" else 0) * walked.bsize
+        k = np.repeat(counts, walked.bsize).astype(np.float64)
+        k = k[None, :] if axis else k[:, None]
+        ref, ref_abs = fn(a, W64), fn(np.abs(a), np.abs(W64))
+        bound_fn = fma_gemm_bound if kernels[op].startswith("fma_") else mma_gemm_bound
+        assert_within(sample(got), ref, bound_fn(ref, ref_abs, name, k), "%s (%s)" % (op, kernels[op]), ref_abs, k, name,
+                      kernels[op].split("_bs")[0])
+    abs_dw = orc.updat_blocks(np.abs(X.float().cpu().numpy()), np.abs(E.float().cpu().numpy()), blk)
+    bound_fn = fma_gemm_bound if kernels["updat"].startswith("fma_") else mma_gemm_bound
+    got_dw = dw.index_select(0, torch.as_tensor(blk, device="cuda")).float().cpu().numpy()
+    assert_within(got_dw, ref_dw, bound_fn(ref_dw, abs_dw, name, N), "updat (%s)" % kernels["updat"], abs_dw, N, name,
+                  kernels["updat"].split("_bs")[0])
     # rows of Y that belong to empty output block-columns must be exactly zero (cn_64.cu:243-253)
     empty = np.nonzero(np.asarray(layout).sum(axis=0) == 0)[0]
     if len(empty):

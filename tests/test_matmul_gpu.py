@@ -9,7 +9,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests._util import GOLDEN, golden_files, ref_errors
+from tests._util import (GOLDEN, _on_poisoned_output, assert_within, assert_zero_filled, feature_terms, fma_gemm_bound,
+                         golden_files, oracle_dense, ref_errors)
 from blocksparse_b200 import BlocksparseMatMul, group_param_grads, _lib
 from oracle.bsmm_oracle import MatmulOracle
 
@@ -83,10 +84,23 @@ def test_ragged_minibatch_fp32(axis, bs, N):
         orc.__dict__.update(base.__dict__)
         orc.bsize, orc.C, orc.K, orc.w_shape = bs, lay.shape[0] * bs, lay.shape[1] * bs, bsmm.w_shape
     Wd, Xd, Ed = (torch.as_tensor(a).cuda() for a in (W, X, E))
-    y = bsmm.fprop(Xd, Wd)
-    check(y, orc.fprop_dense(X, W), torch.float32, "fprop")
-    check(bsmm.bprop(Ed, Wd), orc.bprop_dense(E, W), torch.float32, "bprop")
-    check(bsmm.updat([Xd], [Ed]), orc.updat_dense(X, E), torch.float32, "updat")
+    # true fp32 FMA kernels, elementwise against float64 (fma_gemm_bound: bs x the LUT row length terms per output
+    # block, N per dw element), each on NaN-poisoned output memory
+    for op, inp, fn in [("fprop", X, bsmm.fprop), ("bprop", E, bsmm.bprop)]:
+        ref, ref_abs = oracle_dense(orc, op, inp, W), oracle_dense(orc, op, np.abs(inp), np.abs(W))
+        dev = torch.as_tensor(inp).cuda()
+        got = _on_poisoned_output(lambda: fn(dev, Wd))
+        assert _lib.last_kernel() == "fma_sdd_xn", _lib.last_kernel()
+        assert_zero_filled(got, np.nonzero(lay.sum(axis=1 if op == "bprop" else 0) == 0)[0], bs, axis, op)
+        assert_within(got, ref, fma_gemm_bound(ref, ref_abs, "float32", feature_terms(lay, bs, op == "bprop", axis)), op)
+        check(got, ref, torch.float32, op)
+        if op == "fprop":
+            y = got
+    ref, ref_abs = oracle_dense(orc, "updat", X, E), oracle_dense(orc, "updat", np.abs(X), np.abs(E))
+    dw = _on_poisoned_output(lambda: bsmm.updat([Xd], [Ed]))
+    assert _lib.last_kernel() == "fma_dds_nt", _lib.last_kernel()
+    assert_within(dw, ref, fma_gemm_bound(ref, ref_abs, "float32", N), "updat")
+    check(dw, ref, torch.float32, "updat")
     yv = y.reshape(bsmm.KB, bs, N) if axis == 0 else y.reshape(N, bsmm.KB, bs).permute(1, 2, 0)
     assert float(yv[4].abs().max()) == 0.0
 

@@ -1,10 +1,16 @@
 """GPU parity of the wgmma kernel families (forced with BSMM_FLAG_FORCE_TC so a silent fall-back to the
-CUDA-core kernels cannot pass) against the oracle, at sizes the NumPy loops finish in seconds."""
+CUDA-core kernels cannot pass) against the oracle, at sizes the NumPy loops finish in seconds.
+
+The matmul results are checked elementwise against the float64 oracle with mma_gemm_bound (tests/_util.py), each on
+memory filled with NaN first, so an element the kernel never writes fails too. Every family also has a case with
+operands uniform in (0, 1): there the bound is within a few eps32 of one output rounding, tight enough to tell
+round-to-nearest from truncation, which sign-mixed data hides behind cancellation."""
 import numpy as np
 import pytest
 import torch
 
-from tests._util import fma_gemm_bound, ref_errors
+from tests._util import (_on_poisoned_output, assert_within, assert_zero_filled, dtype_name, feature_terms,
+                         fma_gemm_bound, mma_gemm_bound, oracle_dense, record_kernels, ref_errors)
 from blocksparse_b200 import BlocksparseMatMul, _lib
 from oracle.bsmm_oracle import MatmulOracle
 
@@ -24,7 +30,7 @@ def layout(rng, CB, KB, density, empty_col=None, empty_row=None):
 
 
 CASES = [
-    # CB, KB, density, N, bs
+    # CB, KB, density, N, bs[, "pos": operands uniform in (0, 1)]
     (8, 8, 0.3, 128, 32),
     (5, 37, 0.5, 200, 32),        # ragged N, more than two output tiles (16 blocks each), rectangular
     (40, 33, 0.08, 1, 32),        # single row
@@ -36,14 +42,46 @@ CASES = [
     (6, 9, 0.5, 130, 64),
     (16, 17, 0.3, 64, 64),
     (12, 12, 1.0, 300, 64),
+    (10, 12, 0.4, 136, 32, "pos"),
+    (9, 14, 0.4, 128, 16, "pos"),
+    (6, 9, 0.5, 130, 64, "pos"),
 ]
+
+
+def operands(rng, bsmm, N, dtype, positive=False):
+    """W, X, E on the host in dtype: N(0, 0.1) weights and N(0, 1) activations, or all uniform in (0, 1)."""
+    draw = (lambda shape, s: rng.uniform(0, 1, shape)) if positive else (lambda shape, s: rng.normal(0, s, shape))
+    return tuple(torch.as_tensor(draw(shape, s).astype(np.float32)).to(dtype)
+                 for shape, s in ((bsmm.w_shape, 0.1), (bsmm.i_shape(N), 1), (bsmm.o_shape(N), 1)))
+
+
+def check_xprop(orc, lay, bs, bprop, inp, W, run, what, k=None, family="wgmma_xprop"):
+    """run() (an fprop / bprop of inp and W, already on the device) on NaN-poisoned output memory: every element is
+    written, the output blocks of lay (block size bs) with an empty LUT row are exactly zero, and the result is within
+    mma_gemm_bound of the float64 oracle. k: k_terms (default: bs x the LUT row length of each output block of lay).
+    Returns the output and the kernel that ran."""
+    name = dtype_name(inp.dtype)
+    inp_n, Wn = inp.float().numpy(), W.float().numpy()
+    op = "bprop" if bprop else "fprop"
+    ref, ref_abs = oracle_dense(orc, op, inp_n, Wn), oracle_dense(orc, op, np.abs(inp_n), np.abs(Wn))
+    got = _on_poisoned_output(run)
+    assert _lib.device_error() == 0, "a wgmma kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
+    kern = _lib.last_kernel()
+    if k is None:
+        k = feature_terms(lay, bs, bprop, orc.axis)
+    empty = np.nonzero((np.asarray(lay) != 0).sum(axis=1 if bprop else 0) == 0)[0]
+    assert_zero_filled(got, empty, bs, orc.axis, "%s (%s)" % (what, kern))
+    assert_within(got, ref, mma_gemm_bound(ref, ref_abs, name, k), "%s (%s)" % (what, kern), ref_abs, k, name, family)
+    mx, l2 = ref_errors(got.double().cpu().numpy(), ref)
+    assert l2 <= (4e-3 if inp.dtype == torch.bfloat16 else 1e-3), "%s (%s) l2 %.3e" % (what, kern, l2)
+    return got, kern
 
 
 @pytest.mark.parametrize("axis", [1, 0])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("case", CASES)
 def test_tc_xprop_matches_oracle(case, dtype, axis):
-    CB, KB, density, N, bs = case
+    CB, KB, density, N, bs, *opt = case
     if axis == 0:
         N = max(8, (N + 7) // 8 * 8)          # TMA needs a 16-byte row pitch when the minibatch is the inner dim
     rng = np.random.default_rng(CB * 1000 + KB * 10 + N)
@@ -51,21 +89,16 @@ def test_tc_xprop_matches_oracle(case, dtype, axis):
     bsmm = BlocksparseMatMul(lay, block_size=bs, feature_axis=axis)
     orc = MatmulOracle(lay, 32, axis)         # (axis 0, bs 64) is outside the reference's pairs: reuse the dense restatement
     orc.bsize, orc.C, orc.K, orc.w_shape = bs, CB * bs, KB * bs, bsmm.w_shape
-    W = torch.as_tensor(rng.normal(0, 0.1, bsmm.w_shape).astype(np.float32)).to(dtype)
-    X = torch.as_tensor(rng.normal(0, 1, bsmm.i_shape(N)).astype(np.float32)).to(dtype)
-    E = torch.as_tensor(rng.normal(0, 1, bsmm.o_shape(N)).astype(np.float32)).to(dtype)
-    Wn, Xn, En = W.float().numpy(), X.float().numpy(), E.float().numpy()
-    for name, got_fn, ref in [("fprop", lambda: bsmm.fprop(X.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_TC), orc.fprop_dense(Xn, Wn)),
-                              ("bprop", lambda: bsmm.bprop(E.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_TC), orc.bprop_dense(En, Wn))]:
-        got = got_fn()
-        assert _lib.device_error() == 0, "a wgmma kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
-        assert _lib.last_kernel().startswith("wgmma_xprop"), _lib.last_kernel()
-        mx, l2 = ref_errors(got.float().cpu().numpy(), ref)
-        assert l2 <= (4e-3 if dtype == torch.bfloat16 else 1e-3), "%s l2 %.3e max %.3e" % (name, l2, mx)
-        assert mx <= (4e-2 if dtype == torch.bfloat16 else 1e-2), "%s l2 %.3e max %.3e" % (name, l2, mx)
+    W, X, E = operands(rng, bsmm, N, dtype, "pos" in opt)
+    Wd = W.cuda()
+    for bprop, inp in [(False, X), (True, E)]:
+        fn = bsmm.bprop if bprop else bsmm.fprop
+        xd = inp.cuda()
+        got, kern = check_xprop(orc, lay, bs, bprop, inp, W, lambda: fn(xd, Wd, flags=_lib.FLAG_FORCE_TC),
+                                "bprop" if bprop else "fprop")
+        assert kern.startswith("wgmma_xprop"), kern
         # agrees with the fp32-accumulating CUDA-core path up to one output rounding
-        gen = bsmm.fprop(X.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_GENERIC) if name == "fprop" else \
-            bsmm.bprop(E.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_GENERIC)
+        gen = fn(xd, Wd, flags=_lib.FLAG_FORCE_GENERIC)
         diff = (got.float() - gen.float()).abs().max().item()
         scale = gen.float().abs().max().item()
         assert diff <= scale * 2.0 ** -7, "wgmma vs FMA path differ by %g (scale %g)" % (diff, scale)
@@ -85,8 +118,8 @@ def test_tc_xprop_repeatable_and_stream_ordered():
 
 @pytest.mark.parametrize("bs", [32, 64])
 def test_gated_xprop_runs_on_tcgen05(bs):
-    """gate folded into a scaled weight copy (bsmm_gate_weights) + wgmma kernel == oracle's gated product;
-    zero gates drop their blocks exactly."""
+    """gate folded into a scaled weight copy (bsmm_gate_weights) + wgmma kernel == oracle's product with that copy
+    (tests/test_bsmm_paths_gpu.py checks the copy bit for bit); zero gates drop their blocks exactly."""
     rng = np.random.default_rng(11)
     lay = layout(rng, 12, 10, 0.4)
     bsmm = BlocksparseMatMul(lay, block_size=bs, feature_axis=1)
@@ -98,73 +131,101 @@ def test_gated_xprop_runs_on_tcgen05(bs):
     E = torch.as_tensor(rng.normal(0, 1, bsmm.o_shape(N)).astype(np.float32)).bfloat16()
     gate = rng.uniform(0.5, 1.5, bsmm.blocks).astype(np.float32)
     gate[rng.random(bsmm.blocks) < 0.3] = 0.0
-    Wg = (W.float().numpy() * gate[:, None, None])
+    Wg = (W.float() * torch.as_tensor(gate)[:, None, None]).bfloat16()
     g = torch.as_tensor(gate).cuda()
-    y = bsmm.fprop(X.cuda(), W.cuda(), gate=g)
-    assert _lib.last_kernel().startswith("wgmma_xprop")
-    dx = bsmm.bprop(E.cuda(), W.cuda(), gate=g)
-    assert _lib.last_kernel().startswith("wgmma_xprop") and _lib.device_error() == 0
-    for got, ref in [(y, orc.fprop_dense(X.float().numpy(), Wg)), (dx, orc.bprop_dense(E.float().numpy(), Wg))]:
-        err = np.abs(got.float().cpu().numpy() - ref)
-        assert err.max() <= 4e-2 * np.abs(ref).max() and np.sqrt((err ** 2).sum() / (ref ** 2).sum()) <= 1e-2
-    yg = bsmm.fprop(X.cuda(), W.cuda(), gate=g, flags=_lib.FLAG_FORCE_GENERIC)      # CUDA-core gated path agrees
+    Xd, Ed, Wd = X.cuda(), E.cuda(), W.cuda()
+    y, kern = check_xprop(orc, lay, bs, False, X, Wg, lambda: bsmm.fprop(Xd, Wd, gate=g), "gated fprop")
+    assert kern.startswith("wgmma_xprop"), kern
+    _, kern = check_xprop(orc, lay, bs, True, E, Wg, lambda: bsmm.bprop(Ed, Wd, gate=g), "gated bprop")
+    assert kern.startswith("wgmma_xprop"), kern
+    yg = bsmm.fprop(Xd, Wd, gate=g, flags=_lib.FLAG_FORCE_GENERIC)      # CUDA-core gated path agrees
     assert (y.float() - yg.float()).abs().max().item() <= 2.0 ** -6 * yg.float().abs().max().item()
 
 
 UPDAT_CASES = [
-    # CB, KB, density, N, bs, pairs
+    # CB, KB, density, N, bs, pairs[, "pos": operands uniform in (0, 1) | "sms3": schedule built for 3 SMs]
     (8, 8, 0.3, 128, 32, 1),
     (5, 37, 0.5, 200, 32, 2),      # group of 4 input blocks is ragged (5 = 4 + 1), N not a multiple of 64
     (40, 33, 0.08, 1, 32, 1),
-    (20, 20, 1.0, 257, 32, 3),
+    (20, 20, 1.0, 257, 32, 3),     # 20 kept output blocks per group: three windows of <= 8 slots
     (64, 64, 0.2, 640, 32, 8),     # 8 (x, dy) pairs in one launch
     (9, 40, 0.3, 200, 16, 2),      # 16 x 16 blocks: 8 input blocks per group, 16 slots per tile, two blocks per epilogue warp
     (33, 17, 0.15, 64, 16, 1),
     (12, 12, 1.0, 130, 16, 8),
     (6, 9, 0.5, 130, 64, 1),
     (16, 17, 0.3, 64, 64, 2),
-    (12, 12, 1.0, 300, 64, 1),
+    (12, 12, 1.0, 300, 64, 1),     # 12 kept output blocks per group: three windows of 4 slots
+    (10, 12, 0.4, 136, 32, 3, "pos"),
+    (9, 14, 0.4, 128, 16, 2, "pos"),
+    (6, 9, 0.5, 130, 64, 1, "pos"),
+    (9, 40, 0.3, 200, 16, 2, "sms3"),   # _balance_windows splits groups into extra windows to fill whole waves
+    (64, 64, 0.2, 256, 32, 2, "sms3"),
 ]
 
 
 @pytest.mark.parametrize("axis", [1, 0])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("case", UPDAT_CASES)
-def test_tc_updat_matches_oracle(case, dtype, axis):
-    CB, KB, density, N, bs, pairs = case
+def test_tc_updat_matches_oracle(case, dtype, axis, monkeypatch):
+    CB, KB, density, N, bs, pairs, *opt = case
     if axis == 0:
         N = max(8, (N + 7) // 8 * 8)
     rng = np.random.default_rng(CB * 1000 + KB * 10 + N + 7)
     lay = layout(rng, CB, KB, density, empty_col=KB // 2 if density < 1 else None, empty_row=1 if density < 1 and CB > 2 else None)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    if "sms3" in opt:               # the schedule is cached per object: build a fresh one for 3 SMs
+        default_tiles = BlocksparseMatMul(lay, block_size=bs, feature_axis=axis)._device_luts(dev)["updat_tiles"]
+        monkeypatch.setattr(_lib, "grid_sms", lambda d: 3)
     bsmm = BlocksparseMatMul(lay, block_size=bs, feature_axis=axis)
+    if "sms3" in opt:
+        assert bsmm._device_luts(dev)["updat_tiles"] > default_tiles
     orc = MatmulOracle(lay, 32, axis)
     orc.bsize, orc.C, orc.K, orc.w_shape = bs, CB * bs, KB * bs, bsmm.w_shape
-    xs, es, ref = [], [], np.zeros(bsmm.w_shape)
+    draw = (lambda shape: rng.uniform(0, 1, shape)) if "pos" in opt else (lambda shape: rng.normal(0, 1, shape))
+    xs, es, ref, ref_abs = [], [], 0.0, 0.0
     for _ in range(pairs):
-        X = torch.as_tensor(rng.normal(0, 1, bsmm.i_shape(N)).astype(np.float32)).to(dtype)
-        E = torch.as_tensor(rng.normal(0, 1, bsmm.o_shape(N)).astype(np.float32)).to(dtype)
+        X = torch.as_tensor(draw(bsmm.i_shape(N)).astype(np.float32)).to(dtype)
+        E = torch.as_tensor(draw(bsmm.o_shape(N)).astype(np.float32)).to(dtype)
         xs.append(X.cuda()); es.append(E.cuda())
-        ref += orc.updat_dense(X.float().numpy(), E.float().numpy())
-    # fp32 output: only the 16-bit INPUT rounding separates us from the oracle (which sees the same rounded inputs)
-    dw32 = bsmm.updat(xs, es, dw_dtype=torch.float32, flags=_lib.FLAG_FORCE_TC)
-    assert _lib.device_error() == 0, "a wgmma kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
-    assert _lib.last_kernel().startswith("wgmma_updat"), _lib.last_kernel()
-    mx, l2 = ref_errors(dw32.cpu().numpy(), ref)
-    assert l2 <= 1e-5 and mx <= 1e-4, "fp32-out updat l2 %.3e max %.3e" % (l2, mx)
-    # native-dtype output, alpha, and in-place accumulation (beta = 1)
-    dw = bsmm.updat(xs, es, alpha=0.5, flags=_lib.FLAG_FORCE_TC)
-    mx, l2 = ref_errors(dw.float().cpu().numpy(), 0.5 * ref)
-    assert l2 <= (4e-3 if dtype == torch.bfloat16 else 1e-3), "updat l2 %.3e max %.3e" % (l2, mx)
-    acc = dw32.clone()
-    bsmm.updat(xs[:1], es[:1], dw=acc, flags=_lib.FLAG_FORCE_TC)
-    ref2 = ref + orc.updat_dense(xs[0].float().cpu().numpy(), es[0].float().cpu().numpy())
-    mx, l2 = ref_errors(acc.cpu().numpy(), ref2)
-    assert l2 <= 1e-5, "accumulate l2 %.3e" % l2
-    gate = torch.as_tensor((rng.random(bsmm.blocks) < 0.7).astype(np.float32) * 1.5).cuda()
-    dwg = bsmm.updat(xs, es, gate=gate, dw_gated=True, dw_dtype=torch.float32, flags=_lib.FLAG_FORCE_TC)
-    mx, l2 = ref_errors(dwg.cpu().numpy(), ref * gate.cpu().numpy()[:, None, None])
-    assert l2 <= 1e-5, "gated l2 %.3e" % l2
-    assert _lib.device_error() == 0
+        Xn, En = X.float().numpy(), E.float().numpy()
+        ref = ref + oracle_dense(orc, "updat", Xn, En)
+        ref_abs = ref_abs + oracle_dense(orc, "updat", np.abs(Xn), np.abs(En))
+    k, name, F = N * pairs, dtype_name(dtype), _lib.FLAG_FORCE_TC
+
+    def check(got, r, a, k_terms, extra, what, max_tol=np.inf):
+        assert _lib.device_error() == 0, "a wgmma kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
+        assert _lib.last_kernel().startswith("wgmma_updat"), _lib.last_kernel()
+        assert not bool(torch.isnan(got).any()), "%s: %d dw elements never written" % (what, int(torch.isnan(got).sum()))
+        out = dtype_name(got.dtype)
+        assert_within(got, r, mma_gemm_bound(r, a, out, k_terms, extra), what, a, k_terms, out, "wgmma_updat")
+        # the aggregate metrics too: on sign-mixed data the linear worst-case bound is loose, and l2 is the tighter
+        # statistical guard for an fp32 dw (only the 16-bit input rounding separates it from the oracle)
+        mx, l2 = ref_errors(got.double().cpu().numpy(), r)
+        assert l2 <= {"float32": 1e-5, "bfloat16": 4e-3, "float16": 1e-3}[out] and mx <= max_tol, \
+            "%s l2 %.3e max %.3e" % (what, l2, mx)
+
+    # fresh outputs on NaN-poisoned memory: every dw element is written. fp32 dw, then 16-bit dw with alpha.
+    dw32 = _on_poisoned_output(lambda: bsmm.updat(xs, es, dw_dtype=torch.float32, flags=F))
+    check(dw32, ref, ref_abs, k, 0, "fp32 dw", max_tol=1e-4)
+    dw = _on_poisoned_output(lambda: bsmm.updat(xs, es, alpha=0.5, flags=F))
+    check(dw, 0.5 * ref, 0.5 * ref_abs, k, 1, "%s dw, alpha 0.5" % name)
+    # in-place accumulation (beta = 1), into an fp32 and into a 16-bit dw
+    X0, E0 = xs[0].float().cpu().numpy(), es[0].float().cpu().numpy()
+    ref0, abs0 = oracle_dense(orc, "updat", X0, E0), oracle_dense(orc, "updat", np.abs(X0), np.abs(E0))
+    for base in (dw32, dw):
+        acc = base.clone()
+        old = base.double().cpu().numpy()
+        bsmm.updat(xs[:1], es[:1], dw=acc, flags=F)
+        check(acc, old + ref0, np.abs(old) + abs0, N, 1, "accumulate into %s dw" % dtype_name(base.dtype))
+    # gated dw with alpha != 1, accumulated: g = alpha * gate, then a * g + old (zero gates leave old untouched)
+    gate = ((rng.random(bsmm.blocks) < 0.7) * rng.uniform(0.5, 1.5, bsmm.blocks)).astype(np.float32)
+    g, gn = torch.as_tensor(gate).cuda(), gate.astype(np.float64)[:, None, None]
+    for base in (dw32, dw):
+        acc = base.clone()
+        old = base.double().cpu().numpy()
+        bsmm.updat(xs, es, dw=acc, alpha=0.75, gate=g, dw_gated=True, flags=F)
+        check(acc, old + 0.75 * gn * ref, np.abs(old) + 0.75 * gn * ref_abs, k, 3,
+              "gated, alpha 0.75, accumulate into %s dw" % dtype_name(base.dtype))
 
 
 # ------------------------------------------------------------------------------------------------------------
@@ -191,24 +252,6 @@ def _bst_layout(rng, heads_l, qb, kb, density, empty_q=(), empty_k=()):
         for q, k in free[: target - int(lay[h].sum())]:
             lay[h, q, k] = 1
     return lay
-
-
-def _on_poisoned_output(fn, shape, dtype, tries=8):
-    """Run fn(), whose output is a fresh torch.empty(shape, dtype), on memory just filled with NaN: a tensor of that
-    size is filled and freed, and the caching allocator hands the block back to the next allocation of that size, so
-    an element the kernel never writes shows up as NaN. Should the allocator pick another free block instead (it
-    prefers the best fit, and the freed block may have merged with a neighbour), that output is kept alive, so the
-    next try cannot get it again."""
-    held = []
-    for _ in range(tries):
-        t = torch.full(shape, float("nan"), dtype=dtype, device="cuda")
-        ptr = t.data_ptr()
-        del t
-        c = fn()
-        if c.data_ptr() == ptr:
-            return c
-        held.append(c)
-    raise AssertionError("the output never landed on the NaN-filled block")
 
 
 def _assert_zero_blocks(c, empty, bs, what):
@@ -266,8 +309,7 @@ def test_tc_bst_gemms_match_oracle(case, dtype):
     if holes:
         Pd, Vd, DYd = P.cuda(), V.cuda(), DY.cuda()
         for transpose, dense, empty, what in [(False, Vd, empty_q, "nn"), (True, DYd, empty_k, "tn")]:
-            shape = (batch, (kb if transpose else qb) * 64, S)
-            c = _on_poisoned_output(lambda: bst._xn(Pd, dense, transpose, flags=F), shape, dtype)
+            c = _on_poisoned_output(lambda: bst._xn(Pd, dense, transpose, flags=F))
             assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_" + what
             _assert_zero_blocks(c, empty, 64, what)
 
@@ -302,11 +344,10 @@ def test_fma_bst_gemms_match_oracle(case):
     P = mk(a_dtype, batch, heads, bst.blocks, bs, bs)
     Qn, Kn, DYn, Pn = (t.float().numpy() for t in (Q, K, DY, P))
     Qd, Kd, DYd, Pd = Q.cuda(), K.cuda(), DY.cuda(), P.cuda()
-    name = lambda dt: str(dt).replace("torch.", "")
 
     def check(got, ref, ref_abs, k_terms, what):
         g = got.double().cpu().numpy().reshape(ref.shape)
-        bound = fma_gemm_bound(ref.astype(np.float64), ref_abs.astype(np.float64), name(got.dtype), k_terms)
+        bound = fma_gemm_bound(ref.astype(np.float64), ref_abs.astype(np.float64), dtype_name(got.dtype), k_terms)
         err = np.abs(g - ref)
         assert np.all(err <= bound), "%s: %d elements out of bound, worst excess %.3e" % (
             what, int((err > bound).sum()), float((err - bound).max()))
@@ -319,8 +360,7 @@ def test_fma_bst_gemms_match_oracle(case):
     for transpose, dense, dn, empty, lmax, what in [(False, Kd, Kn, empty_q, bst.nn_max, "nn"),
                                                     (True, DYd, DYn, empty_k, bst.tn_max, "tn")]:
         bst._xn(Pd, dense, transpose, flags=flags)              # first call builds the device LUTs
-        got = _on_poisoned_output(lambda: bst._xn(Pd, dense, transpose, flags=flags),
-                                  (batch, (kb if transpose else qb) * bs, S), dtype)
+        got = _on_poisoned_output(lambda: bst._xn(Pd, dense, transpose, flags=flags))
         assert _lib.device_error() == 0 and _lib.last_kernel() == "fma_sdd_xn", _lib.last_kernel()
         assert got.dtype == dtype
         op = orc.tn if transpose else orc.nn
@@ -330,14 +370,25 @@ def test_fma_bst_gemms_match_oracle(case):
 
 
 X2_CASES = [
-    # CB, KB, density, N            (32 x 32 blocks; csrc/tc_xprop2.cuh wide tiles)
+    # CB, KB, density, N[, "pos"]    (32 x 32 blocks; csrc/tc_xprop2.cuh wide tiles)
     (8, 8, 0.3, 128),
     (5, 37, 0.5, 200),            # odd number of input blocks (last pair is half out of range), ragged N
     (7, 20, 1.0, 257),            # dense: every pair-group overflows its W slots and is split
     (40, 33, 0.08, 1),
     (6, 32, -1, 136),             # checkerboard: 8 isolated runs per half (the record's run limit)
     (64, 64, 0.2, 640),
+    (10, 12, 0.4, 136, "pos"),
 ]
+
+
+def wide_terms(lay, bprop, tb, axis):
+    """k_terms of the wide-tile kernel: every output block of a tile of tb walks the tile's merged LUT row, one entry
+    per input block that any of them consumes."""
+    m = np.asarray(lay) != 0
+    m = m if bprop else m.T                                  # (output blocks, input blocks)
+    merged = [int(m[t:t + tb].any(axis=0).sum()) for t in range(0, m.shape[0], tb)]
+    kf = np.repeat(np.repeat(merged, tb)[:m.shape[0]] * 32, 32).astype(np.float64)
+    return kf[None, :] if axis else kf[:, None]
 
 
 @pytest.mark.parametrize("variant", [1, 2, 3])
@@ -348,7 +399,7 @@ def test_tc_xprop2_variants_match_oracle(case, dtype, axis, variant, monkeypatch
     """Every variant of the wide-activation-tile kernel (forced through matmul._X2_FORCE), both feature axes."""
     import blocksparse_b200.matmul as mm
     monkeypatch.setattr(mm, "_X2_FORCE", variant)
-    CB, KB, density, N = case
+    CB, KB, density, N, *opt = case
     if axis == 0:
         N = max(8, (N + 7) // 8 * 8)
     rng = np.random.default_rng(CB * 1000 + KB * 10 + N)
@@ -358,20 +409,16 @@ def test_tc_xprop2_variants_match_oracle(case, dtype, axis, variant, monkeypatch
         lay = layout(rng, CB, KB, density, empty_col=KB // 2 if density < 1 else None, empty_row=1 if density < 1 and CB > 2 else None)
     bsmm = BlocksparseMatMul(lay, block_size=32, feature_axis=axis)
     orc = MatmulOracle(lay, 32, axis)
-    W = torch.as_tensor(rng.normal(0, 0.1, bsmm.w_shape).astype(np.float32)).to(dtype)
-    X = torch.as_tensor(rng.normal(0, 1, bsmm.i_shape(N)).astype(np.float32)).to(dtype)
-    E = torch.as_tensor(rng.normal(0, 1, bsmm.o_shape(N)).astype(np.float32)).to(dtype)
-    Wn, Xn, En = W.float().numpy(), X.float().numpy(), E.float().numpy()
-    for name, fn, inp, ref in [("fprop", bsmm.fprop, X, orc.fprop_dense(Xn, Wn)), ("bprop", bsmm.bprop, E, orc.bprop_dense(En, Wn))]:
-        got = fn(inp.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_TC)
-        assert _lib.device_error() == 0, _lib.device_error_text()
-        assert _lib.last_kernel() == "wgmma_xprop2_bs32", _lib.last_kernel()
-        mx, l2 = ref_errors(got.float().cpu().numpy(), ref)
-        # max metric = worst element over MEAN magnitude: the bf16 output rounding alone (2^-9 of the largest element,
-        # max/mean ~ 20 for these N(0,1) inputs at 4-10 terms per sum) reaches ~4e-2; the l2 bound is the meaningful one
-        assert l2 <= (4e-3 if dtype == torch.bfloat16 else 1e-3) and mx <= (6e-2 if dtype == torch.bfloat16 else 1e-2), \
-            "%s variant %d: l2 %.3e max %.3e" % (name, variant, l2, mx)
-        again = fn(inp.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_TC)
+    W, X, E = operands(rng, bsmm, N, dtype, "pos" in opt)
+    Wd = W.cuda()
+    for bprop, inp in [(False, X), (True, E)]:
+        fn = bsmm.bprop if bprop else bsmm.fprop
+        xd = inp.cuda()
+        got, kern = check_xprop(orc, lay, 32, bprop, inp, W, lambda: fn(xd, Wd, flags=_lib.FLAG_FORCE_TC),
+                                "%s variant %d" % ("bprop" if bprop else "fprop", variant),
+                                k=wide_terms(lay, bprop, mm._X2_VARIANTS[variant], axis), family="wgmma_xprop2")
+        assert kern == "wgmma_xprop2_bs32", kern
+        again = fn(xd, Wd, flags=_lib.FLAG_FORCE_TC)
         assert torch.equal(got, again)            # deterministic accumulation order
 
 
@@ -411,43 +458,68 @@ def test_cuda_graph_capture_and_replay():
     assert _lib.device_error() == 0
 
 
+PAIR_CASES = [
+    # CB, KB, density, N[, "pos"]
+    (8, 8, 0.3, 128),
+    (40, 33, 0.08, 1),
+    (64, 64, 0.2, 640),
+    (9, 47, 0.3, 200),
+    (128, 128, 0.25, 1024),
+    (12, 20, 0.3, 300),           # three 128-row tiles: the last cluster's partner CTA lies wholly past N
+    (10, 12, 0.4, 136, "pos"),
+]
+
+
 @pytest.mark.parametrize("axis", [1, 0])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-@pytest.mark.parametrize("case", [(8, 8, 0.3, 128), (40, 33, 0.08, 1), (64, 64, 0.2, 640), (9, 47, 0.3, 200), (128, 128, 0.25, 1024)])
+@pytest.mark.parametrize("case", PAIR_CASES)
 def test_tc_xprop_pair_tiles_match_oracle(case, dtype, axis, monkeypatch):
     """2-CTA clusters sharing every W block by TMA multicast (BSMM_PAIR_TILES, csrc/tc.cuh CL = 2): same results, bit for
-    bit, as the single-CTA kernel (each output block still sees its MMAs in LUT order)."""
+    bit, as the single-CTA kernel (each output block still sees its MMAs in LUT order), and within the bound of the
+    oracle for fprop and bprop."""
     import blocksparse_b200.matmul as mm
-    CB, KB, density, N = case
+    CB, KB, density, N, *opt = case
+    positive = "pos" in opt
     if axis == 0:
         N = max(8, (N + 7) // 8 * 8)
     rng = np.random.default_rng(CB * 1000 + KB * 10 + N)
     lay = layout(rng, CB, KB, density, empty_col=KB // 2, empty_row=1)
-    W = torch.as_tensor(rng.normal(0, 0.1, (int(lay.sum()), 32, 32)).astype(np.float32)).to(dtype).cuda()
+    w_shape = (int(lay.sum()), 32, 32)
+    W = torch.as_tensor((rng.uniform(0, 1, w_shape) if positive else rng.normal(0, 0.1, w_shape)).astype(np.float32)).to(dtype)
+    orc = MatmulOracle(lay, 32, axis)
+    Wd = W.cuda()
     res = {}
     for pair in (0, 1):
         monkeypatch.setattr(mm, "_PAIR_TILES", pair)
         bsmm = BlocksparseMatMul(lay, block_size=32, feature_axis=axis)
-        X = torch.as_tensor(np.random.default_rng(1).normal(0, 1, bsmm.i_shape(N)).astype(np.float32)).to(dtype).cuda()
-        E = torch.as_tensor(np.random.default_rng(2).normal(0, 1, bsmm.o_shape(N)).astype(np.float32)).to(dtype).cuda()
-        y = bsmm.fprop(X, W, flags=_lib.FLAG_FORCE_TC); k1 = _lib.last_kernel()
-        dx = bsmm.bprop(E, W, flags=_lib.FLAG_FORCE_TC); k2 = _lib.last_kernel()
-        assert _lib.device_error() == 0, _lib.device_error_text()
+        draw = (lambda r, shape: r.uniform(0, 1, shape)) if positive else (lambda r, shape: r.normal(0, 1, shape))
+        X = torch.as_tensor(draw(np.random.default_rng(1), bsmm.i_shape(N)).astype(np.float32)).to(dtype)
+        E = torch.as_tensor(draw(np.random.default_rng(2), bsmm.o_shape(N)).astype(np.float32)).to(dtype)
+        Xd, Ed = X.cuda(), E.cuda()
+        if pair:
+            y, k1 = check_xprop(orc, lay, 32, False, X, W, lambda: bsmm.fprop(Xd, Wd, flags=_lib.FLAG_FORCE_TC), "fprop",
+                                family="wgmma_xprop_pair")
+            dx, k2 = check_xprop(orc, lay, 32, True, E, W, lambda: bsmm.bprop(Ed, Wd, flags=_lib.FLAG_FORCE_TC), "bprop",
+                                 family="wgmma_xprop_pair")
+        else:
+            y = bsmm.fprop(Xd, Wd, flags=_lib.FLAG_FORCE_TC); k1 = _lib.last_kernel()
+            dx = bsmm.bprop(Ed, Wd, flags=_lib.FLAG_FORCE_TC); k2 = _lib.last_kernel()
+            assert _lib.device_error() == 0, _lib.device_error_text()
         assert k1 == k2 == ("wgmma_xprop_bs32_pair" if pair else "wgmma_xprop_bs32"), (k1, k2)
         res[pair] = (y, dx)
     assert torch.equal(res[0][0], res[1][0]) and torch.equal(res[0][1], res[1][1])
-    orc = MatmulOracle(lay, 32, axis)
-    mx, l2 = ref_errors(res[1][0].float().cpu().numpy(), orc.fprop_dense(X.float().cpu().numpy(), W.float().cpu().numpy()))
-    assert l2 <= (4e-3 if dtype == torch.bfloat16 else 1e-3), "pair-tile fprop l2 %.3e" % l2
 
 
 @pytest.mark.parametrize("axis", [0, 1])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-def test_bs8_runs_padded_on_tcgen05(dtype, axis):
+def test_bs8_runs_padded_on_tcgen05(dtype, axis, monkeypatch):
     """8 x 8 blocks: 2 x 2 neighbourhoods padded into 16 x 16 super-blocks (csrc/wutil.cuh pad/unpad) and run by the wgmma
-    kernels; fprop / bprop / updat (alpha, accumulate, gate) against the oracle and against the CUDA-core path."""
+    kernels; fprop / bprop (plain, gated, positive operands) and updat (alpha, accumulate, gate) elementwise against the
+    oracle, and against the CUDA-core path."""
     rng = np.random.default_rng(8 + axis)
     lay = layout(rng, 20, 14, 0.3, empty_col=3, empty_row=5)
+    lay[:, 2] = 0                  # an empty super-block column (8 x 8 columns 2-3) and row (rows 4-5) too
+    lay[4, :] = 0
     bsmm = BlocksparseMatMul(lay, block_size=8, feature_axis=axis)
     assert bsmm._shadow is not None and bsmm._shadow.bsize == 16
     orc = MatmulOracle(lay, 8, 0)
@@ -456,28 +528,46 @@ def test_bs8_runs_padded_on_tcgen05(dtype, axis):
     W = torch.as_tensor(rng.normal(0, 0.2, bsmm.w_shape).astype(np.float32)).to(dtype)
     X = torch.as_tensor(rng.normal(0, 1, bsmm.i_shape(N)).astype(np.float32)).to(dtype)
     E = torch.as_tensor(rng.normal(0, 1, bsmm.o_shape(N)).astype(np.float32)).to(dtype)
-    Wn, Xn, En = W.float().numpy(), X.float().numpy(), E.float().numpy()
-    gate = (rng.random(bsmm.blocks) < 0.7).astype(np.float32) * 1.5
+    gate = ((rng.random(bsmm.blocks) < 0.7) * rng.uniform(0.5, 1.5, bsmm.blocks)).astype(np.float32)
     g = torch.as_tensor(gate).cuda()
-    tol = 4e-3 if dtype == torch.bfloat16 else 1e-3
-    for name, got, ref in [("fprop", bsmm.fprop(X.cuda(), W.cuda()), orc.fprop_dense(Xn, Wn)),
-                           ("bprop", bsmm.bprop(E.cuda(), W.cuda()), orc.bprop_dense(En, Wn)),
-                           ("fprop gated", bsmm.fprop(X.cuda(), W.cuda(), gate=g), orc.fprop_dense(Xn, Wn * gate[:, None, None]))]:
-        assert _lib.last_kernel() == "wgmma_xprop_bs16", _lib.last_kernel()
-        mx, l2 = ref_errors(got.float().cpu().numpy(), ref)
-        assert l2 <= tol, "%s l2 %.3e" % (name, l2)
-    ref_dw = orc.updat_dense(Xn, En)
-    dw = bsmm.updat([X.cuda()], [E.cuda()], dw_dtype=torch.float32)
-    assert _lib.last_kernel() == "unpad_blocks"
-    mx, l2 = ref_errors(dw.cpu().numpy(), ref_dw)
-    assert l2 <= 1e-5, "updat l2 %.3e" % l2
-    bsmm.updat([X.cuda()], [E.cuda()], dw=dw, alpha=0.5)                           # in-place accumulate
-    mx, l2 = ref_errors(dw.cpu().numpy(), 1.5 * ref_dw)
-    assert l2 <= 1e-5, "accumulate l2 %.3e" % l2
-    dwg = bsmm.updat([X.cuda()], [E.cuda()], gate=g, dw_gated=True, dw_dtype=torch.float32)
-    mx, l2 = ref_errors(dwg.cpu().numpy(), ref_dw * gate[:, None, None])
-    assert l2 <= 1e-5
-    fma = bsmm.fprop(X.cuda(), W.cuda(), flags=_lib.FLAG_FORCE_GENERIC)
+    Wg = (W.float() * torch.as_tensor(gate)[:, None, None]).to(dtype)      # what bsmm_pad_blocks feeds the kernel
+    P = lambda shape: torch.as_tensor(rng.uniform(0, 1, shape).astype(np.float32)).to(dtype)
+    Wp, Xp, Ep = P(bsmm.w_shape), P(bsmm.i_shape(N)), P(bsmm.o_shape(N))
+    name = dtype_name(dtype)
+    for what, bprop, inp, w, gt, w_ref in [("fprop", False, X, W, None, W), ("bprop", True, E, W, None, W),
+                                           ("fprop gated", False, X, W, g, Wg), ("bprop gated", True, E, W, g, Wg),
+                                           ("fprop positive", False, Xp, Wp, None, Wp), ("bprop positive", True, Ep, Wp, None, Wp)]:
+        xd, wd = inp.cuda(), w.cuda()
+        fn = bsmm.bprop if bprop else bsmm.fprop
+        _, kern = check_xprop(orc, lay, 8, bprop, inp, w_ref, lambda: fn(xd, wd, gate=gt), what,
+                              k=feature_terms(bsmm._shadow.layout, 16, bprop, axis))
+        assert kern == "wgmma_xprop_bs16", kern
+    Xd, Ed = X.cuda(), E.cuda()
+    Xn, En = X.float().numpy(), E.float().numpy()
+    ref_dw, abs_dw = oracle_dense(orc, "updat", Xn, En), oracle_dense(orc, "updat", np.abs(Xn), np.abs(En))
+
+    seen = []
+    record_kernels(monkeypatch, bsmm._shadow, ("updat",), seen)      # the padded product behind each updat
+
+    def check_dw(got, r, a, extra, what):
+        assert _lib.device_error() == 0 and _lib.last_kernel() == "unpad_blocks", _lib.last_kernel()
+        assert seen.pop() == ("updat", "wgmma_updat_bs16") and not seen
+        assert not bool(torch.isnan(got).any()), "%s: dw elements never written" % what
+        out = dtype_name(got.dtype)
+        assert_within(got, r, mma_gemm_bound(r, a, out, N, extra), what, a, N, out, "wgmma_updat")
+        mx, l2 = ref_errors(got.double().cpu().numpy(), r)
+        assert l2 <= {"float32": 1e-5, "bfloat16": 4e-3, "float16": 1e-3}[out], "%s l2 %.3e" % (what, l2)
+
+    dw = _on_poisoned_output(lambda: bsmm.updat([Xd], [Ed], dw_dtype=torch.float32))
+    check_dw(dw, ref_dw, abs_dw, 0, "updat")
+    old = dw.double().cpu().numpy()
+    bsmm.updat([Xd], [Ed], dw=dw, alpha=0.5)                           # in-place accumulate
+    check_dw(dw, old + 0.5 * ref_dw, np.abs(old) + 0.5 * abs_dw, 2, "accumulate")
+    dwg = _on_poisoned_output(lambda: bsmm.updat([Xd], [Ed], gate=g, dw_gated=True))
+    gn = gate.astype(np.float64)[:, None, None]
+    check_dw(dwg, ref_dw * gn, abs_dw * gn, 1, "gated %s dw" % name)
+    Wd = W.cuda()
+    fma = bsmm.fprop(Xd, Wd, flags=_lib.FLAG_FORCE_GENERIC)
     assert _lib.last_kernel().startswith("fma_")
-    assert (fma.float() - bsmm.fprop(X.cuda(), W.cuda()).float()).abs().max().item() <= 2.0 ** -7 * fma.float().abs().max().item()
+    assert (fma.float() - bsmm.fprop(Xd, Wd).float()).abs().max().item() <= 2.0 ** -7 * fma.float().abs().max().item()
     assert _lib.device_error() == 0

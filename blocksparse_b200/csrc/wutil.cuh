@@ -223,13 +223,14 @@ __global__ void reduced_gemm_finish_kernel(const float* __restrict__ partial, fl
 // op 0: out[r,:] = idx[r] >= 0 ? x[idx[r],:] : 0            (gather with gather_lut, scatter with scatter_lut)
 // op 1: out[r,:] = x[r,:] + (idx[r] >= 0 ? y[idx[r],:] : 0)  (scatter_add; idx = scatter_lut)
 // op 2: out[r,:] = x[r,:] * (idx[r] >= 0 ? y[idx[r],:] : 1)  (scatter_mul)
+// The row comes from blockIdx.x (up to 2^31 - 1 rows; gridDim.y stops at 65535) and blockIdx.y grid-strides over N.
 template <typename T>
 __global__ void gather_rows_kernel(const T* __restrict__ x, const T* __restrict__ y, const int32_t* __restrict__ idx, T* __restrict__ out,
                                    int rows, long long N, int op) {
-  const int r = blockIdx.y;
+  const int r = blockIdx.x;
   if (r >= rows) return;
   const int src = idx[r];
-  for (long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x; n < N; n += (long long)gridDim.x * blockDim.x) {
+  for (long long n = (long long)blockIdx.y * blockDim.x + threadIdx.x; n < N; n += (long long)gridDim.y * blockDim.x) {
     float v;
     if (op == 0) v = src >= 0 ? to_f32(x[(long long)src * N + n]) : 0.f;
     else {

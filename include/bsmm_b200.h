@@ -231,14 +231,16 @@ int bsmm_l2_normalize_grad(int dtype, int y_dtype, int bsize, const int32_t* lut
                            const float* sum_sqr, void* dx, float* dg, float epsilon, void* stream);
 /* Block-reduced FULL weight gradient for network growth: x_red / y_red = per-block max|.| (norm_type 0) or l2 norm over the
  * bsize features of each block of every x_p / dy_p (layout (pair, n, block) for axis 1, (block, pair, n) for axis 0, activation
- * dtype), then dw[bC][bK] (float) = scale * sum_{p,n} x_red * y_red (+ dw when accumulate).  scale == 0 skips the reductions.
+ * dtype), then dw[bC][bK] (float) = scale * sum_{p,n} x_red * y_red (+ dw when accumulate).  scale == 0 launches no reduction
+ * and no GEMM: x_red and y_red are zero-filled, dw is left as it is when accumulating and zero-filled otherwise.
  * workspace: bsmm_reduced_dw_workspace_bytes(bC, bK) bytes of device memory. */
 size_t bsmm_reduced_dw_workspace_bytes(int n_c_blocks, int n_k_blocks);
 int bsmm_reduced_dw(int dtype, int axis, int bsize, const void* const* xs, const void* const* dys, int pcount,
                     int n_c_blocks, int n_k_blocks, int N, float scale, int norm_type, float* dw, int accumulate,
                     void* x_red, void* y_red, void* workspace, void* stream);
 /* Row gather / scatter on (rows, N) activations (SparseProj): op 0: out[r] = idx[r] >= 0 ? x[idx[r]] : 0;
- * op 1: out[r] = x[r] + (idx[r] >= 0 ? y[idx[r]] : 0);  op 2: out[r] = x[r] * (idx[r] >= 0 ? y[idx[r]] : 1). */
+ * op 1: out[r] = x[r] + (idx[r] >= 0 ? y[idx[r]] : 0);  op 2: out[r] = x[r] * (idx[r] >= 0 ? y[idx[r]] : 1).
+ * rows is limited only by int. */
 int bsmm_gather_rows(int dtype, const void* x, const void* y, const int32_t* idx, void* out, int rows, long long N, int op, void* stream);
 
 /* 8 x 8 blocks on wgmma (K = 16 per MMA step): scatter a (blocks_small, bs, bs) weight tensor into (blocks_big, 2bs, 2bs)

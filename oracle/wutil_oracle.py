@@ -95,8 +95,9 @@ def identity_init(updat_list, CB, KB, bsize, scale=1.0):
     return W
 
 
-def reduced_dw(XS, YS, scale, bsize, axis, norm, DWA=None):
-    """test/blocksparse_reduced_dw_test.py:87-112."""
+def reduced_dw(XS, YS, scale, bsize, axis, norm, DWA=None, round_red=None):
+    """test/blocksparse_reduced_dw_test.py:87-112. round_red, if given, maps X_RED / Y_RED to the values a kernel that
+    stores them in a narrower dtype multiplies (e.g. rounding to float16); the returned X_RED / Y_RED are rounded too."""
     depth = len(XS)
     if axis == 0:
         bx, by, N = XS[0].shape[0] // bsize, YS[0].shape[0] // bsize, XS[0].shape[1]
@@ -107,6 +108,8 @@ def reduced_dw(XS, YS, scale, bsize, axis, norm, DWA=None):
                 X_RED[:, i, :] = np.max(np.abs(X), axis=1); Y_RED[:, i, :] = np.max(np.abs(Y), axis=1)
             else:
                 X_RED[:, i, :] = np.sqrt(np.sum(np.square(X), axis=1)); Y_RED[:, i, :] = np.sqrt(np.sum(np.square(Y), axis=1))
+        if round_red is not None:
+            X_RED, Y_RED = round_red(X_RED), round_red(Y_RED)
         DW = np.dot(X_RED.reshape(bx, -1), Y_RED.reshape(by, -1).T) * scale
     else:
         bx, by, N = XS[0].shape[1] // bsize, YS[0].shape[1] // bsize, XS[0].shape[0]
@@ -117,6 +120,8 @@ def reduced_dw(XS, YS, scale, bsize, axis, norm, DWA=None):
                 X_RED[i] = np.max(np.abs(X), axis=2); Y_RED[i] = np.max(np.abs(Y), axis=2)
             else:
                 X_RED[i] = np.sqrt(np.sum(np.square(X), axis=2)); Y_RED[i] = np.sqrt(np.sum(np.square(Y), axis=2))
+        if round_red is not None:
+            X_RED, Y_RED = round_red(X_RED), round_red(Y_RED)
         DW = np.dot(X_RED.reshape(-1, bx).T, Y_RED.reshape(-1, by)) * scale
     if DWA is not None:
         DW = DW + DWA

@@ -90,6 +90,26 @@ def mma_gemm_bound(ref, ref_abs, out_dtype, k_terms, extra=0):
     return u * np.abs(ref) + (k_terms * MMA_C * EPS32 * (1 + u) + extra * EPS32) * ref_abs + 2.0 ** -25
 
 
+# Largest absolute error of one round-to-nearest conversion in the subnormal range of a storage dtype: half its
+# smallest subnormal. fp32 and bf16 share fp32's exponent range, so their floor lies far below any value checked here.
+SUBNORMAL_FLOOR = {"float16": 2.0 ** -25, "bfloat16": 2.0 ** -134, "float32": 2.0 ** -150}
+
+
+def chain_bound(ref, ref_abs, out_dtype, k_terms):
+    """Largest |got - ref| of an fp32 CUDA-core computation that is rounded once to out_dtype, elementwise.
+
+    k_terms counts the fp32 roundings on the path to the result, each worth at most eps32 * ref_abs: one per addition
+    in the order the kernel sums (serial loop, then shuffle levels or partials), one per product that is not exact,
+    2 ulp = 4 eps32 for rsqrtf (CUDA C Programming Guide, math appendix) and one for sqrtf and division, which are
+    correctly rounded without --use_fast_math. A value that depends on a computed quantity q as q^p carries |p| times
+    q's relative error. ref_abs is the same expression on absolute values, so that cancelling terms keep their
+    rounding budget; callers that weigh parts of a result differently pass the weighted sum with k_terms = 1. The
+    first-order sum undercounts by a factor below 1 + k eps32, which the 2^-10 margin covers for k < 2^14. Then one
+    rounding to out_dtype (relative u_out) and the subnormal floor of out_dtype."""
+    u = U_OUT[out_dtype]
+    return u * np.abs(ref) + k_terms * EPS32 * (1 + u) * (1 + 2.0 ** -10) * ref_abs + SUBNORMAL_FLOOR[out_dtype]
+
+
 def assert_within(got, ref, bound, what, ref_abs=None, k_terms=None, out_dtype=None, family=None):
     """Every element of got (tensor or array) lies within bound of the float64 ref.
 
@@ -167,8 +187,9 @@ def record_kernels(monkeypatch, obj, names, seen):
 
 def _on_poisoned_output(fn):
     """Run fn() with every floating-point tensor it allocates through torch.empty / torch.empty_like (its output and
-    any temporaries) filled with NaN first, so an element a kernel never writes shows up as NaN. The returned tensor
-    must be one of those: an output allocated any other way would make the NaN checks vacuous, so it fails here."""
+    any temporaries) filled with NaN first, so an element a kernel never writes shows up as NaN. The returned tensor,
+    or every tensor of a returned tuple, must be one of those: an output allocated any other way would make the NaN
+    checks vacuous, so it fails here."""
     empty, empty_like = torch.empty, torch.empty_like
     ptrs = set()
 
@@ -183,5 +204,6 @@ def _on_poisoned_output(fn):
         out = fn()
     finally:
         torch.empty, torch.empty_like = empty, empty_like
-    assert out.data_ptr() in ptrs, "the output was not allocated through torch.empty / torch.empty_like: nothing poisoned it"
+    for i, t in enumerate(out if isinstance(out, tuple) else (out,)):
+        assert t.data_ptr() in ptrs, "output %d was not allocated through torch.empty / torch.empty_like: nothing poisoned it" % i
     return out

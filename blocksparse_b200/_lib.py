@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libbsmm_b200.so")
 F32, F16, BF16 = 0, 1, 2
 FLAG_FORCE_GENERIC, FLAG_FORCE_TC = 1, 2
 MAX_PAIRS = 8
+E_NOKERNEL = -7          # BSMM_E_NOKERNEL: no fused kernel for the configuration
 
 _c = ctypes
 _vp, _i, _f = _c.c_void_p, _c.c_int, _c.c_float
@@ -34,6 +35,7 @@ SIGNATURES = {
     "bst_xn": (_i, [_i, _i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "bst_softmax": (_i, [_i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _f, _i, _i, _i, _vp]),
     "bst_softmax_grad": (_i, [_i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _f, _i, _i, _i, _vp]),
+    "bst_attention": (_i, [_i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp]),
     "bst_autoregressive_mask": (_i, [_i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_block_norm": (_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),

@@ -352,6 +352,21 @@ int bst_softmax_grad(int dtype, int dx_dtype, int bsize,
   return check_launch("bst_softmax_grad");
 }
 
+int bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                  const void* mask, int mask_heads, int autoregress_at_key,
+                  const void* q, const void* k, const void* v, void* o, float scale,
+                  int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k, void* stream) {
+  if (int e = check_bst(bsize, lut_heads, heads, head_state, batch, blocks)) return e;
+  if (!nn_lut || !q || !k || !v || !o) return fail(BSMM_E_ARG, "bst_attention: null pointer");
+  if (ctx_blks_q <= 0 || ctx_blks_k <= 0) return fail(BSMM_E_ARG, "bst_attention: bad context sizes");
+  if (autoregress_at_key >= 0 && !mask) return fail(BSMM_E_ARG, "bst_attention: autoregress_at_key needs a mask");
+  if (mask && mask_heads != 1 && mask_heads != heads) return fail(BSMM_E_ARG, "bst_attention: mask_heads must be 1 or heads");
+  // the fused kernel's envelope; the reason stays in bsmm_last_error()
+  const int rc = tc_bst_attention(dtype, bsize, nn_lut, lut_heads, blocks, mask, mask_heads, autoregress_at_key, q, k, v, o,
+                                  scale, batch, heads, head_state, ctx_blks_q, ctx_blks_k, (cudaStream_t)stream);
+  return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
+}
+
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,
                             const void* mask_in, void* mask_out, int autoregress_at_key, void* stream) {
   if (!nt_lut || !mask_in || !mask_out || lut_heads <= 0 || blocks <= 0)

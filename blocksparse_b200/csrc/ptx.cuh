@@ -197,6 +197,26 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t 
                    BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56)
                  : "l"(a), "l"(b), "n"(TA), "n"(TB));
 }
+// D[64 x 64] (fp32, registers) += A[64 x 16] * B[16 x 64] with A in registers: four b32 per thread, each two 16-bit
+// elements, low half first.  Fragment layout (PTX ISA, register fragment of matrix A for .f16 / .bf16 wgmma):
+//   a[h + 2i] = A[16w + l/4 + 8h][8i + 2(l%4) + {0,1}]      (h, i in {0, 1})
+// i.e. the accumulator layout above for the two 8-column groups j = 2kk, 2kk + 1 of a K = 16 slice: a[r] packs
+// d[8kk + 2r], d[8kk + 2r + 1].  B comes from shared memory (TB: 0 = K-major, 1 = MN-major).
+template <bool BF16, int TB>
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
+  if constexpr (BF16)
+    asm volatile(BSMM_WG_TAIL("bf16", 64)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, %37;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24)
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "n"(TB));
+  else
+    asm volatile(BSMM_WG_TAIL("f16", 64)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, %37;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24)
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "n"(TB));
+}
 // N = 16, 32, 64 or 128 dispatch
 template <bool BF16, int TA, int TB, int N>
 __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b) {

@@ -298,3 +298,4 @@ inline int tc_xprop(int dtype, int axis, int bsize, int bprop, const int32_t* lu
 #include "tc_xprop2.cuh"
 #include "tc_updat.cuh"
 #include "tc_bst.cuh"
+#include "tc_bst_attn.cuh"

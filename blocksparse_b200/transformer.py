@@ -158,6 +158,33 @@ class BlocksparseTransformer(TransformerCheckers):
         _lib.check(rc, "bst_softmax_grad")
         return dx
 
+    @_lib.guarded
+    def _attention(self, q, k, v, scale, autoregress_at_key):
+        """Fused NT -> (masked) softmax -> NN in one launch, or None where the library has no fused kernel for the
+        call (BSMM_E_NOKERNEL): the caller then composes the three ops."""
+        lib = _lib.load()
+        if not q.is_cuda:
+            raise _lib.BsmmError("BlocksparseTransformer needs CUDA tensors (no CPU path)")
+        q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+        batch, ctx_q, S = q.shape
+        if ctx_q != self.ctx_blks_q * self.blk_size or k.shape[1] != self.ctx_blks_k * self.blk_size:
+            raise ValueError("context sizes do not match the layout")
+        if S % self.heads or tuple(k.shape) != (batch, k.shape[1], S) or v.shape != k.shape or q.dtype != k.dtype:
+            raise ValueError("state size / dtype mismatch")
+        o = torch.empty((batch, ctx_q, S), dtype=v.dtype, device=v.device)
+        d = self._device_luts(q.device)
+        ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
+        # one dtype code stands for q, k and v; mixed dtypes name none, and the library answers with E_NOKERNEL
+        dt = _lib.dtype_code(q.dtype) if v.dtype == q.dtype else -1
+        rc = lib.bst_attention(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
+                               _lib.ptr(d["mask"]), self.lut_heads, ak,
+                               q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), float(scale),
+                               batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k, _lib.stream_ptr())
+        if rc == _lib.E_NOKERNEL:
+            return None
+        _lib.check(rc, "bst_attention")
+        return o
+
     def partial_autoregressive_mask(self, autoregress_at_key, device="cuda"):
         """Device mask rewritten so causality starts at key `autoregress_at_key` (bst_op.cc:519-575).
 
@@ -233,6 +260,20 @@ class BlocksparseTransformer(TransformerCheckers):
         dtype = dtype or self.softmax_dtype or x.dtype
         return _SoftmaxFunction.apply(x, self, float(scale), False, None, dtype)
 
+    def attention(self, q, k, v, scale=1.0, autoregress_at_key=None):
+        """weight_value_op(masked_softmax(query_key_op(q, k), scale, autoregress_at_key), v) -- softmax without a
+        mask_callback -- as one fused kernel that never writes the (batch, heads, blocks, bs, bs) scores or
+        probabilities; the backward pass recomputes them from q and k. Returns (batch, ctx_q, heads*head_state) in
+        v.dtype. Configurations without a fused kernel (fp32, mixed dtypes, block size other than 64, head_state other
+        than 64 / 128, unaligned tensors) run the three ops instead."""
+        if autoregress_at_key is not None and self.softmax_mask_np is None:
+            raise ValueError("autoregress_at_key only applies to ops with mask_callback defined.")
+        try:
+            return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key)
+        except _NoFusedKernel:
+            w = self.query_key_op(q, k)
+            return self.weight_value_op(self.masked_softmax(w, scale, autoregress_at_key), v)
+
 
 class _NtFunction(torch.autograd.Function):
     """reference transformer.py:391-416: d(a.b^T) -> db = dw^T.a (TN), da = dw.b (NN)."""
@@ -274,6 +315,43 @@ class _XnFunction(torch.autograd.Function):
             # NN: dw[blk] = dy[q-blk] . v[k-blk]^T ; TN: dw[blk] = v[q-blk] . dy[k-blk]^T
             dw = bst._nt(v, dy, w.dtype) if ctx.transpose else bst._nt(dy, v, w.dtype)
         return dw, dv, None, None
+
+
+class _NoFusedKernel(Exception):
+    """The library has no fused attention kernel for the call."""
+
+
+class _AttentionFunction(torch.autograd.Function):
+    """Fused attention. Saves q, k and v only; the backward recomputes the scores and the probabilities with the
+    chain's own NT and softmax kernels, then runs the chain's backward ops (_XnFunction, _SoftmaxFunction and
+    _NtFunction in turn) on them, so its gradients are bit-identical to the three-op chain's."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, bst, scale, autoregress_at_key):
+        o = bst._attention(q, k, v, scale, autoregress_at_key)
+        if o is None:
+            raise _NoFusedKernel()
+        ctx.bst, ctx.scale, ctx.ak = bst, scale, autoregress_at_key
+        ctx.save_for_backward(q, k, v)
+        return o
+
+    @staticmethod
+    def backward(ctx, dy):
+        q, k, v = ctx.saved_tensors
+        bst, scale = ctx.bst, ctx.scale
+        dy = dy.contiguous()
+        # forward of the chain up to the probabilities: bf16 scores, probabilities in q's dtype (query_key_op)
+        p = bst._softmax(bst._nt(q, k, torch.bfloat16), scale, bst.softmax_mask_np is not None, ctx.ak, q.dtype)
+        dq = dk = dv = None
+        if ctx.needs_input_grad[2]:
+            dv = bst._xn(p, dy, True)
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+            dw = bst._softmax_grad(bst._nt(dy, v, p.dtype), p, scale).to(torch.bfloat16).contiguous()
+            if ctx.needs_input_grad[1]:
+                dk = bst._xn(dw, q, True)
+            if ctx.needs_input_grad[0]:
+                dq = bst._xn(dw, k, False)
+        return dq, dk, dv, None, None, None
 
 
 class _SoftmaxFunction(torch.autograd.Function):

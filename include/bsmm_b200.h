@@ -18,6 +18,7 @@
  *   bst_softmax           <- BlocksparseMaskedSoftmax<T,V> (src/bst_op.cc:331-340,374-428)
  *   bst_softmax_grad      <- BlocksparseSoftmaxGrad<T,V>   (src/bst_op.cc:443-512)
  *   bst_autoregressive_mask <- BstPartialAutoregressiveMask (src/bst_op.cc:519-575)
+ *   bst_attention         <- no single launcher: replaces bst_nt + bst_masked_softmax + bst_xn (NN)
  *   bsmm_block_norm / bsmm_l2_decay / bsmm_threshold_prune / bsmm_prune_topk
  *                         <- BlocksparseNorm / BlocksparseL2Decay / BlocksparseThresholdPrune / BlocksparsePrune
  *                            (src/optimize_op_gpu.cu:794-1098)
@@ -65,7 +66,8 @@ enum {
   BSMM_E_ARG     = -3,   /* null pointer, negative size, pcount > 8 …  */
   BSMM_E_LIMIT   = -4,   /* size limit exceeded (mirrors reference OP_REQUIRES) */
   BSMM_E_NODEV   = -5,   /* no sm_90 device / driver entry point missing */
-  BSMM_E_ALIGN   = -6    /* pointer or leading dimension not aligned as the tensor-core path needs */
+  BSMM_E_ALIGN   = -6,   /* pointer or leading dimension not aligned as the tensor-core path needs */
+  BSMM_E_NOKERNEL = -7   /* no fused kernel for this configuration; compose the op from the others */
 };
 
 /* flags for bsmm_xprop / bsmm_updat / bst_* */
@@ -202,6 +204,24 @@ int bst_softmax_grad(int dtype, int dx_dtype, int bsize,
                      const int32_t* nn_lut, int lut_heads, int blocks, int max_lut,
                      const void* dy, const void* y, void* dx, float scale,
                      int batch, int heads, int ctx_blks_q, void* stream);
+
+/*
+ * Fused attention: o = NN(softmax(NT(q, k), scale, mask), v), i.e. the composition bst_nt + bst_masked_softmax +
+ * bst_xn(NN) in one launch that never writes the scores or the probabilities.  No single reference launcher
+ * corresponds to it.
+ *   q, o: (batch, ctx_blks_q*bsize, heads*head_state), k, v: (batch, ctx_blks_k*bsize, heads*head_state).
+ *   nn_lut, mask, mask_heads, autoregress_at_key: as bst_softmax (autoregress_at_key >= 0 needs a mask).
+ *   Masked keys score -FLT_MAX, so a row that sees no key gets uniform weights over its blocks' keys; a query block
+ *   with an empty LUT row is written as zeros.  Rows of any length.  Scores stay in fp32, the probabilities enter the
+ *   second product in `dtype`.
+ * dtype is the dtype of q, k, v and o alike.  Returns BSMM_E_NOKERNEL, launching nothing, unless dtype is BSMM_F16
+ * or BSMM_BF16 (a caller whose tensors differ in dtype passes any other value), bsize is 64, head_state is 64 or
+ * 128, every pointer is 16-byte aligned and the device is sm_90; the caller then composes the three ops.
+ */
+int bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                  const void* mask, int mask_heads, int autoregress_at_key,
+                  const void* q, const void* k, const void* v, void* o, float scale,
+                  int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k, void* stream);
 
 /* mask_out[hl][blk][r] = mask_in[hl][blk][r] & (ones >> shift(r)), same layout as bst_softmax's mask */
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,

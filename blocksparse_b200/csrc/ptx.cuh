@@ -24,6 +24,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -94,6 +97,16 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 }
 __device__ __forceinline__ void cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+// ---- register reallocation between warpgroups --------------------------------------------
+// Executed by every warp of a warpgroup: lowers (dec) or raises (inc) its per-thread register limit to R (a multiple
+// of 8 in [24, 256]); an inc blocks until the registers released by a dec are free.
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
 }
 
 // ---- wgmma ---------------------------------------------------------------------------------
@@ -197,6 +210,66 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t 
                    BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56)
                  : "l"(a), "l"(b), "n"(TA), "n"(TB));
 }
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_n192(float (&d)[96], uint64_t a, uint64_t b) {
+  if constexpr (BF16)
+    asm volatile(BSMM_WG_TAIL("bf16", 192)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+                 "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+                 "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+                 "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95}, %96, %97, p, 1, 1, %98, %99;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24),
+                   BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56),
+                   BSMM_WG_OPS8(64), BSMM_WG_OPS8(72), BSMM_WG_OPS8(80), BSMM_WG_OPS8(88)
+                 : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  else
+    asm volatile(BSMM_WG_TAIL("f16", 192)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+                 "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+                 "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+                 "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95}, %96, %97, p, 1, 1, %98, %99;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24),
+                   BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56),
+                   BSMM_WG_OPS8(64), BSMM_WG_OPS8(72), BSMM_WG_OPS8(80), BSMM_WG_OPS8(88)
+                 : "l"(a), "l"(b), "n"(TA), "n"(TB));
+}
+template <bool BF16, int TA, int TB>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t a, uint64_t b) {
+  if constexpr (BF16)
+    asm volatile(BSMM_WG_TAIL("bf16", 256)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+                 "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+                 "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+                 "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+                 "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+                 "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, %130, %131;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24),
+                   BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56),
+                   BSMM_WG_OPS8(64), BSMM_WG_OPS8(72), BSMM_WG_OPS8(80), BSMM_WG_OPS8(88),
+                   BSMM_WG_OPS8(96), BSMM_WG_OPS8(104), BSMM_WG_OPS8(112), BSMM_WG_OPS8(120)
+                 : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  else
+    asm volatile(BSMM_WG_TAIL("f16", 256)
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+                 "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+                 "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+                 "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+                 "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+                 "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, %130, %131;\n\t}\n"
+                 : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24),
+                   BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56),
+                   BSMM_WG_OPS8(64), BSMM_WG_OPS8(72), BSMM_WG_OPS8(80), BSMM_WG_OPS8(88),
+                   BSMM_WG_OPS8(96), BSMM_WG_OPS8(104), BSMM_WG_OPS8(112), BSMM_WG_OPS8(120)
+                 : "l"(a), "l"(b), "n"(TA), "n"(TB));
+}
 // D[64 x 64] (fp32, registers) += A[64 x 16] * B[16 x 64] with A in registers: four b32 per thread, each two 16-bit
 // elements, low half first.  Fragment layout (PTX ISA, register fragment of matrix A for .f16 / .bf16 wgmma):
 //   a[h + 2i] = A[16w + l/4 + 8h][8i + 2(l%4) + {0,1}]      (h, i in {0, 1})
@@ -217,13 +290,15 @@ __device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)
                  : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24)
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "n"(TB));
 }
-// N = 16, 32, 64 or 128 dispatch
+// N = 16, 32, 64, 128, 192 or 256 dispatch
 template <bool BF16, int TA, int TB, int N>
 __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b) {
   if constexpr (N == 16) wgmma_n16<BF16, TA, TB>(d, a, b);
   else if constexpr (N == 32) wgmma_n32<BF16, TA, TB>(d, a, b);
   else if constexpr (N == 64) wgmma_n64<BF16, TA, TB>(d, a, b);
-  else wgmma_n128<BF16, TA, TB>(d, a, b);
+  else if constexpr (N == 128) wgmma_n128<BF16, TA, TB>(d, a, b);
+  else if constexpr (N == 192) wgmma_n192<BF16, TA, TB>(d, a, b);
+  else wgmma_n256<BF16, TA, TB>(d, a, b);
 }
 #undef BSMM_WG_TAIL
 #undef BSMM_WG_OPS8

@@ -4,29 +4,40 @@
 //   (reference src/blocksparse_hgemm_nc_op_gpu.cu:553-897) and their Volta parameter-bank hack.
 //
 // Formulation ("gathered dense GEMM", schedule = blocksparse_b200/lut.py:build_updat_schedule):
-//   M axis   = 128 input features = a group of 128/bs consecutive input blocks; warpgroup g owns features 64g..64g+63
+//   M axis   = 128 input features = a group of 128/bs consecutive input blocks; consumer warpgroup c owns features
+//              64c..64c+63
 //   N axis   = the output blocks that have at least one active block in that group, COMPACTED side by side in
-//              shared memory (n_act*bs <= 256 columns, multiplied in 64-column wgmma chunks: absent slots cost nothing)
+//              shared memory (n_act*bs <= 256 columns); every K=16 step is ONE wgmma of N = 64, 128, 192 or 256, the
+//              narrowest that holds the kept blocks, so the A slice is read once per step and absent slots cost nothing
 //   K axis   = the minibatch (reduction), 64 rows per pipeline stage, 4 wgmma K=16 steps per stage
 // Output blocks with nothing to update are neither loaded nor multiplied, and the reference's one-CTA-per-block
 // re-read of X and DY becomes one pass per (group, window).  The epilogue writes only the blocks that exist.
-//   axis 1: A = X[n][c] (MN-major, two 64-feature boxes), B = DY[n][k] (MN-major, one box per kept block).
+//   axis 1: A = X[n][c] (MN-major, two 64-feature boxes), B = DY[n][k] (MN-major, one box per kept block: the slots
+//           are the MN atoms of B, BSLOT bytes apart).
 //   axis 0: A = X[c][n], B = DY[k][n]: both K-major with 128-byte rows; kept blocks continue the row index.
+//
+// Warp-specialized and persistent: min(tiles, SMs) CTAs, CTA b runs tiles b, b + gridDim.x, ... (the schedule lists
+// them longest first, and lut.py:_balance_windows sizes the windows for exactly this deal).  Warpgroup 0 is the producer:
+// one thread streams the stages of all the CTA's tiles through a ring guarded by full / empty mbarriers, running ahead
+// into the next tile while the consumers write the previous one out.  Warpgroups 1 and 2 multiply; each consumer warp
+// releases a stage as soon as wgmma.wait_group has retired the MMAs that read it.  No CTA-wide barrier after set-up.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace bsmm {
 
-constexpr int UPDAT_THREADS = 2 * 128;  // two warpgroups
+constexpr int UPDAT_THREADS = 3 * 128;  // one producer warpgroup, two consumer warpgroups
 constexpr int UPDAT_STAGES = 4;
 constexpr int UPDAT_KCHUNK = 64;        // minibatch rows per stage
+constexpr int UPDAT_PRODUCER_REGS = 40, UPDAT_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 // record layout of lut.py:build_updat_schedule: 64 ints for <= 8 slots per tile (bs 32 / 64), 192 for the 16 slots of bs 16
 __host__ __device__ constexpr int updat_rec_ints(int bs) { return bs >= 32 ? 64 : 192; }
 __host__ __device__ constexpr int updat_tab_off(int bs) { return bs >= 32 ? 16 : 32; }
 
 struct UpdatTcParams {
   const int32_t* sched;     // build_updat_schedule
+  int n_tiles;
   int N;                    // minibatch rows per pair
   int pcount;
   float alpha, beta;
@@ -36,110 +47,66 @@ struct UpdatTcParams {
 };
 struct UpdatTmaps { CUtensorMap x[BSMM_MAX_PAIRS]; CUtensorMap dy[BSMM_MAX_PAIRS]; };
 
-template <int BS>
-constexpr size_t updat_smem_bytes() {
-  return (size_t)UPDAT_STAGES * (128 * UPDAT_KCHUNK * 2 + 256 * UPDAT_KCHUNK * 2) + SMEM_ALIGN_SLACK;
-}
+template <int BS> struct UpdatShape {
+  static constexpr uint32_t ABYTES = 128 * UPDAT_KCHUNK * 2;     // 16 KB: 128 features
+  static constexpr uint32_t BSLOT = BS * UPDAT_KCHUNK * 2;       // one kept output block
+  static constexpr uint32_t STAGE = ABYTES + (256 / BS) * BSLOT; // 48 KB
+  static constexpr size_t SMEM = UPDAT_STAGES * STAGE + SMEM_ALIGN_SLACK;
+};
 
-template <int BS, bool BF16, bool AXIS0, typename TO>
-__global__ void __launch_bounds__(UPDAT_THREADS, 1)
-tc_updat_kernel(const UpdatTcParams p, const __grid_constant__ UpdatTmaps maps) {
-  constexpr int ST = UPDAT_STAGES;
-  constexpr int KT = 256 / BS;                        // slots per tile
-  constexpr uint32_t ABYTES = 128 * UPDAT_KCHUNK * 2; // 16 KB
-  constexpr uint32_t BSLOT = BS * UPDAT_KCHUNK * 2;   // one kept output block
-  constexpr uint32_t STAGE_BYTES = ABYTES + KT * BSLOT;
+// One tile of one consumer warpgroup: features 64cw..64cw+63 of the group x NCH*64 compacted columns, reduced over
+// the n_chunks stages at ring positions g0, g0 + 1, ...; then its part of the epilogue.
+template <int NCH, int BS, bool BF16, bool AXIS0, typename TO>
+__device__ __forceinline__ void updat_tile(const UpdatTcParams& p, const int32_t* rec, int n_act, uint32_t base,
+                                           uint64_t* full, uint64_t* empty, int g0, int n_chunks, int cw, int warp, int lane) {
+  using Sh = UpdatShape<BS>;
+  constexpr int ST = UPDAT_STAGES, KT = 256 / BS, TAB = updat_tab_off(BS);
   constexpr uint32_t B_ROW = BS * 2;                  // axis 1: bytes per row of a DY box
-  constexpr int REC = updat_rec_ints(BS), TAB = updat_tab_off(BS);
-
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t full[ST];
-  __shared__ int rec[REC];
-  const uint32_t base = aligned_smem_base(smem_raw);
-  const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32, wg = warp / 4;
-  const int chunks_per_pair = (p.N + UPDAT_KCHUNK - 1) / UPDAT_KCHUNK;
-  const int n_chunks = chunks_per_pair * p.pcount;
-
-  for (int i = tid; i < REC; i += UPDAT_THREADS) rec[i] = p.sched[4 + (size_t)blockIdx.x * REC + i];
-  if (tid == 0) {
-    for (int i = 0; i < ST; ++i) ptx::mbar_init(&full[i], 1);
-    ptx::fence_mbar_init();
-  }
-  __syncthreads();
-  const int c0 = rec[0], n_act = rec[1];
-  const int nch = (n_act * BS + 63) / 64;             // 64-column wgmma chunks holding kept blocks
-
-  auto issue = [&](int ch) {                          // one thread: stage minibatch chunk ch
-    const uint32_t st = base + (uint32_t)(ch % ST) * STAGE_BYTES;
-    uint64_t* bar = &full[ch % ST];
-    const int pair = ch / chunks_per_pair;
-    const int n0 = (ch % chunks_per_pair) * UPDAT_KCHUNK;
-    ptx::mbar_expect_tx(bar, ABYTES + (uint32_t)n_act * BSLOT);
-    if (!AXIS0) {
-      ptx::tma_load_2d(st, &maps.x[pair], bar, c0 * BS, n0);
-      ptx::tma_load_2d(st + ABYTES / 2, &maps.x[pair], bar, c0 * BS + 64, n0);
-      for (int s = 0; s < n_act; ++s) ptx::tma_load_2d(st + ABYTES + s * BSLOT, &maps.dy[pair], bar, rec[8 + s] * BS, n0);
-    } else {                                          // [128 features][64 n], 128-byte rows
-      ptx::tma_load_2d(st, &maps.x[pair], bar, n0, c0 * BS);
-      for (int s = 0; s < n_act; ++s) ptx::tma_load_2d(st + ABYTES + s * BSLOT, &maps.dy[pair], bar, n0, rec[8 + s] * BS);
-    }
-  };
-  if (tid == 0)
-    for (int ch = 0; ch < n_chunks && ch < ST; ++ch) issue(ch);
-
-  float acc[4][32];
+  float acc[NCH * 32];
 #pragma unroll
-  for (int q = 0; q < 4; ++q)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
+  for (int i = 0; i < NCH * 32; ++i) acc[i] = 0.f;
 
   for (int ch = 0; ch < n_chunks; ++ch) {
-    const uint32_t st = base + (uint32_t)(ch % ST) * STAGE_BYTES;
-    if (!ptx::mbar_wait(&full[ch % ST], (uint32_t)(ch / ST) & 1)) g_tc_error = 11;
+    const int g = g0 + ch;
+    const uint32_t st = base + (uint32_t)(g % ST) * Sh::STAGE;
+    if (!ptx::mbar_wait(&full[g % ST], (uint32_t)(g / ST) & 1)) g_tc_error = 11;
     ptx::wg_fence();
 #pragma unroll
     for (int ks = 0; ks < UPDAT_KCHUNK / 16; ++ks) {
-      const uint64_t adesc = AXIS0 ? ptx::make_desc(st + wg * (ABYTES / 2) + ks * 32, 16, 1024, ptx::SWZ_128B)
-                                   : ptx::make_desc(st + wg * (ABYTES / 2) + ks * 2048, ABYTES / 2, 1024, ptx::SWZ_128B);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        if (q < nch) {                                // uniform across the CTA
-          const uint32_t b0 = st + ABYTES + q * 8192;  // 64 columns = 64 rows of 128 bytes (axis 0) or 64/BS slots (axis 1)
-          const uint64_t bdesc = AXIS0 ? ptx::make_desc(b0 + ks * 32, 16, 1024, ptx::SWZ_128B)
-                                       : ptx::make_desc(b0 + ks * 16 * B_ROW, BSLOT, 8 * B_ROW, ptx::swz_for_row(B_ROW));
-          if (AXIS0) ptx::wgmma_n64<BF16, 0, 0>(acc[q], adesc, bdesc);
-          else       ptx::wgmma_n64<BF16, 1, 1>(acc[q], adesc, bdesc);
-        }
-      }
+      const uint64_t adesc = AXIS0 ? ptx::make_desc(st + cw * (Sh::ABYTES / 2) + ks * 32, 16, 1024, ptx::SWZ_128B)
+                                   : ptx::make_desc(st + cw * (Sh::ABYTES / 2) + ks * 2048, Sh::ABYTES / 2, 1024, ptx::SWZ_128B);
+      const uint64_t bdesc = AXIS0 ? ptx::make_desc(st + Sh::ABYTES + ks * 32, 16, 1024, ptx::SWZ_128B)
+                                   : ptx::make_desc(st + Sh::ABYTES + ks * 16 * B_ROW, Sh::BSLOT, 8 * B_ROW, ptx::swz_for_row(B_ROW));
+      ptx::wgmma<BF16, AXIS0 ? 0 : 1, AXIS0 ? 0 : 1, NCH * 64>(acc, adesc, bdesc);
     }
     ptx::wg_commit();
-    ptx::wg_wait<1>();
-    __syncthreads();
-    if (tid == 0 && ch >= 1 && ch - 1 + ST < n_chunks) issue(ch - 1 + ST);
+    ptx::wg_wait<1>();                                // the MMAs of the previous stage have retired: hand it back
+    if (ch > 0 && lane == 0) ptx::mbar_arrive(&empty[(g - 1) % ST]);
   }
   ptx::wg_wait<0>();
-#pragma unroll
-  for (int q = 0; q < 4; ++q) ptx::wg_fence_regs(acc[q]);
+  if (lane == 0) ptx::mbar_arrive(&empty[(g0 + n_chunks - 1) % ST]);
+  ptx::wg_fence_regs(acc);
 
-  // epilogue: accumulator (feature row r of the group, column c) -> DW[w][r % BS][c % BS], w from the record's table
+  // epilogue: accumulator (feature row r of the group, column c) -> DW[w][r % BS][c % BS], w from the record's table.
+  // Accumulator column 8J + 2(lane % 4) + e sits in acc[4J + 2h + e] (rows r0, r0 + 8), so slot s holds J in
+  // [s*BS/8, (s+1)*BS/8).  Both rows lie in one input block (BS >= 16): one table row per thread.
   TO* dw = reinterpret_cast<TO*>(p.dw);
+  const int r0 = cw * 64 + warp * 16 + lane / 4;
+  const int32_t* wid = rec + TAB + (r0 / BS) * KT;
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    if (q >= nch) continue;
+  for (int s = 0; s < NCH * 64 / BS; ++s) {
+    if (s >= n_act) break;
+    const int w = __ldg(wid + s);
+    if (w < 0) continue;
+    float g = p.alpha;
+    if (p.gated) g *= p.gate[w];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int col = q * 64 + 8 * j + 2 * (lane % 4);
-      const int s = col / BS, jj = col % BS;
-      if (s >= n_act) continue;
+    for (int jj = 0; jj < BS / 8; ++jj) {
+      const int J = s * (BS / 8) + jj;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int r = wg * 64 + (warp % 4) * 16 + lane / 4 + 8 * h;
-        const int w = rec[TAB + (r / BS) * KT + s];
-        if (w < 0) continue;
-        float g = p.alpha;
-        if (p.gated) g *= p.gate[w];
-        float a = acc[q][4 * j + 2 * h] * g, b = acc[q][4 * j + 2 * h + 1] * g;
-        TO* out = dw + ((size_t)w * BS + r % BS) * BS + jj;
+        float a = acc[4 * J + 2 * h] * g, b = acc[4 * J + 2 * h + 1] * g;
+        TO* out = dw + ((size_t)w * BS + (r0 + 8 * h) % BS) * BS + 8 * jj + 2 * (lane % 4);
         if constexpr (sizeof(TO) == 4) {
           float2* o2 = reinterpret_cast<float2*>(out);
           if (p.beta != 0.f) { const float2 old = *o2; a += old.x; b += old.y; }
@@ -159,18 +126,87 @@ tc_updat_kernel(const UpdatTcParams p, const __grid_constant__ UpdatTmaps maps) 
 }
 
 template <int BS, bool BF16, bool AXIS0, typename TO>
-int launch_tc_updat(const UpdatTcParams& p, const UpdatTmaps& maps, int n_tiles, cudaStream_t s) {
+__global__ void __launch_bounds__(UPDAT_THREADS, 1)
+tc_updat_kernel(const __grid_constant__ UpdatTcParams p, const __grid_constant__ UpdatTmaps maps) {
+  using Sh = UpdatShape<BS>;
+  constexpr int ST = UPDAT_STAGES, KT = 256 / BS, REC = updat_rec_ints(BS);
+
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ uint64_t full[ST], empty[ST];
+  __shared__ int kcol[KT];                            // producer only: first DY feature of each kept slot
+  const uint32_t base = aligned_smem_base(smem_raw);
+  const int tid = threadIdx.x, wg = tid / 128;
+  const int chunks_per_pair = (p.N + UPDAT_KCHUNK - 1) / UPDAT_KCHUNK;
+  const int n_chunks = chunks_per_pair * p.pcount;   // stages per tile
+
+  if (tid == 0) {
+    for (int i = 0; i < ST; ++i) {
+      ptx::mbar_init(&full[i], 1);
+      ptx::mbar_init(&empty[i], 8);                   // one arrival per consumer warp
+    }
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    ptx::setmaxnreg_dec<UPDAT_PRODUCER_REGS>();
+    if (tid != 0) return;
+    int g = 0;                                        // ring position, continued across the CTA's tiles
+    for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
+      const int32_t* rec = p.sched + 4 + (size_t)t * REC;
+      const int c0 = __ldg(rec) * BS, n_act = __ldg(rec + 1);
+      for (int s = 0; s < n_act; ++s) kcol[s] = __ldg(rec + 8 + s) * BS;
+      const uint32_t tx = Sh::ABYTES + (uint32_t)n_act * Sh::BSLOT;
+      for (int ch = 0; ch < n_chunks; ++ch, ++g) {
+        const int slot = g % ST;
+        if (g >= ST && !ptx::mbar_wait(&empty[slot], (uint32_t)(g / ST - 1) & 1)) g_tc_error = 12;
+        const uint32_t st = base + (uint32_t)slot * Sh::STAGE;
+        uint64_t* bar = &full[slot];
+        const int pair = ch / chunks_per_pair;
+        const int n0 = (ch % chunks_per_pair) * UPDAT_KCHUNK;
+        ptx::mbar_expect_tx(bar, tx);
+        if (!AXIS0) {
+          ptx::tma_load_2d(st, &maps.x[pair], bar, c0, n0);
+          ptx::tma_load_2d(st + Sh::ABYTES / 2, &maps.x[pair], bar, c0 + 64, n0);
+          for (int s = 0; s < n_act; ++s) ptx::tma_load_2d(st + Sh::ABYTES + s * Sh::BSLOT, &maps.dy[pair], bar, kcol[s], n0);
+        } else {                                      // [128 features][64 n], 128-byte rows
+          ptx::tma_load_2d(st, &maps.x[pair], bar, n0, c0);
+          for (int s = 0; s < n_act; ++s) ptx::tma_load_2d(st + Sh::ABYTES + s * Sh::BSLOT, &maps.dy[pair], bar, n0, kcol[s]);
+        }
+      }
+    }
+    return;
+  }
+
+  ptx::setmaxnreg_inc<UPDAT_CONSUMER_REGS>();
+  const int cw = wg - 1, warp = (tid / 32) % 4, lane = tid % 32;
+  int g = 0;
+  for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x, g += n_chunks) {
+    const int32_t* rec = p.sched + 4 + (size_t)t * REC;
+    const int n_act = __ldg(rec + 1);
+    switch ((n_act * BS + 63) / 64) {                 // MMA width: the 64-column chunks holding kept blocks
+      case 1:  updat_tile<1, BS, BF16, AXIS0, TO>(p, rec, n_act, base, full, empty, g, n_chunks, cw, warp, lane); break;
+      case 2:  updat_tile<2, BS, BF16, AXIS0, TO>(p, rec, n_act, base, full, empty, g, n_chunks, cw, warp, lane); break;
+      case 3:  updat_tile<3, BS, BF16, AXIS0, TO>(p, rec, n_act, base, full, empty, g, n_chunks, cw, warp, lane); break;
+      default: updat_tile<4, BS, BF16, AXIS0, TO>(p, rec, n_act, base, full, empty, g, n_chunks, cw, warp, lane); break;
+    }
+  }
+}
+
+template <int BS, bool BF16, bool AXIS0, typename TO>
+int launch_tc_updat(const UpdatTcParams& p, const UpdatTmaps& maps, cudaStream_t s) {
   auto kern = tc_updat_kernel<BS, BF16, AXIS0, TO>;
-  constexpr size_t smem = updat_smem_bytes<BS>();
+  constexpr size_t smem = UpdatShape<BS>::SMEM;
   static thread_local uint64_t configured = 0;
   if (int e = ensure_dyn_smem(kern, smem, configured)) return e;
-  kern<<<n_tiles, UPDAT_THREADS, smem, s>>>(p, maps);
+  const int grid = p.n_tiles < device_info().sm_grid ? p.n_tiles : device_info().sm_grid;
+  kern<<<grid, UPDAT_THREADS, smem, s>>>(p, maps);
   return check_launch(BS == 16 ? "wgmma_updat_bs16" : BS == 32 ? "wgmma_updat_bs32" : "wgmma_updat_bs64");
 }
 
 template <int BS, bool BF16, typename TO>
-int dispatch_tc_updat(const UpdatTcParams& p, const UpdatTmaps& maps, int n_tiles, bool axis0, cudaStream_t s) {
-  return axis0 ? launch_tc_updat<BS, BF16, true, TO>(p, maps, n_tiles, s) : launch_tc_updat<BS, BF16, false, TO>(p, maps, n_tiles, s);
+int dispatch_tc_updat(const UpdatTcParams& p, const UpdatTmaps& maps, bool axis0, cudaStream_t s) {
+  return axis0 ? launch_tc_updat<BS, BF16, true, TO>(p, maps, s) : launch_tc_updat<BS, BF16, false, TO>(p, maps, s);
 }
 
 inline int tc_updat(int dtype, int dw_dtype, int axis, int bsize, int n_c_blocks, int n_k_blocks,
@@ -201,15 +237,15 @@ inline int tc_updat(int dtype, int dw_dtype, int axis, int bsize, int n_c_blocks
     }
   }
   UpdatTcParams p;
-  p.sched = sched; p.N = N; p.pcount = pcount;
+  p.sched = sched; p.n_tiles = sched_tiles; p.N = N; p.pcount = pcount;
   p.alpha = alpha; p.beta = beta; p.gate = gate; p.gated = (gated_dw && gate) ? 1 : 0; p.dw = dw;
   const bool bf = dtype == BSMM_BF16, a0 = axis == 0;
   const bool f32out = dw_dtype == BSMM_F32;
 #define BSMM_UPDAT_BS(BSV)                                                                                            \
-  if (f32out) return bf ? dispatch_tc_updat<BSV, true, float>(p, maps, sched_tiles, a0, s)                            \
-                        : dispatch_tc_updat<BSV, false, float>(p, maps, sched_tiles, a0, s);                          \
-  return bf ? dispatch_tc_updat<BSV, true, __nv_bfloat16>(p, maps, sched_tiles, a0, s)                                \
-            : dispatch_tc_updat<BSV, false, __half>(p, maps, sched_tiles, a0, s);
+  if (f32out) return bf ? dispatch_tc_updat<BSV, true, float>(p, maps, a0, s)                            \
+                        : dispatch_tc_updat<BSV, false, float>(p, maps, a0, s);                          \
+  return bf ? dispatch_tc_updat<BSV, true, __nv_bfloat16>(p, maps, a0, s)                                \
+            : dispatch_tc_updat<BSV, false, __half>(p, maps, a0, s);
   if (bsize == 16) { BSMM_UPDAT_BS(16) }
   if (bsize == 32) { BSMM_UPDAT_BS(32) }
   BSMM_UPDAT_BS(64)

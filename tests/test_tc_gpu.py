@@ -143,7 +143,7 @@ def test_gated_xprop_runs_on_tcgen05(bs):
 
 
 UPDAT_CASES = [
-    # CB, KB, density, N, bs, pairs[, "pos": operands uniform in (0, 1) | "sms3": schedule built for 3 SMs]
+    # CB, KB, density, N, bs, pairs[, "pos": operands uniform in (0, 1) | "sms3": host schedule balanced for 3 SMs]
     (8, 8, 0.3, 128, 32, 1),
     (5, 37, 0.5, 200, 32, 2),      # group of 4 input blocks is ragged (5 = 4 + 1), N not a multiple of 64
     (40, 33, 0.08, 1, 32, 1),
@@ -158,7 +158,9 @@ UPDAT_CASES = [
     (10, 12, 0.4, 136, 32, 3, "pos"),
     (9, 14, 0.4, 128, 16, 2, "pos"),
     (6, 9, 0.5, 130, 64, 1, "pos"),
-    (9, 40, 0.3, 200, 16, 2, "sms3"),   # _balance_windows splits groups into extra windows to fill whole waves
+    # "sms3" checks _balance_windows' extra windows only: the launch grid stays the device's (BSMM_SM_MARGIN), so each
+    # CTA still runs one tile. tests/test_updat_persistent_gpu.py runs CTAs over several tiles.
+    (9, 40, 0.3, 200, 16, 2, "sms3"),
     (64, 64, 0.2, 256, 32, 2, "sms3"),
 ]
 

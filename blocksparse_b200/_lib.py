@@ -36,6 +36,9 @@ SIGNATURES = {
     "bst_softmax": (_i, [_i, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _f, _i, _i, _i, _vp]),
     "bst_softmax_grad": (_i, [_i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _f, _i, _i, _i, _vp]),
     "bst_attention": (_i, [_i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp]),
+    "bst_attention_train": (_i, [_i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp]),
+    "bst_attention_grad": (_i, [_i, _i, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp]),
     "bst_autoregressive_mask": (_i, [_i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_block_norm": (_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),

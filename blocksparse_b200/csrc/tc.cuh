@@ -299,3 +299,4 @@ inline int tc_xprop(int dtype, int axis, int bsize, int bprop, const int32_t* lu
 #include "tc_updat.cuh"
 #include "tc_bst.cuh"
 #include "tc_bst_attn.cuh"
+#include "tc_bst_attn_bwd.cuh"

@@ -14,7 +14,8 @@
 //                      (as tc_bst_xn_kernel).
 // The stage of entry e is refilled with entry e + ST once O += P V of entry e has retired.  The epilogue divides by l
 // and stores 16-bit rows; an empty LUT row is written as zeros.  Accumulation follows LUT order: results are
-// deterministic.
+// deterministic.  With STATS the epilogue also stores every row's final running max m and full sum l, which the fused
+// backward (tc_bst_attn_bwd.cuh) needs to recompute P = exp(s - m) / l; o is the same either way.
 #pragma once
 #include <float.h>
 #include "softmax.cuh"
@@ -34,10 +35,12 @@ struct BstAttnParams {
   int n_q, heads, head_state;     // n_q = ctx_blks_q
   int ctx_rows_q, ctx_rows_k;
   void* o;
+  float* row_max;                 // STATS: [batch][heads][ctx_rows_q] final running max m and full sum l of each row
+  float* row_sum;
 };
 struct BstAttnTmaps { CUtensorMap q, k, v; };
 
-template <bool BF16, int CH>      // CH = head_state / 64
+template <bool BF16, int CH, bool STATS = false>      // CH = head_state / 64
 __global__ void __launch_bounds__(BST_THREADS)
 wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps maps) {
   constexpr int ST = BST_ATTN_STAGES;
@@ -185,6 +188,11 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
     sum += __shfl_xor_sync(0xffffffffu, sum, 2);
     const float inv = count > 0 ? 1.f / sum : 0.f;
     const int row = r0 + 8 * hh;
+    if (STATS && lane % 4 == 0) {                       // m is already the quad's common value
+      const long long r = ((long long)b * p.heads + h) * p.ctx_rows_q + qb * 64 + row;
+      p.row_max[r] = m[hh];
+      p.row_sum[r] = sum;
+    }
     uint16_t* out = obase + ((long long)b * p.ctx_rows_q + qb * 64 + row) * S + col0;
 #pragma unroll
     for (int c = 0; c < CH; ++c)
@@ -200,7 +208,7 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
 inline int tc_bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks, const void* mask,
                             int mask_heads, int autoregress_at_key, const void* q, const void* k, const void* v, void* o,
                             float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
-                            cudaStream_t s) {
+                            cudaStream_t s, float* row_max = nullptr, float* row_sum = nullptr) {
   if ((uintptr_t)o & 15) { fail(0, "pointers must be 16-byte aligned for TMA"); return TC_NOT_APPLICABLE; }
   if (!bst_tc_applicable(dtype, bsize, head_state, q, k, v)) return TC_NOT_APPLICABLE;
   const uint64_t S = (uint64_t)heads * head_state;
@@ -215,19 +223,24 @@ inline int tc_bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut
   p.autoregress_at_key = autoregress_at_key; p.scale = scale;
   p.n_q = ctx_blks_q; p.heads = heads; p.head_state = head_state;
   p.ctx_rows_q = ctx_blks_q * 64; p.ctx_rows_k = ctx_blks_k * 64; p.o = o;
+  p.row_max = row_max; p.row_sum = row_sum;
+  const bool stats = row_max != nullptr;
   const int ch = head_state / 64;
   const size_t smem = (size_t)(1 + 2 * BST_ATTN_STAGES) * ch * BST_TILE + SMEM_ALIGN_SLACK;
   const unsigned grid = (unsigned)((long long)batch * heads * ctx_blks_q);
-#define BSMM_LAUNCH_ATTN(BFV, CHV)                                                       \
-  { auto kern = wgmma_bst_attention<BFV, CHV>;                                           \
+#define BSMM_LAUNCH_ATTN(BFV, CHV, STV)                                                  \
+  { auto kern = wgmma_bst_attention<BFV, CHV, STV>;                                      \
     static thread_local uint64_t cfg = 0;                                                \
     if (int e = ensure_dyn_smem(kern, smem, cfg)) return e;                              \
     kern<<<grid, BST_THREADS, smem, s>>>(p, maps); }
+#define BSMM_LAUNCH_ATTN_CH(BFV, STV) \
+  { if (ch == 2) BSMM_LAUNCH_ATTN(BFV, 2, STV) else BSMM_LAUNCH_ATTN(BFV, 1, STV) }
   const bool bf = dtype == BSMM_BF16;
-  if (ch == 2) { if (bf) BSMM_LAUNCH_ATTN(true, 2) else BSMM_LAUNCH_ATTN(false, 2) }
-  else { if (bf) BSMM_LAUNCH_ATTN(true, 1) else BSMM_LAUNCH_ATTN(false, 1) }
+  if (stats) { if (bf) BSMM_LAUNCH_ATTN_CH(true, true) else BSMM_LAUNCH_ATTN_CH(false, true) }
+  else { if (bf) BSMM_LAUNCH_ATTN_CH(true, false) else BSMM_LAUNCH_ATTN_CH(false, false) }
+#undef BSMM_LAUNCH_ATTN_CH
 #undef BSMM_LAUNCH_ATTN
-  return check_launch("wgmma_bst_attention");
+  return check_launch(stats ? "wgmma_bst_attention_train" : "wgmma_bst_attention");
 }
 
 }  // namespace bsmm

@@ -185,6 +185,56 @@ class BlocksparseTransformer(TransformerCheckers):
         _lib.check(rc, "bst_attention")
         return o
 
+    @_lib.guarded
+    def _attention_train(self, q, k, v, scale, autoregress_at_key):
+        """_attention that also returns each query row's softmax statistics (max m and sum l, float32
+        (batch, heads, ctx_q)) for _attention_grad; None where the library has no fused kernel for the call."""
+        lib = _lib.load()
+        if not q.is_cuda:
+            raise _lib.BsmmError("BlocksparseTransformer needs CUDA tensors (no CPU path)")
+        q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+        batch, ctx_q, S = q.shape
+        if ctx_q != self.ctx_blks_q * self.blk_size or k.shape[1] != self.ctx_blks_k * self.blk_size:
+            raise ValueError("context sizes do not match the layout")
+        if S % self.heads or tuple(k.shape) != (batch, k.shape[1], S) or v.shape != k.shape or q.dtype != k.dtype:
+            raise ValueError("state size / dtype mismatch")
+        o = torch.empty((batch, ctx_q, S), dtype=v.dtype, device=v.device)
+        m = torch.empty((batch, self.heads, ctx_q), dtype=torch.float32, device=v.device)
+        l = torch.empty_like(m)
+        d = self._device_luts(q.device)
+        ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
+        dt = _lib.dtype_code(q.dtype) if v.dtype == q.dtype else -1
+        rc = lib.bst_attention_train(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
+                                     _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                     q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), m.data_ptr(), l.data_ptr(),
+                                     float(scale), batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
+                                     _lib.stream_ptr())
+        if rc == _lib.E_NOKERNEL:
+            return None
+        _lib.check(rc, "bst_attention_train")
+        return o, m, l
+
+    @_lib.guarded
+    def _attention_grad(self, q, k, v, o, dy, m, l, scale, autoregress_at_key):
+        """dq, dk, dv of the fused attention from what _attention_train saved, in one bst_attention_grad call. The
+        forward ran the fused kernel, so the call is inside its envelope; dy is made contiguous and aligned."""
+        lib = _lib.load()
+        dy = _aligned(dy.to(o.dtype))
+        batch, ctx_q, S = q.shape
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        delta = torch.empty_like(m)
+        d = self._device_luts(q.device)
+        ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
+        rc = lib.bst_attention_grad(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(), d["tn"].data_ptr(),
+                                    d["tn_order"].data_ptr(), self.lut_heads, self.blocks,
+                                    _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                    q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dy.data_ptr(),
+                                    m.data_ptr(), l.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+                                    float(scale), batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
+                                    _lib.stream_ptr())
+        _lib.check(rc, "bst_attention_grad")
+        return dq, dk, dv
+
     def partial_autoregressive_mask(self, autoregress_at_key, device="cuda"):
         """Device mask rewritten so causality starts at key `autoregress_at_key` (bst_op.cc:519-575).
 
@@ -260,15 +310,23 @@ class BlocksparseTransformer(TransformerCheckers):
         dtype = dtype or self.softmax_dtype or x.dtype
         return _SoftmaxFunction.apply(x, self, float(scale), False, None, dtype)
 
-    def attention(self, q, k, v, scale=1.0, autoregress_at_key=None):
+    def attention(self, q, k, v, scale=1.0, autoregress_at_key=None, fused_backward=False):
         """weight_value_op(masked_softmax(query_key_op(q, k), scale, autoregress_at_key), v) -- softmax without a
         mask_callback -- as one fused kernel that never writes the (batch, heads, blocks, bs, bs) scores or
         probabilities; the backward pass recomputes them from q and k. Returns (batch, ctx_q, heads*head_state) in
         v.dtype. Configurations without a fused kernel (fp32, mixed dtypes, block size other than 64, head_state other
-        than 64 / 128, unaligned tensors) run the three ops instead."""
+        than 64 / 128, unaligned tensors) run the three ops instead.
+
+        fused_backward selects the numerical contract of the gradients. False: they are bit-identical to the three-op
+        chain's, which rounds the scores and dS to bfloat16 and holds several sparse tensors during the backward.
+        True: the forward also keeps each row's softmax max and sum, and the backward is two fused kernels that keep the
+        scores in fp32 and store nothing of sparse shape. The output is the same either way; so is the fallback to the
+        three ops outside the fused kernels' envelope."""
         if autoregress_at_key is not None and self.softmax_mask_np is None:
             raise ValueError("autoregress_at_key only applies to ops with mask_callback defined.")
         try:
+            if fused_backward:
+                return _AttentionTrainFunction.apply(q, k, v, self, float(scale), autoregress_at_key)
             return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key)
         except _NoFusedKernel:
             w = self.query_key_op(q, k)
@@ -352,6 +410,28 @@ class _AttentionFunction(torch.autograd.Function):
             if ctx.needs_input_grad[0]:
                 dq = bst._xn(dw, k, False)
         return dq, dk, dv, None, None, None
+
+
+class _AttentionTrainFunction(torch.autograd.Function):
+    """Fused attention with a fused backward. Saves q, k, v, o and the row statistics (nothing of sparse shape); the
+    backward computes dq, dk and dv in one bst_attention_grad call and returns the requested ones."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, bst, scale, autoregress_at_key):
+        r = bst._attention_train(q, k, v, scale, autoregress_at_key)
+        if r is None:
+            raise _NoFusedKernel()
+        o, m, l = r
+        ctx.bst, ctx.scale, ctx.ak = bst, scale, autoregress_at_key
+        ctx.save_for_backward(q.contiguous(), k.contiguous(), v.contiguous(), o, m, l)
+        return o
+
+    @staticmethod
+    def backward(ctx, dy):
+        q, k, v, o, m, l = ctx.saved_tensors
+        dq, dk, dv = ctx.bst._attention_grad(q, k, v, o, dy, m, l, ctx.scale, ctx.ak)
+        need = ctx.needs_input_grad
+        return dq if need[0] else None, dk if need[1] else None, dv if need[2] else None, None, None, None
 
 
 class _SoftmaxFunction(torch.autograd.Function):

@@ -223,6 +223,39 @@ int bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, in
                   const void* q, const void* k, const void* v, void* o, float scale,
                   int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k, void* stream);
 
+/*
+ * bst_attention that also keeps what the fused backward needs: row_max and row_sum (float [batch][heads][ctx_blks_q*64])
+ * receive every query row's final running max m of its scaled, masked scores and the full sum l of exp(s - m).  They
+ * are stored apart rather than folded into one log-sum-exp: a row whose keys are all masked has m = -FLT_MAX, and
+ * -FLT_MAX + log l rounds back to -FLT_MAX, which would lose its uniform weights 1/l.  A query block with an empty LUT
+ * row gets m = -FLT_MAX, l = 0.  o is bit-identical to bst_attention's.  Same envelope and error codes as
+ * bst_attention (BSMM_E_NOKERNEL before any launch outside it; BSMM_E_ARG for null row_max / row_sum).  No reference
+ * launcher corresponds to it.
+ */
+int bst_attention_train(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                        const void* mask, int mask_heads, int autoregress_at_key,
+                        const void* q, const void* k, const void* v, void* o, float* row_max, float* row_sum, float scale,
+                        int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k, void* stream);
+
+/*
+ * Fused attention backward: dq, dk, dv (dtype, the layouts of q, k, v) of o = bst_attention_train(q, k, v) given
+ * dy = d(loss)/d(o), in two launches that never write the scores, the probabilities or their gradients:
+ *   wgmma_bst_attention_bwd_dq    per query block: delta = rowsum(dy * o) (float [batch][heads][ctx_blks_q*64], a
+ *                                 workspace this call fills), then dq = sum over nn_lut of dS k;
+ *   wgmma_bst_attention_bwd_dkdv  per key block, in tn_order (int32 [lut_heads][ctx_blks_k], longest tn_lut row first):
+ *                                 dv = sum over tn_lut of P^T dy, dk = sum of dS^T q;
+ * with P = exp(s - row_max) / row_sum recomputed from the scores and dS = scale * P * (dy v^T - delta).  The scores
+ * stay in fp32; P and dS enter the products in dtype.  nn_lut, tn_lut: as bst_xn; mask, mask_heads,
+ * autoregress_at_key: as bst_attention.  A block whose LUT row is empty gets zero gradients.  Deterministic: no
+ * atomics, sums in LUT order.  No reference launcher corresponds to it (the reference differentiates the three-op
+ * chain).  Same envelope and error codes as bst_attention over every 16-bit tensor (q, k, v, o, dy, dq, dk, dv).
+ */
+int bst_attention_grad(int dtype, int bsize, const int32_t* nn_lut, const int32_t* tn_lut, const int32_t* tn_order,
+                       int lut_heads, int blocks, const void* mask, int mask_heads, int autoregress_at_key,
+                       const void* q, const void* k, const void* v, const void* o, const void* dy,
+                       const float* row_max, const float* row_sum, float* delta, void* dq, void* dk, void* dv, float scale,
+                       int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k, void* stream);
+
 /* mask_out[hl][blk][r] = mask_in[hl][blk][r] & (ones >> shift(r)), same layout as bst_softmax's mask */
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,
                             const void* mask_in, void* mask_out, int autoregress_at_key,

@@ -78,7 +78,11 @@ def fma_gemm_bound(ref, ref_abs, out_dtype, k_terms):
 # the accumulation shows directly; 0.77 with its alpha / gate / beta roundings, which the unit leaves out; and <= 0.05
 # for the 16-bit outputs (xprop, xprop2, pair tiles, updat), whose own rounding hides most of it. Per MMA width of the
 # updat kernel (tests/test_updat_persistent_gpu.py, H100 80GB HBM3 at a 400 W power limit), the fp32 dW showed 0.052,
-# 0.058, 0.075 and 0.064 at N = 64, 128, 192 and 256.
+# 0.058, 0.075 and 0.064 at N = 64, 128, 192 and 256. The wgmma attention GEMMs (csrc/tc_bst.cuh;
+# tests/test_tc_gpu.py::test_tc_bst_gemms_match_oracle, H100 80GB HBM3; the same at 400 W and 700 W) showed 0.099 for the
+# fp32-output NT, where the accumulation shows directly; 0.0079 / 0.0059 for NT to fp16 / bf16, 0.0032 / 0.0008 for NN
+# and 0.025 / 0.0011 for TN to fp16 / bf16; <= 0.007 for the ops of the attention chain in
+# tests/test_bst_chain_elementwise_gpu.py.
 MMA_C = 4
 
 
@@ -146,6 +150,73 @@ def oracle_dense(orc, op, a, b):
     if op == "fprop":
         return a @ D if orc.axis else D.T @ a
     return a @ D.T if orc.axis else D @ a
+
+
+def _bst_entries(orc, op):
+    """(out, blk, inp) index arrays of shape (heads, blocks) for a BST product: output block, sparse block and input
+    block of every LUT entry, read from nt_list ("nt": out = blk) or the rows of nn_list / tn_list, per head (lut_heads 1
+    broadcasts its layout to every head). Entries are grouped by output block, in row order."""
+    out, blk, inp = [], [], []
+    for h in range(orc.heads):
+        hl = orc._hl(h)
+        if op == "nt":
+            pairs = np.array(orc.nt_list[hl], dtype=np.int64).reshape(-1, 2)
+            out.append(pairs[:, 0]); blk.append(np.arange(len(pairs))); inp.append(pairs[:, 1])
+            continue
+        rows = orc.nn_list[hl] if op == "nn" else orc.tn_list[hl]
+        e = [(o, b, i) for o, row in enumerate(rows) for b, i in row]
+        out.append([o for o, _, _ in e]); blk.append([b for _, b, _ in e]); inp.append([i for _, _, i in e])
+    return tuple(np.array(x, dtype=np.int64) for x in (out, blk, inp))
+
+
+def bst_dense(orc, op, a, b, with_abs=False):
+    """The BST products of TransformerOracle.nt / nn / tn in float64, through batched matmuls instead of per-block loops.
+
+    "nt": a, b dense (batch, ctx, heads * head_state) -> (batch, heads, blocks, bs, bs), block (q, k) of nt_list.
+    "nn": a sparse (batch, heads, blocks, bs, bs), b dense over the key blocks -> dense over the query blocks, each
+          query block the sum over its nn_list row of a[block] . b[key block].
+    "tn": the same with a[block]^T over the tn_list row of each key block, b dense over the query blocks.
+    with_abs: also return the product of |a| and |b|, the ref_abs of the error bounds."""
+    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
+    res = _bst_dense(orc, op, a, b)
+    return (res, _bst_dense(orc, op, np.abs(a), np.abs(b))) if with_abs else res
+
+
+def _bst_dense(orc, op, a, b):
+    bs, H = orc.blk_size, orc.heads
+    out, blk, inp = _bst_entries(orc, op)
+    hidx = np.arange(H)[:, None]
+
+    def heads_view(x):                       # (batch, ctx, H * hs) -> (batch, H, ctx blocks, bs, hs)
+        n, ctx, S = x.shape
+        return x.reshape(n, ctx // bs, bs, H, S // H).transpose(0, 3, 1, 2, 4)
+    if op == "nt":
+        A, B = heads_view(a), heads_view(b)
+        return np.matmul(A[:, hidx, out], B[:, hidx, inp].swapaxes(-1, -2))
+    B = heads_view(b)
+    sp = a[:, hidx, blk]                                           # (batch, H, blocks, bs, bs)
+    prod = np.matmul(sp.swapaxes(-1, -2) if op == "tn" else sp, B[:, hidx, inp])
+    n_out = orc.ctx_blks_q if op == "nn" else orc.ctx_blks_k
+    n, S = b.shape[0], b.shape[2]
+    C = np.zeros((n, H, n_out, bs, S // H))
+    for h in range(H):                       # sum each output block's run of entries (entries are grouped by block)
+        counts = np.bincount(out[h], minlength=n_out)
+        live = np.nonzero(counts)[0]
+        if len(live):
+            C[:, h, live] = np.add.reduceat(prod[:, h], (np.cumsum(counts) - counts)[live], axis=1)
+    return C.transpose(0, 2, 3, 1, 4).reshape(n, n_out * bs, S)
+
+
+def bst_terms(orc, op, head_state):
+    """k_terms of a BST product, broadcastable against its output: head_state for "nt"; for "nn" / "tn", bs x the
+    length of each output block's nn_list / tn_list row in its head."""
+    if op == "nt":
+        return float(head_state)
+    bs = orc.blk_size
+    rows = orc.nn_list if op == "nn" else orc.tn_list
+    k = np.array([[len(r) for r in rows[orc._hl(h)]] for h in range(orc.heads)], dtype=np.float64) * bs   # (H, n_out)
+    k = np.repeat(np.repeat(k.T[:, None, :, None], bs, axis=1), head_state, axis=3)                      # (n_out, bs, H, hs)
+    return k.reshape(1, -1, orc.heads * head_state)
 
 
 def feature_terms(layout, bs, bprop, axis):

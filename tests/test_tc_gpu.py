@@ -9,8 +9,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests._util import (_on_poisoned_output, assert_within, assert_zero_filled, dtype_name, feature_terms,
-                         fma_gemm_bound, mma_gemm_bound, oracle_dense, record_kernels, ref_errors)
+from tests._util import (_on_poisoned_output, assert_within, assert_zero_filled, bst_dense, bst_terms, dtype_name,
+                         feature_terms, fma_gemm_bound, mma_gemm_bound, oracle_dense, record_kernels, ref_errors)
 from blocksparse_b200 import BlocksparseMatMul, _lib
 from oracle.bsmm_oracle import MatmulOracle
 
@@ -265,6 +265,7 @@ def _assert_zero_blocks(c, empty, bs, what):
 
 BST_CASES = [
     # lut_heads, heads, q_blks, k_blks, density, head_state, batch, (empty query blocks, empty key blocks)
+    # [, "pos": operands uniform in (0, 1)]. density "tril": the causal block layout, rows and columns of 1 .. q_blks.
     (1, 2, 4, 4, 0.6, 64, 2, None),
     (1, 3, 5, 7, 0.4, 64, 1, None),        # rectangular, odd number of blocks per key column
     (2, 2, 6, 5, 0.5, 128, 2, None),       # per-head layouts, head_state 128 (two column atoms)
@@ -273,47 +274,111 @@ BST_CASES = [
     (1, 2, 5, 6, 0.5, 128, 1, None),       # shared layout at head_state 128
     (1, 2, 12, 12, 0.85, 64, 1, None),     # rows of 9+ blocks: the 4-stage ring wraps more than twice
     (2, 2, 7, 6, 0.5, 64, 2, ((1, 4), (2,))),   # empty query rows (NN zero-fill) and an empty key column (TN zero-fill)
+    (1, 2, 6, 6, "tril", 64, 2, None),     # rows of exactly 1, 4 and 5 entries: the ring's first refill is entry 4
+    (1, 1, 24, 24, 1.0, 64, 1, None),      # dense: rows of 24, the ring wraps six times
+    (3, 3, 5, 8, 0.4, 64, 3, None),        # batch 3, ctx_q != ctx_k, a layout per head: offsets cannot cancel
+    (2, 2, 7, 6, 0.5, 128, 2, ((1, 4), (2,))),  # head_state 128 with per-head layouts and holes
+    (1, 2, 5, 5, 0.6, 64, 2, None, "pos"),
+    (2, 2, 6, 5, 0.5, 128, 2, None, "pos"),
 ]
 
 
-@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+def bst_case_layout(case):
+    """The layout of a BST_CASES entry ((lut_heads, q_blks, k_blks) array) and the rng that drew it, which then draws
+    the operands."""
+    lh, heads, qb, kb, density, hs, batch, holes, *opt = case
+    rng = np.random.default_rng(lh * 100 + heads * 10 + qb)
+    if density == "tril":
+        return np.tril(np.ones((lh, qb, kb), np.int32)), rng
+    empty_q, empty_k = holes or ((), ())
+    return _bst_layout(rng, lh, qb, kb, density, empty_q, empty_k), rng
+
+
+BST_DTYPES = (torch.float16, torch.bfloat16)               # dense operands, and the sparse one of NN / TN
+BST_NT_OUT = ((torch.float32, 1e-5), (torch.bfloat16, 4e-3), (torch.float16, 1e-3))   # NT output dtype, l2 limit
+
+
+@pytest.mark.parametrize("dtype", BST_DTYPES)
 @pytest.mark.parametrize("case", BST_CASES)
 def test_tc_bst_gemms_match_oracle(case, dtype):
-    lh, heads, qb, kb, density, hs, batch, holes = case
-    rng = np.random.default_rng(lh * 100 + heads * 10 + qb)
+    """The wgmma attention GEMMs (csrc/tc_bst.cuh): NT at every output dtype, NN and TN, each on NaN-poisoned output
+    memory and elementwise within mma_gemm_bound of the float64 product (k_terms: head_state for NT, 64 x the LUT row
+    length of each output block, per head, for NN / TN). The relative l2 error against the same reference is kept as a
+    second metric."""
+    lh, heads, qb, kb, density, hs, batch, holes, *opt = case
+    lay, rng = bst_case_layout(case)
     empty_q, empty_k = holes or ((), ())
-    lay = _bst_layout(rng, lh, qb, kb, density, empty_q, empty_k)
     bst = BlocksparseTransformer(lay if lh > 1 else lay[0], 64, heads=heads)
-    if density > 0.8:
+    if density == 1.0:
+        assert bst.nn_max == kb and bst.tn_max == qb
+    elif density != "tril" and density > 0.8:
         assert bst.nn_max > 8 and bst.tn_max > 8
     orc = TransformerOracle(lay if lh > 1 else lay[0], 64, heads=heads)
     S = heads * hs
-    mk = lambda *shape: torch.as_tensor(rng.uniform(-1, 1, shape).astype(np.float32)).to(dtype)
+    lo = 0 if "pos" in opt else -1
+    mk = lambda *shape: torch.as_tensor(rng.uniform(lo, 1, shape).astype(np.float32)).to(dtype)
     Q, K, V = mk(batch, qb * 64, S), mk(batch, kb * 64, S), mk(batch, kb * 64, S)
     DY = mk(batch, qb * 64, S)
     P = torch.as_tensor(rng.uniform(0, 1, (batch, heads, bst.blocks, 64, 64)).astype(np.float32)).to(dtype)
     Qn, Kn, Vn, DYn, Pn = (t.float().numpy() for t in (Q, K, V, DY, P))
+    Qd, Kd, Vd, DYd, Pd = Q.cuda(), K.cuda(), V.cuda(), DY.cuda(), P.cuda()
     F = _lib.FLAG_FORCE_TC
     tol = 4e-3 if dtype == torch.bfloat16 else 1e-3
-    for c_dtype in (torch.float32, torch.bfloat16):
-        got = bst._nt(Q.cuda(), K.cuda(), c_dtype, flags=F)
-        assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_nt"
-        mx, l2 = ref_errors(got.float().cpu().numpy(), orc.nt(Qn, Kn))
-        assert l2 <= (1e-5 if c_dtype == torch.float32 else 4e-3), "nt l2 %.3e" % l2
-    got = bst._xn(P.cuda(), V.cuda(), False, flags=F)
-    assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_nn"
-    mx, l2 = ref_errors(got.float().cpu().numpy(), orc.nn(Pn, Vn))
-    assert l2 <= tol, "nn l2 %.3e" % l2
-    got = bst._xn(P.cuda(), DY.cuda(), True, flags=F)
-    assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_tn"
-    mx, l2 = ref_errors(got.float().cpu().numpy(), orc.tn(Pn, DYn))
-    assert l2 <= tol, "tn l2 %.3e" % l2
-    if holes:
-        Pd, Vd, DYd = P.cuda(), V.cuda(), DY.cuda()
-        for transpose, dense, empty, what in [(False, Vd, empty_q, "nn"), (True, DYd, empty_k, "tn")]:
-            c = _on_poisoned_output(lambda: bst._xn(Pd, dense, transpose, flags=F))
-            assert _lib.device_error() == 0 and _lib.last_kernel() == "wgmma_bst_" + what
-            _assert_zero_blocks(c, empty, 64, what)
+
+    def check(run, op, a, b, kern, l2_tol):
+        got = _on_poisoned_output(run)
+        assert _lib.device_error() == 0, "a wgmma kernel hit its bounded-wait timeout or faulted: " + _lib.device_error_text()
+        assert _lib.last_kernel() == kern, _lib.last_kernel()
+        out = dtype_name(got.dtype)
+        what = "%s -> %s (%s)" % (op, out, kern)
+        assert not bool(torch.isnan(got).any()), "%s: %d elements never written" % (what, int(torch.isnan(got).sum()))
+        ref, ref_abs = bst_dense(orc, op, a, b, with_abs=True)
+        k = bst_terms(orc, op, hs)
+        assert_within(got, ref, mma_gemm_bound(ref, ref_abs, out, k), what, ref_abs, k, out, "wgmma_bst")
+        mx, l2 = ref_errors(got.double().cpu().numpy(), ref)
+        assert l2 <= l2_tol, "%s l2 %.3e" % (what, l2)
+        return got
+
+    for c_dtype, l2_tol in BST_NT_OUT:
+        check(lambda: bst._nt(Qd, Kd, c_dtype, flags=F), "nt", Qn, Kn, "wgmma_bst_nt", l2_tol)
+    c = check(lambda: bst._xn(Pd, Vd, False, flags=F), "nn", Pn, Vn, "wgmma_bst_nn", tol)
+    _assert_zero_blocks(c, empty_q, 64, "nn")
+    c = check(lambda: bst._xn(Pd, DYd, True, flags=F), "tn", Pn, DYn, "wgmma_bst_tn", tol)
+    _assert_zero_blocks(c, empty_k, 64, "tn")
+
+
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
+def test_bst_misaligned_views_take_the_cuda_core_route(dtype):
+    """Dense operands at an odd element offset into a larger buffer are legal torch, but TMA needs 16-byte aligned
+    bases: the public nt_op / nn_op / tn_op run them on the CUDA-core kernels, elementwise within fma_gemm_bound."""
+    lay = np.tril(np.ones((4, 4), np.int32))
+    heads, hs, batch = 2, 64, 2
+    bst = BlocksparseTransformer(lay, 64, heads=heads)
+    orc = TransformerOracle(lay, 64, heads=heads)
+    rng = np.random.default_rng(31)
+    shape = (batch, 4 * 64, heads * hs)
+    n = int(np.prod(shape))
+
+    def misaligned(offset):
+        host = torch.as_tensor(rng.uniform(-1, 1, shape).astype(np.float32)).to(dtype)
+        t = torch.zeros(n + offset, dtype=dtype, device="cuda")[offset:].view(shape)
+        t.copy_(host.cuda())
+        assert t.is_contiguous() and t.data_ptr() % 16
+        return t, host.float().numpy()
+    (Q, Qn), (K, Kn), (DY, DYn) = misaligned(1), misaligned(3), misaligned(5)
+    P = torch.as_tensor(rng.uniform(0, 1, (batch, heads, bst.blocks, 64, 64)).astype(np.float32)).to(dtype)
+    Pn, Pd = P.float().numpy(), P.cuda()
+    for run, op, a, b, kern in [(lambda: bst.nt_op(Q, K), "nt", Qn, Kn, "fma_dds_nt"),
+                                (lambda: bst.nn_op(Pd, K), "nn", Pn, Kn, "fma_sdd_xn"),
+                                (lambda: bst.tn_op(Pd, DY), "tn", Pn, DYn, "fma_sdd_xn")]:
+        got = _on_poisoned_output(run)
+        assert _lib.device_error() == 0, _lib.device_error_text()
+        assert _lib.last_kernel() == kern, (op, _lib.last_kernel())
+        assert not bool(torch.isnan(got).any()), "%s: elements never written" % op
+        ref, ref_abs = bst_dense(orc, op, a, b, with_abs=True)
+        out = dtype_name(got.dtype)
+        k = bst_terms(orc, op, hs)
+        assert_within(got, ref, fma_gemm_bound(ref, ref_abs, out, k), "misaligned %s (%s)" % (op, kern))
 
 
 FMA_CASES = [

@@ -15,7 +15,7 @@ MAX_PAIRS = 8
 E_NOKERNEL = -7          # BSMM_E_NOKERNEL: no fused kernel for the configuration
 
 _c = ctypes
-_vp, _i, _f = _c.c_void_p, _c.c_int, _c.c_float
+_vp, _i, _f, _ll = _c.c_void_p, _c.c_int, _c.c_float, _c.c_longlong
 
 # name -> (restype, argtypes); must list every symbol include/bsmm_b200.h declares
 SIGNATURES = {
@@ -40,6 +40,10 @@ SIGNATURES = {
     "bst_attention_grad": (_i, [_i, _i, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                 _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp]),
     "bst_autoregressive_mask": (_i, [_i, _vp, _i, _i, _vp, _vp, _i, _vp]),
+    "bst_dense_softmax": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),
+    "bst_dense_softmax_grad": (_i, [_i, _vp, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),
+    "bst_topk_softmax": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _i, _f, _vp]),
+    "bst_topk": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _i, _vp]),
     "bsmm_block_norm": (_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),

@@ -165,3 +165,55 @@ class TransformerCheckers(object):
                 np.add.at(tot[n], q, prod[n])
             dx[:, h] = (dy[:, h] - tot[:, q][..., None]) * y[:, h] * scale
         return dx
+
+
+# ---- module-level checkers of the dense ops (reference blocksparse/transformer.py:536-549, 609-656) ----------------------
+# The reference's NumPy checkers restated with NumPy broadcasting of the mask, which also gives the right answer for a
+# (D1, 1, D3) mask where the reference's flattening checker does not (transformer.py:613), and with a stable sort, so
+# that ties rank by index ascending like the ops.
+def _masked_values(x, mask, scale):
+    x = np.asarray(x, dtype=np.float32)
+    if mask is None:
+        return x * np.float32(scale)
+    m = np.broadcast_to(np.asarray(mask, dtype=np.float32), x.shape)
+    return np.where(m != 0, x * m * np.float32(scale), -np.finfo(np.float32).max).astype(np.float32)
+
+
+def _rank(v):
+    """Column order of each row of v (..., D3): value descending, then index ascending."""
+    return np.argsort(-v, axis=-1, kind="stable")
+
+
+def masked_softmax_test(x, mask=None, scale=1.0):
+    """transformer.py:609-625."""
+    y = _masked_values(x, mask, scale)
+    e = np.exp(y - y.max(axis=-1, keepdims=True))
+    return e / e.sum(axis=-1, keepdims=True)
+
+
+def masked_top_k_softmax_test(x, k, mask=None, scale=1.0):
+    """transformer.py:627-649."""
+    y = _masked_values(x, mask, scale)
+    top = _rank(y)[..., :k]
+    v = np.take_along_axis(y, top, axis=-1)
+    e = np.exp(v - v[..., :1])
+    z = np.zeros(y.shape, dtype=np.float32)
+    np.put_along_axis(z, top, (e / e.sum(axis=-1, keepdims=True)).astype(np.float32), axis=-1)
+    return z
+
+
+def masked_softmax_grad_test(dy, y, mask=None, scale=1.0):
+    """transformer.py:651-656."""
+    m = 1.0 if mask is None else mask
+    return (dy - np.sum(dy * y, axis=-1, keepdims=True)) * y * m * scale
+
+
+def rectified_top_k_test(x, k, rebase=True):
+    """transformer.py:536-549."""
+    x = np.asarray(x, dtype=np.float32)
+    top = _rank(x)[..., :k]
+    v = np.take_along_axis(x, top, axis=-1)
+    base = np.maximum(v[..., k - 1:k], 0.0) if rebase else np.zeros_like(v[..., :1])
+    y = np.zeros(x.shape, dtype=np.float32)
+    np.put_along_axis(y, top, np.maximum(v, base) - base, axis=-1)
+    return y

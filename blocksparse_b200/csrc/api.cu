@@ -2,6 +2,7 @@
 // See include/bsmm_b200.h for the contract and the reference launchers each entry replaces.
 #include <atomic>
 #include "common.cuh"
+#include "dense_softmax.cuh"
 #include "generic.cuh"
 #include "softmax.cuh"
 #include "tc.cuh"
@@ -409,6 +410,82 @@ int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int
                                                             mask_in, mask_out, blocks, autoregress_at_key);
   });
   return check_launch("bst_autoregressive_mask");
+}
+
+// ---- dense softmax and top-k (csrc/dense_softmax.cuh) ---------------------------------------------------------------
+static bool dense_dtype_ok(int dtype) { return dtype == BSMM_F32 || dtype == BSMM_F16 || dtype == BSMM_BF16; }
+
+// Validates the (D0, D1, D2, D3) shape and the mask strides, fills a's row map; `rows` = 0 means nothing to launch.
+static int dense_args(const char* what, int dtype, long long D0, int D1, int D2, int D3, const float* mask,
+                      long long M1, long long M2, DenseArgs& a) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "%s: unsupported dtype code %d", what, dtype);
+  if (D0 < 0 || D1 < 0 || D2 < 0 || D3 <= 0) return fail(BSMM_E_ARG, "%s: bad sizes (%lld, %d, %d, %d)", what, D0, D1, D2, D3);
+  if (!mask) M1 = M2 = 0;
+  if ((M2 != 0 && M2 != D3) || (M1 != 0 && M1 != (long long)D3 * (M2 ? D2 : 1)))
+    return fail(BSMM_E_ARG, "%s: mask strides (%lld, %lld) do not describe a (1|D1, 1|D2, D3) mask", what, M1, M2);
+  a.mask = mask;
+  a.D3 = D3;
+  a.rows = D0 * D1 * D2;
+  a.map = {D1, D2, M1, M2, D0 * (M1 ? 1 : D1) * (M2 ? 1 : D2)};
+  // one CTA per row on every route but the warp one; grid.x holds at most 2^31 - 1
+  if (a.rows > 0x7fffffffLL * (D3 <= DSM_WARP_MAX ? DSM_WARPS : 1))
+    return fail(BSMM_E_LIMIT, "%s: %lld rows exceed the grid", what, a.rows);
+  return 0;
+}
+
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+int bst_dense_softmax(int dtype, const void* x, const float* mask, void* y, long long D0, int D1, int D2, int D3,
+                      long long mask_stride1, long long mask_stride2, float scale, void* stream) {
+  DenseArgs a = {};
+  if (int e = dense_args("bst_dense_softmax", dtype, D0, D1, D2, D3, mask, mask_stride1, mask_stride2, a)) return e;
+  if (!x || !y) return fail(BSMM_E_ARG, "bst_dense_softmax: null pointer");
+  if (a.rows == 0) return 0;
+  a.a = x; a.out = y; a.scale = scale;
+  const bool vec = aligned16(x) && aligned16(y) && (!mask || aligned16(mask)) && D3 % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_dense_softmax<T>(a, false, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bst_dense_softmax_grad(int dtype, const void* dy, const void* y, const float* mask, void* dx, long long D0, int D1,
+                           int D2, int D3, long long mask_stride1, long long mask_stride2, float scale, void* stream) {
+  DenseArgs a = {};
+  if (int e = dense_args("bst_dense_softmax_grad", dtype, D0, D1, D2, D3, mask, mask_stride1, mask_stride2, a)) return e;
+  if (!dy || !y || !dx) return fail(BSMM_E_ARG, "bst_dense_softmax_grad: null pointer");
+  if (a.rows == 0) return 0;
+  a.a = dy; a.b = y; a.out = dx; a.scale = scale;
+  const bool vec = aligned16(dy) && aligned16(y) && aligned16(dx) && (!mask || aligned16(mask)) &&
+                   D3 % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_dense_softmax<T>(a, true, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bst_topk_softmax(int dtype, const void* x, const float* mask, void* y, long long D0, int D1, int D2, int D3,
+                     long long mask_stride1, long long mask_stride2, int k, float scale, void* stream) {
+  DenseArgs a = {};
+  if (int e = dense_args("bst_topk_softmax", dtype, D0, D1, D2, D3, mask, mask_stride1, mask_stride2, a)) return e;
+  if (!x || !y) return fail(BSMM_E_ARG, "bst_topk_softmax: null pointer");
+  if (D3 > TOPK_MAX || k < 1 || k > D3) return fail(BSMM_E_ARG, "bst_topk_softmax: need 1 <= k <= D3 <= %d, got k %d, D3 %d", TOPK_MAX, k, D3);
+  if (a.rows > 0x7fffffffLL) return fail(BSMM_E_LIMIT, "bst_topk_softmax: %lld rows exceed the grid", a.rows);
+  if (a.rows == 0) return 0;
+  a.a = x; a.out = y; a.k = k; a.mode = TOPK_SOFTMAX; a.scale = scale;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_dense_topk<T>(a, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bst_topk(int dtype, const void* x, void* y, int32_t* idx, long long rows, int D3, int k, int mode, void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bst_topk: unsupported dtype code %d", dtype);
+  if (mode < TOPK_VALUES || mode > TOPK_REBASE) return fail(BSMM_E_ARG, "bst_topk: mode must be 0, 1 or 2, got %d", mode);
+  if (!x || !y || (mode == TOPK_VALUES && !idx)) return fail(BSMM_E_ARG, "bst_topk: null pointer");
+  if (rows < 0 || D3 <= 0 || D3 > TOPK_MAX || k < 1 || k > D3)
+    return fail(BSMM_E_ARG, "bst_topk: need rows >= 0 and 1 <= k <= D3 <= %d, got k %d, D3 %d", TOPK_MAX, k, D3);
+  if (rows > 0x7fffffffLL) return fail(BSMM_E_LIMIT, "bst_topk: %lld rows exceed the grid", rows);
+  if (rows == 0) return 0;
+  DenseArgs a = {};
+  a.a = x; a.out = y; a.idx = idx; a.D3 = D3; a.k = k; a.mode = mode; a.rows = rows;
+  a.map = {1, 1, 0, 0, rows};
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_dense_topk<T>(a, (cudaStream_t)stream); });
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------

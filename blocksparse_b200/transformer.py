@@ -449,3 +449,263 @@ class _SoftmaxFunction(torch.autograd.Function):
         (y,) = ctx.saved_tensors
         dx = ctx.bst._softmax_grad(dy, y, ctx.scale)
         return dx.to(ctx.x_dtype), None, None, None, None, None
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Dense softmax and top-k: the rest of the reference's transformer module (blocksparse/transformer.py:494-656,
+# exported by blocksparse/__init__.py:124-134). x is (..., D3); the ops run along the last dim.
+_TOPK_VALUES, _TOPK_RECTIFIED, _TOPK_REBASE = 0, 1, 2
+
+
+def _dense_input(x, what):
+    if not torch.is_tensor(x) or not x.is_cuda:
+        raise ValueError("%s needs a CUDA tensor (there is no CPU path)" % what)
+    if x.dim() < 1:
+        raise ValueError("%s needs a tensor of rank >= 1" % what)
+    _lib.dtype_code(x.dtype)
+    return x.contiguous()
+
+
+def _dense_dims(shape):
+    """(D0, D1, D2, D3) of a tensor of rank >= 1: D3 the last dim, D2 and D1 the two before it (1 where absent)."""
+    D3 = shape[-1]
+    D2 = shape[-2] if len(shape) >= 2 else 1
+    D1 = shape[-3] if len(shape) >= 3 else 1
+    D0 = 1
+    for d in shape[:-3]:
+        D0 *= d
+    return D0, D1, D2, D3
+
+
+def _dense_mask(x, mask, what):
+    """(fp32 contiguous mask on x's device or None, stride of dim 1, stride of dim 2). The mask has x's rank, its last dim
+    is D3, each of the two dims before it is 1 or x's size, and every dim before those is 1. Strides come from the
+    mask's own shape (the reference derives the dim-1 stride from x's D2: transformer_op.cc:184-185)."""
+    if mask is None:
+        return None, 0, 0
+    mask = torch.as_tensor(mask)
+    xs, ms = tuple(x.shape), tuple(mask.shape)
+    ok = len(ms) == len(xs) and ms[-1] == xs[-1]
+    ok = ok and all(m in (1, d) for m, d in zip(ms[-3:-1], xs[-3:-1])) and all(m == 1 for m in ms[:-3])
+    if not ok:
+        raise ValueError("%s: mask shape %s does not broadcast to %s (supported: (1, ..., 1|D1, 1|D2, D3))" % (what, ms, xs))
+    D3 = xs[-1]
+    m2 = len(ms) >= 2 and ms[-2] > 1
+    m1 = len(ms) >= 3 and ms[-3] > 1
+    M2 = D3 if m2 else 0
+    M1 = D3 * (ms[-2] if m2 else 1) if m1 else 0
+    return mask.to(device=x.device, dtype=torch.float32).contiguous(), M1, M2
+
+
+def _on_device_of(fn):
+    """Run fn with its first argument's device current: the library launches on the current device's current stream."""
+    import functools
+
+    @functools.wraps(fn)
+    def run(x, *args):
+        if x.device.index == torch.cuda.current_device():
+            return fn(x, *args)
+        with torch.cuda.device(x.device):
+            return fn(x, *args)
+    return run
+
+
+def _check_k(x, k, what):
+    k = int(k)
+    D3 = x.shape[-1]
+    if not 1 <= k <= D3 <= 1024:
+        raise ValueError("%s needs 1 <= k <= x.shape[-1] <= 1024, got k %d, x.shape[-1] %d" % (what, k, D3))
+    return k
+
+
+@_on_device_of
+def _dense_softmax_fwd(x, mask, M1, M2, scale):
+    y = torch.empty_like(x)
+    if x.numel() == 0:
+        return y
+    D0, D1, D2, D3 = _dense_dims(x.shape)
+    rc = _lib.load().bst_dense_softmax(_lib.dtype_code(x.dtype), x.data_ptr(), _lib.ptr(mask), y.data_ptr(),
+                                       D0, D1, D2, D3, M1, M2, float(scale), _lib.stream_ptr())
+    _lib.check(rc, "bst_dense_softmax")
+    return y
+
+
+@_on_device_of
+def _dense_softmax_bwd(y, dy, mask, M1, M2, scale):
+    dy = dy.to(y.dtype).contiguous()
+    dx = torch.empty_like(y)
+    if y.numel() == 0:
+        return dx
+    D0, D1, D2, D3 = _dense_dims(y.shape)
+    rc = _lib.load().bst_dense_softmax_grad(_lib.dtype_code(y.dtype), dy.data_ptr(), y.data_ptr(), _lib.ptr(mask),
+                                            dx.data_ptr(), D0, D1, D2, D3, M1, M2, float(scale), _lib.stream_ptr())
+    _lib.check(rc, "bst_dense_softmax_grad")
+    return dx
+
+
+@_on_device_of
+def _topk_softmax_fwd(x, mask, M1, M2, k, scale):
+    y = torch.empty_like(x)
+    if x.numel() == 0:
+        return y
+    D0, D1, D2, D3 = _dense_dims(x.shape)
+    rc = _lib.load().bst_topk_softmax(_lib.dtype_code(x.dtype), x.data_ptr(), _lib.ptr(mask), y.data_ptr(),
+                                      D0, D1, D2, D3, M1, M2, k, float(scale), _lib.stream_ptr())
+    _lib.check(rc, "bst_topk_softmax")
+    return y
+
+
+@_on_device_of
+def _topk_fwd(x, k, mode):
+    if mode == _TOPK_VALUES:
+        y = torch.empty(tuple(x.shape[:-1]) + (k,), dtype=x.dtype, device=x.device)
+        idx = torch.empty(y.shape, dtype=torch.int32, device=x.device)
+    else:
+        y, idx = torch.empty_like(x), None
+    if x.numel() == 0:
+        return y, idx
+    rc = _lib.load().bst_topk(_lib.dtype_code(x.dtype), x.data_ptr(), y.data_ptr(), _lib.ptr(idx),
+                              x.numel() // x.shape[-1], x.shape[-1], k, mode, _lib.stream_ptr())
+    _lib.check(rc, "bst_topk")
+    return y, idx
+
+
+def _dense_bench(what, fn, nbytes, repeat):
+    """The reference's `bench` attribute (transformer_op.cc:268-280): time `repeat` launches between two CUDA events
+    and print one line with the time per launch and the algorithmic bytes moved per second."""
+    import ctypes
+    lib = _lib.load()
+    timer = ctypes.c_void_p()
+    _lib.check(lib.bsmm_timer_create(ctypes.byref(timer)), "timer_create")
+    fn()
+    _lib.check(lib.bsmm_timer_begin(timer, _lib.stream_ptr()), "timer_begin")
+    for _ in range(repeat):
+        fn()
+    ms = ctypes.c_float()
+    _lib.check(lib.bsmm_timer_end(timer, _lib.stream_ptr(), ctypes.byref(ms)), "timer_end")
+    lib.bsmm_timer_destroy(timer)
+    ms_per = ms.value / repeat
+    print("%s ms: %.4f GB/s: %.0f" % (what, ms_per, nbytes / (ms_per * 1e6)))
+    return ms_per
+
+
+def _softmax_bytes(x, mask, tensors):
+    """x's bytes times the tensors the op streams (2 forward: x, y; 3 gradient: dy, y, dx), plus the mask once."""
+    return tensors * x.numel() * x.element_size() + (0 if mask is None else mask.numel() * 4)
+
+
+class _DenseSoftmaxFunction(torch.autograd.Function):
+    """reference transformer.py:598-607: the gradient is masked_softmax_grad of the saved y."""
+
+    @staticmethod
+    def forward(ctx, x, mask, M1, M2, scale, bench):
+        y = _dense_softmax_fwd(x, mask, M1, M2, scale)
+        ctx.mask, ctx.M1, ctx.M2, ctx.scale, ctx.bench = mask, M1, M2, scale, bench
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (y,) = ctx.saved_tensors
+        if ctx.bench:
+            _dense_bench("masked_softmax_grad %s %s" % (tuple(y.shape), str(y.dtype).replace("torch.", "")),
+                         lambda: _dense_softmax_bwd(y, dy, ctx.mask, ctx.M1, ctx.M2, ctx.scale),
+                         _softmax_bytes(y, ctx.mask, 3), ctx.bench)
+        return _dense_softmax_bwd(y, dy, ctx.mask, ctx.M1, ctx.M2, ctx.scale), None, None, None, None, None
+
+
+class _TopKSoftmaxFunction(torch.autograd.Function):
+    """reference transformer.py:588-596: the softmax gradient formula applied to the op's own y."""
+
+    @staticmethod
+    def forward(ctx, x, mask, M1, M2, k, scale):
+        y = _topk_softmax_fwd(x, mask, M1, M2, k, scale)
+        ctx.mask, ctx.M1, ctx.M2, ctx.scale = mask, M1, M2, scale
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (y,) = ctx.saved_tensors
+        return _dense_softmax_bwd(y, dy, ctx.mask, ctx.M1, ctx.M2, ctx.scale), None, None, None, None, None
+
+
+class _TopKFunction(torch.autograd.Function):
+    """reference transformer.py:507-533: dvalues scattered to their indices, zeros elsewhere (a torch scatter, as the
+    reference runs it as framework ops)."""
+
+    @staticmethod
+    def forward(ctx, x, k):
+        y, idx = _topk_fwd(x, k, _TOPK_VALUES)
+        ctx.mark_non_differentiable(idx)
+        ctx.save_for_backward(idx)
+        ctx.x_shape = x.shape
+        return y, idx
+
+    @staticmethod
+    def backward(ctx, dy, _didx):
+        (idx,) = ctx.saved_tensors
+        dx = torch.zeros(ctx.x_shape, dtype=dy.dtype, device=dy.device)
+        return dx.scatter_(-1, idx.long(), dy), None
+
+
+class _RectifiedTopKFunction(torch.autograd.Function):
+    """reference transformer.py:502-505: the ReLU gradient, dz where y > 0 (a torch select, as the reference runs it as
+    an ewops op)."""
+
+    @staticmethod
+    def forward(ctx, x, k, mode):
+        y, _ = _topk_fwd(x, k, mode)
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dz):
+        (y,) = ctx.saved_tensors
+        return torch.where(y > 0, dz, torch.zeros((), dtype=dz.dtype, device=dz.device)), None, None
+
+
+def masked_softmax(x, mask=None, scale=1.0, bench=0):
+    """Softmax along the last dim of v = x * mask * scale where mask != 0, -FLT_MAX where mask == 0 (reference
+    transformer.py:573-585, 609-625). x: fp32 / fp16 / bf16 of any rank >= 1; y has x's dtype. mask: (1, ..., 1|D1,
+    1|D2, D3) of x's rank, converted to fp32. A row whose entries are all masked is uniform, 1 / D3. bench > 0 times
+    that many launches of the forward (and of the gradient, in the backward) and prints one line each."""
+    x = _dense_input(x, "masked_softmax")
+    mask, M1, M2 = _dense_mask(x, mask, "masked_softmax")
+    if bench:
+        _dense_bench("masked_softmax %s %s" % (tuple(x.shape), str(x.dtype).replace("torch.", "")),
+                     lambda: _dense_softmax_fwd(x, mask, M1, M2, scale), _softmax_bytes(x, mask, 2), bench)
+    return _DenseSoftmaxFunction.apply(x, mask, M1, M2, float(scale), int(bench))
+
+
+def softmax(x, scale=1.0, bench=0):
+    """masked_softmax without a mask (reference transformer.py:570-571)."""
+    return masked_softmax(x, None, scale, bench)
+
+
+def masked_top_k_softmax(x, k, mask=None, scale=1.0):
+    """Softmax over the k largest v of each row (v as in masked_softmax), 0 elsewhere (reference transformer.py:552-567,
+    627-649). Entries rank by v descending, then by index ascending: a row with fewer than k visible entries fills the
+    remaining slots with its lowest-index masked columns, which get 0; a fully masked row gives 1/k on its first k
+    columns. Needs 1 <= k <= x.shape[-1] <= 1024."""
+    x = _dense_input(x, "masked_top_k_softmax")
+    k = _check_k(x, k, "masked_top_k_softmax")
+    mask, M1, M2 = _dense_mask(x, mask, "masked_top_k_softmax")
+    return _TopKSoftmaxFunction.apply(x, mask, M1, M2, k, float(scale))
+
+
+def top_k(x, k):
+    """(values, int32 indices) of the k largest entries of each row, shape (..., k), ordered by rank: value descending,
+    then index ascending (reference transformer.py:494-496). Values are bit-exact copies of x's entries. Needs
+    1 <= k <= x.shape[-1] <= 1024."""
+    x = _dense_input(x, "top_k")
+    k = _check_k(x, k, "top_k")
+    return _TopKFunction.apply(x, k)
+
+
+def rectified_top_k(x, k, rebase=True):
+    """x's shape: each top-k entry becomes max(x, base) - base with base = max(kth largest value, 0) if rebase else 0;
+    every other entry is 0 (reference transformer.py:498-500, 536-549). Needs 1 <= k <= x.shape[-1] <= 1024."""
+    x = _dense_input(x, "rectified_top_k")
+    k = _check_k(x, k, "rectified_top_k")
+    return _RectifiedTopKFunction.apply(x, k, _TOPK_REBASE if rebase else _TOPK_RECTIFIED)

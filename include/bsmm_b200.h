@@ -19,6 +19,9 @@
  *   bst_softmax_grad      <- BlocksparseSoftmaxGrad<T,V>   (src/bst_op.cc:443-512)
  *   bst_autoregressive_mask <- BstPartialAutoregressiveMask (src/bst_op.cc:519-575)
  *   bst_attention         <- no single launcher: replaces bst_nt + bst_masked_softmax + bst_xn (NN)
+ *   bst_dense_softmax(_grad) <- MaskedSoftmax / MaskedSoftmaxGrad (src/transformer_op.cc:211-367)
+ *   bst_topk_softmax      <- MaskedTopKSoftmax (src/transformer_op.cc:145-208)
+ *   bst_topk              <- TopK behind Topk / RectifiedTopK (src/transformer_op.cc:20-141)
  *   bsmm_block_norm / bsmm_l2_decay / bsmm_threshold_prune / bsmm_prune_topk
  *                         <- BlocksparseNorm / BlocksparseL2Decay / BlocksparseThresholdPrune / BlocksparsePrune
  *                            (src/optimize_op_gpu.cu:794-1098)
@@ -260,6 +263,43 @@ int bst_attention_grad(int dtype, int bsize, const int32_t* nn_lut, const int32_
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,
                             const void* mask_in, void* mask_out, int autoregress_at_key,
                             void* stream);
+
+/* ---- dense softmax and top-k (the reference's transformer module outside BlocksparseTransformer) ---------------- */
+
+/*
+ * y = softmax over D3 of v, v = x * m * scale where m != 0 and -FLT_MAX where m == 0 (no mask: v = x * scale).
+ * Replaces MaskedSoftmax (src/transformer_op.cc:211-286).
+ *   x, y: (D0, D1, D2, D3) of dtype, contiguous; any alignment (16-byte vector accesses where every row start allows).
+ *   mask: NULL, or fp32 (1|D1, 1|D2, D3) with element strides (mask_stride1, mask_stride2, 1): mask_stride2 is 0
+ *         (broadcast) or D3, mask_stride1 is 0 or D3 * (mask_stride2 ? D2 : 1). The strides come from the mask's own
+ *         shape; the reference derives mask_stride1 from x's D2 (transformer_op.cc:184-185).
+ *   A row whose entries are all masked is uniform, 1 / D3. Rows of any length; 64-bit element offsets.
+ * D3 <= 0, negative sizes, a bad dtype, null x / y or other strides: BSMM_E_ARG before any launch. D0*D1*D2 = 0
+ * launches nothing. Kernels: dense_softmax_warp (D3 <= 1024), dense_softmax_cta (<= 8192), dense_softmax_long.
+ */
+int bst_dense_softmax(int dtype, const void* x, const float* mask, void* y, long long D0, int D1, int D2, int D3,
+                      long long mask_stride1, long long mask_stride2, float scale, void* stream);
+
+/* dx = (dy - sum_D3(dy * y)) * y * m * scale (no mask: m = 1), all of dtype; shapes, mask and errors as
+ * bst_dense_softmax. Replaces MaskedSoftmaxGrad (src/transformer_op.cc:289-367). Kernels: dense_softmax_grad_warp /
+ * _cta / _long on the same row-length routes. */
+int bst_dense_softmax_grad(int dtype, const void* dy, const void* y, const float* mask, void* dx, long long D0, int D1,
+                           int D2, int D3, long long mask_stride1, long long mask_stride2, float scale, void* stream);
+
+/* y = softmax over the k largest v of each row (v as bst_dense_softmax), 0 elsewhere. Entries rank by v descending, then
+ * by index ascending, so a row with fewer than k visible entries fills its k slots with its lowest-index masked columns,
+ * which get 0 (1 / k each when the whole row is masked). Needs 1 <= k <= D3 <= 1024 (BSMM_E_ARG otherwise). Replaces
+ * MaskedTopKSoftmax (src/transformer_op.cc:145-208). Kernel: dense_topk_softmax. */
+int bst_topk_softmax(int dtype, const void* x, const float* mask, void* y, long long D0, int D1, int D2, int D3,
+                     long long mask_stride1, long long mask_stride2, int k, float scale, void* stream);
+
+/* The k largest entries of each of `rows` rows of D3 entries, ranked by value descending, then index ascending.
+ *   mode 0: y (rows, k) of dtype = bit-exact copies of the entries in rank order, idx (rows, k) int32 = their columns;
+ *   mode 1: y (rows, D3) = max(x, 0) at the top-k entries, 0 elsewhere (idx may be NULL);
+ *   mode 2: as 1 with base = max(kth largest entry, 0): y = max(x, base) - base at the top-k entries.
+ * Needs 1 <= k <= D3 <= 1024 (BSMM_E_ARG otherwise). Replaces TopK (src/transformer_op.cc:20-141), which the Topk and
+ * RectifiedTopK ops share. Kernels: dense_topk (mode 0), dense_topk_rectified (modes 1, 2). */
+int bst_topk(int dtype, const void* x, void* y, int32_t* idx, long long rows, int D3, int k, int mode, void* stream);
 
 /* ---- utilities on the (blocks, bsize, bsize) weight format -------------------------------------- */
 

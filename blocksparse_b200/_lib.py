@@ -44,6 +44,9 @@ SIGNATURES = {
     "bst_dense_softmax_grad": (_i, [_i, _vp, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),
     "bst_topk_softmax": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _i, _f, _vp]),
     "bst_topk": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _i, _vp]),
+    "bst_softmax_xent": (_i, [_i, _i, _vp, _vp, _vp, _vp, _ll, _i, _vp]),
+    "bst_softmax_xent_grad": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _i, _vp]),
+    "bst_transpose_0213": (_i, [_i, _vp, _vp, _ll, _ll, _ll, _ll, _vp]),
     "bsmm_block_norm": (_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),
@@ -131,6 +134,23 @@ def dtype_code(torch_dtype):
         return _DTYPE_CODES[torch_dtype]
     except KeyError:
         raise ValueError("unsupported dtype %s (float32, float16, bfloat16 only)" % (torch_dtype,))
+
+
+LABEL_U8, LABEL_U16, LABEL_I32, LABEL_I64 = 0, 1, 2, 3     # BSMM_LABEL_*
+_LABEL_CODES = None
+
+
+def label_code(torch_dtype):
+    global _LABEL_CODES
+    if _LABEL_CODES is None:
+        import torch
+        _LABEL_CODES = {torch.uint8: LABEL_U8, torch.int32: LABEL_I32, torch.int64: LABEL_I64}
+        if hasattr(torch, "uint16"):
+            _LABEL_CODES[torch.uint16] = LABEL_U16
+    try:
+        return _LABEL_CODES[torch_dtype]
+    except KeyError:
+        raise ValueError("unsupported label dtype %s (uint8, uint16, int32, int64 only)" % (torch_dtype,))
 
 
 def ptr(t):

@@ -1,11 +1,13 @@
 // C ABI of libbsmm_b200.so -- argument validation and kernel-family dispatch.
 // See include/bsmm_b200.h for the contract and the reference launchers each entry replaces.
 #include <atomic>
+#include <climits>
 #include "common.cuh"
 #include "dense_softmax.cuh"
 #include "generic.cuh"
 #include "softmax.cuh"
 #include "tc.cuh"
+#include "transpose.cuh"
 #include "wutil.cuh"
 
 using namespace bsmm;
@@ -471,6 +473,52 @@ int bst_topk_softmax(int dtype, const void* x, const float* mask, void* y, long 
   a.a = x; a.out = y; a.k = k; a.mode = TOPK_SOFTMAX; a.scale = scale;
   BSMM_DISPATCH_DTYPE(dtype, T, { return launch_dense_topk<T>(a, (cudaStream_t)stream); });
   return 0;
+}
+
+// ---- softmax cross entropy (csrc/dense_softmax.cuh) and transpose (csrc/transpose.cuh) -------------------------------
+static int xent_args(const char* what, int dtype, int label_type, long long N, int K) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "%s: unsupported dtype code %d", what, dtype);
+  if (label_type < BSMM_LABEL_U8 || label_type > BSMM_LABEL_I64)
+    return fail(BSMM_E_ARG, "%s: unsupported label type %d", what, label_type);
+  if (N < 0 || K <= 0) return fail(BSMM_E_ARG, "%s: bad sizes N %lld, K %d", what, N, K);
+  // one CTA per row on the CTA route; grid.x holds at most 2^31 - 1
+  if (N > 0x7fffffffLL * (K <= DSM_WARP_MAX ? DSM_WARPS : 1)) return fail(BSMM_E_LIMIT, "%s: %lld rows exceed the grid", what, N);
+  return 0;
+}
+
+int bst_softmax_xent(int dtype, int label_type, const void* logits, const void* labels, float* loss, float* lse,
+                     long long N, int K, void* stream) {
+  if (int e = xent_args("bst_softmax_xent", dtype, label_type, N, K)) return e;
+  if (!logits || !labels || !loss || !lse) return fail(BSMM_E_ARG, "bst_softmax_xent: null pointer");
+  if (N == 0) return 0;
+  XentArgs a = {};
+  a.x = logits; a.labels = labels; a.loss = loss; a.lse = lse; a.rows = N; a.K = K; a.label_type = label_type;
+  const bool vec = aligned16(logits) && K % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_softmax_xent<T>(a, false, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bst_softmax_xent_grad(int dtype, int label_type, const void* logits, const void* labels, const float* lse,
+                          const float* dy, void* dx, long long N, int K, void* stream) {
+  if (int e = xent_args("bst_softmax_xent_grad", dtype, label_type, N, K)) return e;
+  if (!logits || !labels || !lse || !dy || !dx) return fail(BSMM_E_ARG, "bst_softmax_xent_grad: null pointer");
+  if (N == 0) return 0;
+  XentArgs a = {};
+  a.x = logits; a.labels = labels; a.lse_in = lse; a.dy = dy; a.dx = dx; a.rows = N; a.K = K; a.label_type = label_type;
+  const bool vec = aligned16(logits) && aligned16(dx) && K % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_softmax_xent<T>(a, true, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bst_transpose_0213(int dtype, const void* x, void* y, long long D0, long long D1, long long D2, long long D3,
+                       void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bst_transpose_0213: unsupported dtype code %d", dtype);
+  if (D0 < 0 || D1 < 0 || D2 < 0 || D3 < 0)
+    return fail(BSMM_E_ARG, "bst_transpose_0213: bad sizes (%lld, %lld, %lld, %lld)", D0, D1, D2, D3);
+  if (!x || !y) return fail(BSMM_E_ARG, "bst_transpose_0213: null pointer");
+  if (D0 == 0 || D1 == 0 || D2 == 0 || D3 == 0) return 0;
+  if (D0 > LLONG_MAX / D1 / D2 / D3) return fail(BSMM_E_LIMIT, "bst_transpose_0213: more than 2^63 elements");
+  return launch_transpose_0213(dtype_size(dtype), x, y, D0, D1, D2, D3, (cudaStream_t)stream);
 }
 
 int bst_topk(int dtype, const void* x, void* y, int32_t* idx, long long rows, int D3, int k, int mode, void* stream) {

@@ -374,7 +374,152 @@ __global__ void __launch_bounds__(512) dense_topk_kernel(DenseArgs a, int npow2)
   for (int i = tid; i < D3; i += nt) y[i] = from_f32<T>(outrow[i]);
 }
 
+// ---- softmax cross entropy (bst_softmax_xent, bst_softmax_xent_grad) ------------------------------------------------------
+// loss[n] = lse[n] - x[n, label[n]] with lse[n] = logsumexp(x[n, :]); dx[n, j] = dy[n] * (exp(x[n, j] - lse[n]) - [j == label]).
+// Nothing is written per element in the forward, so no route keeps a row in registers: every thread runs an online
+// (max, sum) over its chunks in index order (xent_unroll chunks loaded before any is used), then the (max, sum) pairs are
+// combined across the row. A partial whose entries are all -inf is (m = -inf, s = 0) and must stay so: it never adds
+// exp(-inf - (-inf)) = NaN, and it is rescaled to 0 in the combine. A label outside [0, K) makes the row's loss, lse
+// and gradient NaN, with no device assert: the label is compared, never used as an address unless it is in range.
+struct XentArgs {
+  const void* x;          // logits (N, K)
+  const void* labels;     // N labels of label_type
+  const float* lse_in;    // gradient: the forward's lse
+  const float* dy;        // gradient: d(loss)
+  float* loss;            // forward
+  float* lse;             // forward
+  void* dx;               // gradient
+  long long rows;
+  int K, label_type;
+};
+
+__device__ __forceinline__ long long xent_label(const void* p, int type, long long n) {
+  switch (type) {
+    case BSMM_LABEL_U8:  return __ldg(reinterpret_cast<const uint8_t*>(p) + n);
+    case BSMM_LABEL_U16: return __ldg(reinterpret_cast<const uint16_t*>(p) + n);
+    case BSMM_LABEL_I32: return __ldg(reinterpret_cast<const int32_t*>(p) + n);
+    default:       return __ldg(reinterpret_cast<const long long*>(p) + n);
+  }
+}
+
+template <int VEC>
+constexpr int xent_unroll() { return VEC == 1 ? 8 : 4; }
+
+// Row w and thread t of the row on either route (THREADS = 32: a warp per row, DSM_WARPS rows per CTA).
+template <int THREADS>
+__device__ __forceinline__ bool xent_row(long long rows, long long& w, int& t) {
+  if (THREADS == 32) {
+    w = (long long)blockIdx.x * DSM_WARPS + (threadIdx.x >> 5);
+    t = threadIdx.x & 31;
+    return w < rows;                           // whole warps leave; this route has no CTA barrier
+  }
+  w = blockIdx.x;
+  t = threadIdx.x;
+  return true;
+}
+
+template <typename T, int VEC, int THREADS>
+__global__ void __launch_bounds__(THREADS == 32 ? 32 * DSM_WARPS : THREADS) softmax_xent_kernel(XentArgs a) {
+  __shared__ float sh[32];
+  constexpr int U = xent_unroll<VEC>();
+  constexpr long long STEP = (long long)THREADS * VEC;
+  long long n;
+  int t;
+  if (!xent_row<THREADS>(a.rows, n, t)) return;
+  const int K = a.K;
+  const T* x = reinterpret_cast<const T*>(a.x) + n * K;
+  float mx = -INFINITY, s = 0.f;
+  for (long long c0 = (long long)t * VEC; c0 < K; c0 += U * STEP) {
+    float v[U][VEC];
+#pragma unroll
+    for (int u = 0; u < U; ++u)
+      if (c0 + u * STEP < K) dsm_ld<T, VEC, true>(x + c0 + u * STEP, v[u]);
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      if (c0 + u * STEP >= K) break;
+      float cm = v[u][0];
+#pragma unroll
+      for (int j = 1; j < VEC; ++j) cm = fmaxf(cm, v[u][j]);
+      if (cm > mx) { s *= expf(mx - cm); mx = cm; }         // mx = -inf: s is 0 and expf(-inf) = 0
+      if (mx != -INFINITY) {
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) s += expf(v[u][j] - mx);
+      } else {
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) s += v[u][j] != v[u][j] ? v[u][j] : 0.f;   // keep a NaN entry's NaN
+      }
+    }
+  }
+  const float M = dsm_reduce<true>(mx, THREADS, sh);
+  const float S = dsm_reduce<false>(mx == -INFINITY ? s : s * expf(mx - M), THREADS, sh);
+  if (t == 0) {
+    const long long lab = xent_label(a.labels, a.label_type, n);
+    float lse = M + logf(S), loss = NAN;
+    if (lab >= 0 && lab < K) loss = lse - to_f32<T>(x[lab]);
+    else lse = NAN;
+    a.loss[n] = loss;
+    a.lse[n] = lse;
+  }
+}
+
+template <typename T, int VEC, int THREADS>
+__global__ void __launch_bounds__(THREADS == 32 ? 32 * DSM_WARPS : THREADS) softmax_xent_grad_kernel(XentArgs a) {
+  constexpr int U = xent_unroll<VEC>();
+  constexpr long long STEP = (long long)THREADS * VEC;
+  long long n;
+  int t;
+  if (!xent_row<THREADS>(a.rows, n, t)) return;
+  const int K = a.K;
+  const long long lab = xent_label(a.labels, a.label_type, n);
+  const float dy = __ldg(a.dy + n);
+  const float lse = lab >= 0 && lab < K ? __ldg(a.lse_in + n) : NAN;
+  const T* x = reinterpret_cast<const T*>(a.x) + n * K;
+  T* dx = reinterpret_cast<T*>(a.dx) + n * K;
+  for (long long c0 = (long long)t * VEC; c0 < K; c0 += U * STEP) {
+    float v[U][VEC];
+#pragma unroll
+    for (int u = 0; u < U; ++u)
+      if (c0 + u * STEP < K) dsm_ld<T, VEC, true>(x + c0 + u * STEP, v[u]);
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const long long c = c0 + u * STEP;
+      if (c >= K) break;
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) v[u][j] = dy * (expf(v[u][j] - lse) - (c + j == lab ? 1.f : 0.f));
+      dsm_st<T, VEC>(dx + c, v[u]);
+    }
+  }
+}
+
 // ---- launchers ------------------------------------------------------------------------------------------------------------
+template <typename T>
+int launch_softmax_xent(const XentArgs& a, bool grad, bool vec, cudaStream_t s) {
+  constexpr int V = 16 / sizeof(T);
+  const char* name;
+  if (a.K <= DSM_WARP_MAX) {
+    const unsigned grid = (unsigned)((a.rows + DSM_WARPS - 1) / DSM_WARPS);
+    if (grad) {
+      if (vec) softmax_xent_grad_kernel<T, V, 32><<<grid, 32 * DSM_WARPS, 0, s>>>(a);
+      else     softmax_xent_grad_kernel<T, 1, 32><<<grid, 32 * DSM_WARPS, 0, s>>>(a);
+    } else {
+      if (vec) softmax_xent_kernel<T, V, 32><<<grid, 32 * DSM_WARPS, 0, s>>>(a);
+      else     softmax_xent_kernel<T, 1, 32><<<grid, 32 * DSM_WARPS, 0, s>>>(a);
+    }
+    name = grad ? "softmax_xent_grad_warp" : "softmax_xent_warp";
+  } else {
+    const unsigned grid = (unsigned)a.rows;
+    if (grad) {
+      if (vec) softmax_xent_grad_kernel<T, V, DSM_CTA_THREADS><<<grid, DSM_CTA_THREADS, 0, s>>>(a);
+      else     softmax_xent_grad_kernel<T, 1, DSM_CTA_THREADS><<<grid, DSM_CTA_THREADS, 0, s>>>(a);
+    } else {
+      if (vec) softmax_xent_kernel<T, V, DSM_CTA_THREADS><<<grid, DSM_CTA_THREADS, 0, s>>>(a);
+      else     softmax_xent_kernel<T, 1, DSM_CTA_THREADS><<<grid, DSM_CTA_THREADS, 0, s>>>(a);
+    }
+    name = grad ? "softmax_xent_grad_cta" : "softmax_xent_cta";
+  }
+  return check_launch(name);
+}
+
 // vec: every row start of every operand is 16-byte aligned (checked by the caller).
 template <typename T>
 int launch_dense_softmax(const DenseArgs& a, bool grad, bool vec, cudaStream_t s) {

@@ -709,3 +709,127 @@ def rectified_top_k(x, k, rebase=True):
     x = _dense_input(x, "rectified_top_k")
     k = _check_k(x, k, "rectified_top_k")
     return _RectifiedTopKFunction.apply(x, k, _TOPK_REBASE if rebase else _TOPK_RECTIFIED)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Softmax cross entropy and the head transposes (reference blocksparse/transformer.py:664-700, exported by
+# blocksparse/__init__.py:128-130).
+@_on_device_of
+def _xent_fwd(x, labels):
+    """(loss, lse), fp32 of x.shape[:-1]; x contiguous, labels contiguous with one entry per row."""
+    loss = torch.empty(x.shape[:-1], dtype=torch.float32, device=x.device)
+    lse = torch.empty_like(loss)
+    if loss.numel() == 0:
+        return loss, lse
+    K = x.shape[-1]
+    rc = _lib.load().bst_softmax_xent(_lib.dtype_code(x.dtype), _lib.label_code(labels.dtype), x.data_ptr(),
+                                      labels.data_ptr(), loss.data_ptr(), lse.data_ptr(), loss.numel(), K,
+                                      _lib.stream_ptr())
+    _lib.check(rc, "bst_softmax_xent")
+    return loss, lse
+
+
+@_on_device_of
+def _xent_bwd(x, labels, lse, dy):
+    dy = dy.to(torch.float32).contiguous()
+    dx = torch.empty_like(x)
+    if lse.numel() == 0:
+        return dx
+    rc = _lib.load().bst_softmax_xent_grad(_lib.dtype_code(x.dtype), _lib.label_code(labels.dtype), x.data_ptr(),
+                                           labels.data_ptr(), lse.data_ptr(), dy.data_ptr(), dx.data_ptr(), lse.numel(),
+                                           x.shape[-1], _lib.stream_ptr())
+    _lib.check(rc, "bst_softmax_xent_grad")
+    return dx
+
+
+@_on_device_of
+def _transpose_0213(x, D0, D1, D2, D3):
+    """y (D0, D2, D1, D3) of x (D0, D1, D2, D3), contiguous; the caller shapes y."""
+    y = torch.empty((D0, D2, D1, D3), dtype=x.dtype, device=x.device)
+    if y.numel() == 0:
+        return y
+    rc = _lib.load().bst_transpose_0213(_lib.dtype_code(x.dtype), x.data_ptr(), y.data_ptr(), D0, D1, D2, D3,
+                                        _lib.stream_ptr())
+    _lib.check(rc, "bst_transpose_0213")
+    return y
+
+
+class _SoftmaxXentFunction(torch.autograd.Function):
+    """reference transformer.py:688-700, but the backward recomputes the probabilities from the saved logits and the
+    fp32 log-sum-exp instead of reading a gradient the forward stored: three passes over (N, K) instead of four, and dx
+    is rounded once from fp32."""
+
+    @staticmethod
+    def forward(ctx, logits, labels):
+        loss, lse = _xent_fwd(logits, labels)
+        ctx.save_for_backward(logits, labels, lse)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dy):
+        logits, labels, lse = ctx.saved_tensors
+        return _xent_bwd(logits, labels, lse, dy), None
+
+
+class _Transpose0213Function(torch.autograd.Function):
+    """reference transformer.py:679-683: the gradient is the same transpose of dy."""
+
+    @staticmethod
+    def forward(ctx, x):
+        return _transpose_0213(x, *x.shape)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return _transpose_0213(dy.contiguous(), *dy.shape)
+
+
+class _Transpose2DFunction(torch.autograd.Function):
+    """reference transformer.py:671-675."""
+
+    @staticmethod
+    def forward(ctx, x):
+        return _transpose_0213(x, 1, x.shape[0], x.shape[1], 1).view(x.shape[1], x.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        return _transpose_0213(dy.contiguous(), 1, dy.shape[0], dy.shape[1], 1).view(dy.shape[1], dy.shape[0])
+
+
+def softmax_cross_entropy(logits=None, labels=None):
+    """Per-row loss logsumexp(logits[n, :]) - logits[n, labels[n]], fp32 of shape logits.shape[:-1], nothing reduced
+    (reference transformer.py:688-696). logits: CUDA, fp32 / fp16 / bf16, rank >= 1, any K >= 1. labels: uint8, uint16,
+    int32 or int64 with one entry per row, any shape. Differentiable with respect to logits: dx = dy * (softmax(logits) -
+    onehot(labels)) in logits' dtype. A label outside [0, K) gives NaN for its row's loss and gradient, -inf logits get
+    probability 0, and a row of -inf only gives NaN."""
+    if logits is None or labels is None:
+        raise ValueError("softmax_cross_entropy needs logits and labels")
+    logits = _dense_input(logits, "softmax_cross_entropy")
+    K = logits.shape[-1]
+    if not 1 <= K < 2 ** 31:
+        raise ValueError("softmax_cross_entropy needs 1 <= logits.shape[-1] < 2^31, got %d" % K)
+    if not torch.is_tensor(labels) or labels.device != logits.device:
+        raise ValueError("softmax_cross_entropy: labels must be a tensor on the logits' device %s" % logits.device)
+    _lib.label_code(labels.dtype)
+    if labels.numel() != logits.numel() // K:
+        raise ValueError("softmax_cross_entropy: %d labels for %d rows" % (labels.numel(), logits.numel() // K))
+    return _SoftmaxXentFunction.apply(logits, labels.contiguous().view(-1))
+
+
+def _transpose_input(x, rank, what):
+    if not torch.is_tensor(x) or not x.is_cuda:
+        raise ValueError("%s needs a CUDA tensor (there is no CPU path)" % what)
+    if x.dim() != rank:
+        raise ValueError("%s needs a tensor of rank %d, got shape %s" % (what, rank, tuple(x.shape)))
+    _lib.dtype_code(x.dtype)
+    return x.contiguous()
+
+
+def transpose_0213(x):
+    """(D0, D1, D2, D3) -> (D0, D2, D1, D3), a bit-exact copy (reference transformer.py:677-683): splits or merges
+    attention heads. fp32 / fp16 / bf16, no limit on the dims."""
+    return _Transpose0213Function.apply(_transpose_input(x, 4, "transpose_0213"))
+
+
+def transpose_2d(x):
+    """(D0, D1) -> (D1, D0), a bit-exact copy (reference transformer.py:671-675)."""
+    return _Transpose2DFunction.apply(_transpose_input(x, 2, "transpose_2d"))

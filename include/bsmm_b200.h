@@ -22,6 +22,8 @@
  *   bst_dense_softmax(_grad) <- MaskedSoftmax / MaskedSoftmaxGrad (src/transformer_op.cc:211-367)
  *   bst_topk_softmax      <- MaskedTopKSoftmax (src/transformer_op.cc:145-208)
  *   bst_topk              <- TopK behind Topk / RectifiedTopK (src/transformer_op.cc:20-141)
+ *   bst_softmax_xent(_grad) <- SoftmaxCrossEntropy / SoftmaxCrossEntropyGrad (src/transformer_op.cc:462-587)
+ *   bst_transpose_0213    <- Transpose0213 / Transpose2D (src/transformer_op.cc:369-459)
  *   bsmm_block_norm / bsmm_l2_decay / bsmm_threshold_prune / bsmm_prune_topk
  *                         <- BlocksparseNorm / BlocksparseL2Decay / BlocksparseThresholdPrune / BlocksparsePrune
  *                            (src/optimize_op_gpu.cu:794-1098)
@@ -300,6 +302,38 @@ int bst_topk_softmax(int dtype, const void* x, const float* mask, void* y, long 
  * Needs 1 <= k <= D3 <= 1024 (BSMM_E_ARG otherwise). Replaces TopK (src/transformer_op.cc:20-141), which the Topk and
  * RectifiedTopK ops share. Kernels: dense_topk (mode 0), dense_topk_rectified (modes 1, 2). */
 int bst_topk(int dtype, const void* x, void* y, int32_t* idx, long long rows, int D3, int k, int mode, void* stream);
+
+/* label types of bst_softmax_xent(_grad) */
+enum { BSMM_LABEL_U8 = 0, BSMM_LABEL_U16 = 1, BSMM_LABEL_I32 = 2, BSMM_LABEL_I64 = 3 };
+
+/*
+ * Per row n of logits (N, K) of dtype, contiguous: lse[n] = logsumexp(logits[n, :]) and
+ * loss[n] = lse[n] - logits[n, labels[n]], both fp32. labels: N integers of label_type.
+ * Replaces SoftmaxCrossEntropy (src/transformer_op.cc:462-531), without its limits: any K >= 1 (the reference needs
+ * K <= 65536 and a multiple of 8), every dtype, 64-bit element offsets, and the sum is formed from fp32 exponentials.
+ *   A label outside [0, K) (negative included) makes loss[n] and lse[n] NaN; other rows are unaffected, and nothing
+ *   faults or synchronises. -inf logits get probability 0; a label at a -inf entry gives +inf; a row of -inf only gives
+ *   lse -inf and loss NaN.
+ * A bad dtype or label type, null pointers, N < 0 or K <= 0: BSMM_E_ARG before any launch. N = 0 launches nothing.
+ * Kernels: softmax_xent_warp (K <= 1024, a warp per row), softmax_xent_cta (a 256-thread CTA per row); 16-byte loads where
+ * logits is 16-byte aligned and K a multiple of 16 / element size, one element per load otherwise.
+ */
+int bst_softmax_xent(int dtype, int label_type, const void* logits, const void* labels, float* loss, float* lse,
+                     long long N, int K, void* stream);
+
+/* dx[n, j] = dy[n] * (exp(logits[n, j] - lse[n]) - [j == labels[n]]) in dtype, from the logits and the lse of
+ * bst_softmax_xent; dy and lse are fp32 [N]. A row whose label is outside [0, K) gets NaN. Replaces
+ * SoftmaxCrossEntropyGrad (src/transformer_op.cc:533-587), which reads a stored fp16 gradient instead of the logits.
+ * Shapes and errors as bst_softmax_xent. Kernels: softmax_xent_grad_warp / _cta on the same routes. */
+int bst_softmax_xent_grad(int dtype, int label_type, const void* logits, const void* labels, const float* lse,
+                          const float* dy, void* dx, long long N, int K, void* stream);
+
+/* y (D0, D2, D1, D3) = x (D0, D1, D2, D3) with dims 1 and 2 swapped, bit for bit; transpose_2d is (1, D0, D1, 1).
+ * Replaces Transpose0213 and Transpose2D (src/transformer_op.cc:369-459), without their D0, D1 < 65536 limit and their
+ * dims-multiple-of-4 requirement. A bad dtype, null pointers or negative sizes: BSMM_E_ARG before any launch; a zero size
+ * launches nothing. Kernels: transpose_rows (D3 * element size >= 16 bytes), transpose_tile (narrower). */
+int bst_transpose_0213(int dtype, const void* x, void* y, long long D0, long long D1, long long D2, long long D3,
+                       void* stream);
 
 /* ---- utilities on the (blocks, bsize, bsize) weight format -------------------------------------- */
 

@@ -4,12 +4,13 @@ Drop-in for the hot path of openai/blocksparse: `BlocksparseMatMul` (fprop / bpr
 updat, group_param_grads) and `BlocksparseTransformer` (NT / NN / TN + masked softmax),
 implemented as hand-written sm_90a CUDA behind the C ABI in include/bsmm_b200.h, plus the dense ops of the
 reference's transformer module (softmax, masked_softmax, masked_top_k_softmax, top_k, rectified_top_k,
-softmax_cross_entropy, transpose_0213, transpose_2d).
+softmax_cross_entropy, transpose_0213, transpose_2d) and of its norms module (layer_norm).
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
 from .optimize import blocksparse_l2_decay, blocksparse_norm, blocksparse_prune
 from .transformer import (BlocksparseTransformer, masked_softmax, masked_top_k_softmax, rectified_top_k, softmax,
                           softmax_cross_entropy, top_k, transpose_0213, transpose_2d)
+from .norms import layer_norm
 from .lut import z_order_2d
 from . import _lib
 
@@ -17,4 +18,4 @@ __version__ = "0.1.0"
 __all__ = ["BlocksparseMatMul", "BlocksparseTransformer", "SparseProj", "group_param_grads", "blocksparse_reduced_dw",
            "block_reduced_full_dw", "blocksparse_norm", "blocksparse_prune", "blocksparse_l2_decay", "z_order_2d",
            "softmax", "masked_softmax", "masked_top_k_softmax", "top_k", "rectified_top_k", "softmax_cross_entropy",
-           "transpose_0213", "transpose_2d"]
+           "transpose_0213", "transpose_2d", "layer_norm"]

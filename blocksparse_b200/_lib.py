@@ -47,7 +47,10 @@ SIGNATURES = {
     "bst_softmax_xent": (_i, [_i, _i, _vp, _vp, _vp, _vp, _ll, _i, _vp]),
     "bst_softmax_xent_grad": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _i, _vp]),
     "bst_transpose_0213": (_i, [_i, _vp, _vp, _ll, _ll, _ll, _ll, _vp]),
-    "bsmm_block_norm": (_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
+    "bsmm_layer_norm": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _i, _f, _i, _vp]),
+    "bsmm_layer_norm_grad": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _i, _f, _i, _vp]),
+    "bsmm_layer_norm_workspace_bytes": (_c.c_size_t, [_i, _ll, _i, _i]),
+    "bsmm_block_norm":(_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),
     "bsmm_prune_topk": (_i, [_vp, _vp, _i, _i, _vp]),

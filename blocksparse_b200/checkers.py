@@ -217,3 +217,47 @@ def rectified_top_k_test(x, k, rebase=True):
     y = np.zeros(x.shape, dtype=np.float32)
     np.put_along_axis(y, top, np.maximum(v, base) - base, axis=-1)
     return y
+
+
+# ---- module-level checkers of layer norm (reference blocksparse/norms.py, layer_norm_test / layer_norm_grad_test) ------
+# Restated on a (rows, segments, L) view: the feature axis last, or first (x viewed as (K, N) and transposed).
+def _segment_view(a, axis, segments):
+    a = np.asarray(a)
+    K = a.shape[axis]
+    a2 = a.reshape(K, -1).T if axis == 0 else a.reshape(-1, K)
+    return a2.reshape(a2.shape[0], segments, K // segments)
+
+
+def _segment_unview(v, shape, axis):
+    v = v.reshape(v.shape[0], -1)
+    return (v.T if axis == 0 else v).reshape(shape)
+
+
+def layer_norm_test(x, g, b, axis=1, segments=1, epsilon=1e-6, relu=False):
+    """y = relu?(xhat * g + b), the mean and the (biased) variance per segment of each row along `axis`."""
+    xs = _segment_view(x, axis, segments)
+    gs, bs = (np.asarray(p).reshape(1, segments, -1) for p in (g, b))
+    xhat = (xs - xs.mean(axis=2, keepdims=True)) / np.sqrt(xs.var(axis=2, keepdims=True) + epsilon)
+    y = xhat * gs + bs
+    if relu:
+        y = np.maximum(y, 0.0)
+    return _segment_unview(y, np.shape(x), axis).astype(np.result_type(x, np.float32))
+
+
+def layer_norm_grad_test(dy, x, g, b, axis=1, segments=1, epsilon=1e-6, relu=False):
+    """(dx, dg, db) of layer_norm_test; with relu, dy is masked where the pre-activation is not positive. dg and db
+    have g's shape: (K, 1) for axis 0, (1, K) otherwise, as the reference returns them."""
+    xs, dys = _segment_view(x, axis, segments), _segment_view(dy, axis, segments)
+    gs, bs = (np.asarray(p).reshape(1, segments, -1) for p in (g, b))
+    L = xs.shape[2]
+    rstd = 1.0 / np.sqrt(xs.var(axis=2, keepdims=True) + epsilon)
+    xhat = (xs - xs.mean(axis=2, keepdims=True)) * rstd
+    if relu:
+        dys = dys * (xhat * gs + bs > 0)
+    dg = (dys * xhat).sum(axis=0).reshape(-1)
+    db = dys.sum(axis=0).reshape(-1)
+    dyg = dys * gs
+    dx = (dyg - (xhat * (dyg * xhat).sum(axis=2, keepdims=True) + dyg.sum(axis=2, keepdims=True)) / L) * rstd
+    shape = (-1, 1) if axis == 0 else (1, -1)
+    dt = np.result_type(x, np.float32)
+    return (_segment_unview(dx, np.shape(x), axis).astype(dt), dg.reshape(shape).astype(dt), db.reshape(shape).astype(dt))

@@ -5,6 +5,7 @@
 #include "common.cuh"
 #include "dense_softmax.cuh"
 #include "generic.cuh"
+#include "layer_norm.cuh"
 #include "softmax.cuh"
 #include "tc.cuh"
 #include "transpose.cuh"
@@ -533,6 +534,68 @@ int bst_topk(int dtype, const void* x, void* y, int32_t* idx, long long rows, in
   a.a = x; a.out = y; a.idx = idx; a.D3 = D3; a.k = k; a.mode = mode; a.rows = rows;
   a.map = {1, 1, 0, 0, rows};
   BSMM_DISPATCH_DTYPE(dtype, T, { return launch_dense_topk<T>(a, (cudaStream_t)stream); });
+  return 0;
+}
+
+// ---- layer norm (csrc/layer_norm.cuh) -------------------------------------------------------------------------------------
+static int ln_args(const char* what, int dtype, int gdtype, int axis, long long N, int K, int segments, float epsilon) {
+  if (!dense_dtype_ok(dtype) || !dense_dtype_ok(gdtype))
+    return fail(BSMM_E_ARG, "%s: unsupported dtype codes %d, %d", what, dtype, gdtype);
+  if (axis != 0 && axis != 1) return fail(BSMM_E_ARG, "%s: axis must be 0 or 1, got %d", what, axis);
+  if (N < 0 || K <= 0 || segments <= 0 || K % segments)
+    return fail(BSMM_E_ARG, "%s: bad sizes N %lld, K %d, segments %d", what, N, K, segments);
+  if (axis == 0 && segments != 1) return fail(BSMM_E_ARG, "%s: segments need axis 1", what);
+  if (!(epsilon >= 0.f)) return fail(BSMM_E_ARG, "%s: epsilon must be >= 0", what);
+  const int L = K / segments;
+  if (axis == 1 && N * segments > 0x7fffffffLL * (L <= DSM_WARP_MAX ? DSM_WARPS : 1))
+    return fail(BSMM_E_LIMIT, "%s: %lld rows exceed the grid", what, N * segments);
+  if (axis == 0 && (N > 0x7fffffffLL * 32 || K > 65535LL * LN_CN_MIN_ROWS))
+    return fail(BSMM_E_LIMIT, "%s: N %lld or K %d exceeds the grid", what, N, K);
+  return 0;
+}
+
+size_t bsmm_layer_norm_workspace_bytes(int axis, long long N, int K, int segments) {
+  if ((axis != 0 && axis != 1) || N <= 0 || K <= 0 || segments <= 0 || K % segments) return 0;
+  return ln_workspace_floats(axis, N, K, segments) * sizeof(float);
+}
+
+int bsmm_layer_norm(int dtype, int gdtype, int axis, const void* x, const void* g, const void* b, void* y, float* mean,
+                    float* rstd, void* workspace, long long N, int K, int segments, float epsilon, int relu, void* stream) {
+  if (int e = ln_args("bsmm_layer_norm", dtype, gdtype, axis, N, K, segments, epsilon)) return e;
+  if (!x || !g || !b || !y || !mean || !rstd || (axis == 0 && !workspace)) return fail(BSMM_E_ARG, "bsmm_layer_norm: null pointer");
+  if (N == 0) return 0;
+  LnArgs a = {};
+  a.x = x; a.g = g; a.b = b; a.gdtype = gdtype; a.y = y; a.mean = mean; a.rstd = rstd; a.ws = (float*)workspace;
+  a.N = N; a.K = K; a.S = segments; a.L = K / segments; a.eps = epsilon; a.relu = relu != 0;
+  const int V = 16 / dtype_size(dtype);
+  if (axis == 0) {
+    const bool vec = aligned16(x) && aligned16(y) && N % V == 0;
+    BSMM_DISPATCH_DTYPE(dtype, T, { return launch_layer_norm_cn<T>(a, false, vec, gdtype, nullptr, nullptr, (cudaStream_t)stream); });
+  } else {
+    const bool vec = aligned16(x) && aligned16(y) && a.L % V == 0;
+    BSMM_DISPATCH_DTYPE(dtype, T, { return launch_layer_norm_nc<T>(a, false, vec, gdtype, nullptr, nullptr, (cudaStream_t)stream); });
+  }
+  return 0;
+}
+
+int bsmm_layer_norm_grad(int dtype, int gdtype, int axis, const void* dy, const void* x, const void* g, const void* b,
+                         const float* mean, const float* rstd, void* dx, void* dg, void* db, void* workspace, long long N,
+                         int K, int segments, float epsilon, int relu, void* stream) {
+  if (int e = ln_args("bsmm_layer_norm_grad", dtype, gdtype, axis, N, K, segments, epsilon)) return e;
+  if (!dy || !x || !g || !b || !mean || !rstd || !dx || !dg || !db || !workspace)
+    return fail(BSMM_E_ARG, "bsmm_layer_norm_grad: null pointer");
+  if (N == 0) return 0;
+  LnArgs a = {};
+  a.x = x; a.dy = dy; a.g = g; a.b = b; a.gdtype = gdtype; a.y = dx; a.mean = (float*)mean; a.rstd = (float*)rstd;
+  a.ws = (float*)workspace; a.N = N; a.K = K; a.S = segments; a.L = K / segments; a.eps = epsilon; a.relu = relu != 0;
+  const int V = 16 / dtype_size(dtype);
+  if (axis == 0) {
+    const bool vec = aligned16(x) && aligned16(dy) && aligned16(dx) && N % V == 0;
+    BSMM_DISPATCH_DTYPE(dtype, T, { return launch_layer_norm_cn<T>(a, true, vec, gdtype, dg, db, (cudaStream_t)stream); });
+  } else {
+    const bool vec = aligned16(x) && aligned16(dy) && aligned16(dx) && a.L % V == 0;
+    BSMM_DISPATCH_DTYPE(dtype, T, { return launch_layer_norm_nc<T>(a, true, vec, gdtype, dg, db, (cudaStream_t)stream); });
+  }
   return 0;
 }
 

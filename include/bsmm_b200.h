@@ -24,6 +24,9 @@
  *   bst_topk              <- TopK behind Topk / RectifiedTopK (src/transformer_op.cc:20-141)
  *   bst_softmax_xent(_grad) <- SoftmaxCrossEntropy / SoftmaxCrossEntropyGrad (src/transformer_op.cc:462-587)
  *   bst_transpose_0213    <- Transpose0213 / Transpose2D (src/transformer_op.cc:369-459)
+ *   bsmm_layer_norm       <- LayerNormForward_NC / LayerNormSegmentedForward_NC / LayerNormForward_CN
+ *                            (src/layer_norm_op.cc)
+ *   bsmm_layer_norm_grad  <- LayerNormBackward_NC / LayerNormSegmentedBackward_NC / LayerNormBackward_CN
  *   bsmm_block_norm / bsmm_l2_decay / bsmm_threshold_prune / bsmm_prune_topk
  *                         <- BlocksparseNorm / BlocksparseL2Decay / BlocksparseThresholdPrune / BlocksparsePrune
  *                            (src/optimize_op_gpu.cu:794-1098)
@@ -334,6 +337,43 @@ int bst_softmax_xent_grad(int dtype, int label_type, const void* logits, const v
  * launches nothing. Kernels: transpose_rows (D3 * element size >= 16 bytes), transpose_tile (narrower). */
 int bst_transpose_0213(int dtype, const void* x, void* y, long long D0, long long D1, long long D2, long long D3,
                        void* stream);
+
+/* ---- layer norm (the reference's norms module) ------------------------------------------------------------------ */
+
+/*
+ * y = relu?(xhat * g + b), xhat = (x - mean) * rstd, rstd = 1 / sqrt(var + epsilon), the statistics taken per row of
+ * K / segments features in fp32 (two passes over registers, or Welford / Chan merges in a fixed order; never
+ * E[x^2] - E[x]^2). Replaces LayerNormForward_NC, LayerNormSegmentedForward_NC and LayerNormForward_CN
+ * (src/layer_norm_nc_op_gpu.cu, src/layer_norm_cn_op_gpu.cu, launched from src/layer_norm_op.cc).
+ *   axis 1: x, y (N, K) of dtype, contiguous, features last; segment s of row n is x[n, s*L : (s+1)*L], L = K / segments,
+ *           with gain and bias g[s*L : (s+1)*L], b[...]; mean and rstd are fp32 [N][segments].
+ *   axis 0: x, y (K, N), N contiguous (BlocksparseMatMul(feature_axis=0) activations); segments must be 1; mean and
+ *           rstd are fp32 [N]; workspace is required (see bsmm_layer_norm_workspace_bytes).
+ *   g, b: K entries of gdtype (F32, F16 or BF16), read as fp32. relu != 0 applies max(., 0).
+ * Any alignment (16-byte accesses where every row start allows), 64-bit element offsets, no requirement on N.
+ * A bad dtype, axis other than 0 / 1, N < 0, K <= 0, K % segments, segments on axis 0, epsilon < 0 or a null pointer:
+ * BSMM_E_ARG before any launch. N = 0 launches nothing. The work partition depends on the shape only, so results are
+ * bitwise reproducible. Kernels: layer_norm_nc_warp (L <= 1024), layer_norm_nc_cta (<= 8192), layer_norm_nc_long;
+ * layer_norm_cn (a CTA per column strip) or layer_norm_cn_split (rows split across CTAs, when the strips are few).
+ */
+int bsmm_layer_norm(int dtype, int gdtype, int axis, const void* x, const void* g, const void* b, void* y, float* mean,
+                    float* rstd, void* workspace, long long N, int K, int segments, float epsilon, int relu, void* stream);
+
+/*
+ * dx (dtype), dg and db (K entries of gdtype) of bsmm_layer_norm, given dy and the forward's x, g, b, mean and rstd;
+ * xhat and, with relu, the pre-activation mask are recomputed. dx is written in the pass that reads dy and x, together
+ * with fp32 partial sums of dg and db in `workspace`, which a second kernel adds in a fixed order: deterministic, no
+ * atomics. Replaces LayerNormBackward_NC, LayerNormSegmentedBackward_NC and LayerNormBackward_CN (same files), which
+ * read dy and x again for dg / db and add with atomics. Shapes, errors and routes as bsmm_layer_norm (kernels
+ * layer_norm_grad_nc_warp / _cta / _long, layer_norm_grad_cn / _cn_split); workspace is required on both axes.
+ */
+int bsmm_layer_norm_grad(int dtype, int gdtype, int axis, const void* dy, const void* x, const void* g, const void* b,
+                         const float* mean, const float* rstd, void* dx, void* dg, void* db, void* workspace, long long N,
+                         int K, int segments, float epsilon, int relu, void* stream);
+
+/* Bytes of device workspace bsmm_layer_norm and bsmm_layer_norm_grad need for (axis, N, K, segments): the fp32 partial
+ * sums of the backward (and of the axis-0 forward's row splits). 0 for bad arguments or N = 0. */
+size_t bsmm_layer_norm_workspace_bytes(int axis, long long N, int K, int segments);
 
 /* ---- utilities on the (blocks, bsize, bsize) weight format -------------------------------------- */
 

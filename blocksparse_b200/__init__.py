@@ -4,10 +4,12 @@ Drop-in for the hot path of openai/blocksparse: `BlocksparseMatMul` (fprop / bpr
 updat, group_param_grads) and `BlocksparseTransformer` (NT / NN / TN + masked softmax),
 implemented as hand-written sm_90a CUDA behind the C ABI in include/bsmm_b200.h, plus the dense ops of the
 reference's transformer module (softmax, masked_softmax, masked_top_k_softmax, top_k, rectified_top_k,
-softmax_cross_entropy, transpose_0213, transpose_2d) and of its norms module (layer_norm).
+softmax_cross_entropy, transpose_0213, transpose_2d), of its norms module (layer_norm) and of its optimize module
+(AdamOptimizer, clip_by_global_norm, global_norm, Ema).
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
-from .optimize import blocksparse_l2_decay, blocksparse_norm, blocksparse_prune
+from .optimize import (AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay, blocksparse_norm, blocksparse_prune,
+                       clip_by_global_norm, global_norm)
 from .transformer import (BlocksparseTransformer, masked_softmax, masked_top_k_softmax, rectified_top_k, softmax,
                           softmax_cross_entropy, top_k, transpose_0213, transpose_2d)
 from .norms import layer_norm
@@ -18,4 +20,5 @@ __version__ = "0.1.0"
 __all__ = ["BlocksparseMatMul", "BlocksparseTransformer", "SparseProj", "group_param_grads", "blocksparse_reduced_dw",
            "block_reduced_full_dw", "blocksparse_norm", "blocksparse_prune", "blocksparse_l2_decay", "z_order_2d",
            "softmax", "masked_softmax", "masked_top_k_softmax", "top_k", "rectified_top_k", "softmax_cross_entropy",
-           "transpose_0213", "transpose_2d", "layer_norm"]
+           "transpose_0213", "transpose_2d", "layer_norm", "AdamOptimizer", "clip_by_global_norm", "global_norm",
+           "ClipGlobalNorm", "Ema"]

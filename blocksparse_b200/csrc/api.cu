@@ -6,6 +6,7 @@
 #include "dense_softmax.cuh"
 #include "generic.cuh"
 #include "layer_norm.cuh"
+#include "optimize.cuh"
 #include "softmax.cuh"
 #include "tc.cuh"
 #include "transpose.cuh"
@@ -778,5 +779,119 @@ int bsmm_unpad_blocks(int in_dtype, int out_dtype, int bsize, int blocks_small, 
     });
   });
   return check_launch("unpad_blocks");
+}
+
+// ---- optimizer (csrc/optimize.cuh) ----------------------------------------------------------------------------------------
+// Validates tensor i of a multi-tensor call: size >= 0, a known dtype, non-null pointers where the tensor has elements, and
+// for a gated tensor bs in {8, 16, 32, 64}, a gate and a size that is a multiple of bs*bs.
+static int mt_check(const char* what, int i, long long size, int dtype, const void* const* ptrs, int nptr, const float* gate,
+                    int bsize) {
+  if (size < 0) return fail(BSMM_E_ARG, "%s: tensor %d has negative size %lld", what, i, size);
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "%s: tensor %d has unsupported dtype code %d", what, i, dtype);
+  if (bsize != 0 && bsize != 8 && bsize != 16 && bsize != 32 && bsize != 64)
+    return fail(BSMM_E_ARG, "%s: tensor %d has block size %d (0, 8, 16, 32 or 64)", what, i, bsize);
+  if (bsize && size % ((long long)bsize * bsize))
+    return fail(BSMM_E_ARG, "%s: tensor %d of %lld elements is not made of %d x %d blocks", what, i, size, bsize, bsize);
+  if (mt_chunks(size) > 0x7fffffffLL) return fail(BSMM_E_LIMIT, "%s: tensor %d of %lld elements exceeds the grid", what, i, size);
+  if (size == 0) return 0;
+  for (int j = 0; j < nptr; ++j)
+    if (!ptrs[j]) return fail(BSMM_E_ARG, "%s: tensor %d has a null pointer", what, i);
+  if (bsize && !gate) return fail(BSMM_E_ARG, "%s: tensor %d is gated without a gate", what, i);
+  return 0;
+}
+
+static uint8_t mt_bshift(int bsize) { return bsize ? (uint8_t)(2 * (31 - __builtin_clz((unsigned)bsize))) : 0; }
+
+int bsmm_adam(int n, const void* const* grads, const int* grad_dtypes, float* const* params, void* const* means,
+              void* const* vars, const int* moment_codes, const long long* sizes, const float* const* gates,
+              const int* bsizes, const float* norm_scale, float lr, float decay_mean, float decay_var, float epsilon,
+              float grad_scale, float clip_sigma, float saturate, int zero_infs, int zero_nans, void* stream) {
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_adam: n = %d", n);
+  if (n && (!grads || !grad_dtypes || !params || !means || !vars || !moment_codes || !sizes))
+    return fail(BSMM_E_ARG, "bsmm_adam: null array");
+  for (int i = 0; i < n; ++i) {
+    const void* ptrs[4] = {grads[i], params[i], means[i], vars[i]};
+    const int bs = bsizes ? bsizes[i] : 0;
+    if (moment_codes[i] != 0 && moment_codes[i] != 1)
+      return fail(BSMM_E_ARG, "bsmm_adam: tensor %d has moment code %d (0 or 1)", i, moment_codes[i]);
+    if (int e = mt_check("bsmm_adam", i, sizes[i], grad_dtypes[i], ptrs, 4, bs && gates ? gates[i] : nullptr, bs)) return e;
+  }
+  AdamConsts k = {norm_scale, lr, decay_mean, decay_var, epsilon, grad_scale, clip_sigma, saturate, zero_infs, zero_nans};
+  return mt_for_launches(n, sizes,
+      [&](int i, MtTensor& t) {
+        t.a = grads[i]; t.b = params[i]; t.c = means[i]; t.d = vars[i];
+        const int bs = bsizes ? bsizes[i] : 0;
+        t.gate = bs ? gates[i] : nullptr; t.bshift = mt_bshift(bs);
+        t.dtype = (uint8_t)grad_dtypes[i]; t.codes = (uint8_t)moment_codes[i];
+        t.vec = aligned16(t.a) && aligned16(t.b) && aligned16(t.c) && aligned16(t.d);
+      },
+      [&](const MtTable& tab, int chunks, long long) {
+        mt_adam<<<chunks, MT_THREADS, 0, (cudaStream_t)stream>>>(tab, k);
+        return check_launch("mt_adam");
+      });
+}
+
+size_t bsmm_global_norm_workspace_bytes(int n, const long long* sizes) {
+  if (n < 0 || (n && !sizes)) return 0;
+  long long chunks = 0;
+  for (int i = 0; i < n; ++i) {
+    if (sizes[i] < 0) return 0;
+    chunks += mt_chunks(sizes[i]);
+  }
+  return (size_t)chunks * sizeof(float);
+}
+
+int bsmm_global_norm(int n, const void* const* xs, const int* dtypes, const long long* sizes, float grad_scale,
+                     float clip_norm, float saturate, int zero_infs, int zero_nans, float* norm, float* scale,
+                     void* workspace, void* stream) {
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_global_norm: n = %d", n);
+  if (n && (!xs || !dtypes || !sizes)) return fail(BSMM_E_ARG, "bsmm_global_norm: null array");
+  if (!norm || !scale) return fail(BSMM_E_ARG, "bsmm_global_norm: null output");
+  long long total = 0;
+  for (int i = 0; i < n; ++i) {
+    if (int e = mt_check("bsmm_global_norm", i, sizes[i], dtypes[i], &xs[i], 1, nullptr, 0)) return e;
+    total += mt_chunks(sizes[i]);
+  }
+  if (total == 0) return 0;                          // nothing launched: norm and scale are left to the caller (0 and 1)
+  if (total > 0x7fffffffLL) return fail(BSMM_E_LIMIT, "bsmm_global_norm: %lld chunks exceed the grid", total);
+  if (!workspace) return fail(BSMM_E_ARG, "bsmm_global_norm: null workspace");
+  float* partial = static_cast<float*>(workspace);
+  const NormConsts k = {grad_scale, saturate, zero_infs, zero_nans};
+  if (int e = mt_for_launches(n, sizes,
+          [&](int i, MtTensor& t) { t.a = xs[i]; t.dtype = (uint8_t)dtypes[i]; t.vec = aligned16(t.a); },
+          [&](const MtTable& tab, int chunks, long long base) {
+            mt_sumsq<<<chunks, MT_THREADS, 0, (cudaStream_t)stream>>>(tab, k, partial + base);
+            return check_launch("mt_sumsq");
+          }))
+    return e;
+  mt_norm_finish<<<1, MT_NORM_THREADS, 0, (cudaStream_t)stream>>>(partial, (int)total, clip_norm, norm, scale);
+  return check_launch("mt_norm_finish");
+}
+
+int bsmm_ema(int n, void* const* emas, int ema_dtype, const float* const* params, const long long* sizes,
+             const float* const* gates, const int* bsizes, float decay, void* stream) {
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_ema: n = %d", n);
+  if (ema_dtype != BSMM_F32 && ema_dtype != BSMM_F16) return fail(BSMM_E_ARG, "bsmm_ema: ema dtype %d (F32 or F16)", ema_dtype);
+  if (n && (!emas || !params || !sizes)) return fail(BSMM_E_ARG, "bsmm_ema: null array");
+  for (int i = 0; i < n; ++i) {
+    const void* ptrs[2] = {emas[i], params[i]};
+    const int bs = bsizes ? bsizes[i] : 0;
+    if (int e = mt_check("bsmm_ema", i, sizes[i], ema_dtype, ptrs, 2, bs && gates ? gates[i] : nullptr, bs)) return e;
+  }
+  return mt_for_launches(n, sizes,
+      [&](int i, MtTensor& t) {
+        t.a = params[i]; t.b = emas[i];
+        const int bs = bsizes ? bsizes[i] : 0;
+        t.gate = bs ? gates[i] : nullptr; t.bshift = mt_bshift(bs);
+        t.dtype = (uint8_t)ema_dtype; t.vec = aligned16(t.a) && aligned16(t.b);
+      },
+      [&](const MtTable& tab, int chunks, long long) {
+        if (ema_dtype == BSMM_F32) {
+          mt_ema<float><<<chunks, MT_THREADS, 0, (cudaStream_t)stream>>>(tab, decay);
+          return check_launch("mt_ema");
+        }
+        mt_ema<__half><<<chunks, MT_THREADS, 0, (cudaStream_t)stream>>>(tab, decay);
+        return check_launch("mt_ema_f16");
+      });
 }
 }  // extern "C"

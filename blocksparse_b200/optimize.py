@@ -1,10 +1,14 @@
-"""Block-sparse weight utilities of the reference's blocksparse/optimize.py (tail, :294-335) on torch tensors.
+"""The reference's blocksparse/optimize.py on torch tensors.
+
+  AdamOptimizer(params, learning_rate, beta1, beta2, ...)   torch optimizer; gated and 16-bit-moment Adam (:20-110)
+  clip_by_global_norm(grads, clip_norm, ...) / global_norm / ClipGlobalNorm   device norm and clip scale (:197-225)
+  Ema(decay, gated, fp16)                                   parameter moving averages (:231-289)
 
   blocksparse_norm(param, norm="max")                       per-block max|w| or l2 norm -> float32 [blocks]
   blocksparse_l2_decay(param, gate=None, rate, epsilon)     in place: w -= w * min(rate / sqrt(sum w^2 + eps), 1)
   blocksparse_prune(param, gate, step, sparsity= | threshold=, norm, frequency)
                                                             in place on `gate`; top-k by block norm or threshold
-All run as hand-written CUDA kernels (csrc/wutil.cuh) through the C ABI; there is no CPU path.
+All run as hand-written CUDA kernels (csrc/optimize.cuh, csrc/wutil.cuh) through the C ABI; there is no CPU path.
 """
 import numpy as np
 import torch
@@ -65,3 +69,237 @@ def blocksparse_prune(param, gate, step, sparsity=None, threshold=None, norm="ma
                                           float(threshold), 1 if norm.lower() == "l2" else 0, _lib.stream_ptr())
             _lib.check(rc, "bsmm_threshold_prune")
     return gate
+
+
+# ---- AdamOptimizer, clip_by_global_norm and Ema (reference optimize.py:20-110, 197-289) ---------------------------------
+# Each op is one multi-tensor call of csrc/optimize.cuh: a fixed number of kernel launches per step whatever the number of
+# tensors (one per 256), no host synchronisation and no host-to-device copy.
+
+_MIN_CODED = 8 * 1024            # params with at least this many elements keep 16-bit moments under fp16=True (optimize.py:70)
+
+
+def _ptrs(ts):
+    return np.array([t.data_ptr() for t in ts], dtype=np.uint64)
+
+
+def _i32(xs):
+    return np.array(xs, dtype=np.int32)
+
+
+def _i64(xs):
+    return np.array(xs, dtype=np.int64)
+
+
+def _dev_scalar(t, what):
+    if not torch.is_tensor(t) or not t.is_cuda or t.dtype != torch.float32 or t.numel() != 1:
+        raise ValueError("%s must be a one-element float32 CUDA tensor" % what)
+    return t
+
+
+def _gate_of(p, gated):
+    """(gate, bsize) of a gated param, (None, 0) otherwise."""
+    gate = getattr(p, "gate", None) if gated else None
+    if gate is None:
+        return None, 0
+    if p.dim() != 3 or p.shape[1] != p.shape[2] or p.shape[1] not in (8, 16, 32, 64):
+        raise ValueError("a gated param must be (blocks, bsize, bsize) with bsize in {8,16,32,64}, got %s" % (tuple(p.shape),))
+    if (not torch.is_tensor(gate) or gate.dtype != torch.float32 or gate.numel() != p.shape[0] or gate.device != p.device
+            or not gate.is_contiguous()):
+        raise ValueError("param.gate must be a contiguous float32 tensor with one entry per block, on the param's device")
+    return gate, p.shape[1]
+
+
+def _check_qspec(**qspecs):
+    for k, v in qspecs.items():
+        if v is not None:
+            raise ValueError("%s: the quantize module is not carried here; only None is accepted" % k)
+
+
+class AdamOptimizer(torch.optim.Optimizer):
+    """The reference's AdamOptimizer (optimize.py:20-110) as a torch optimizer, stepping every param in one kernel launch
+    (per 256 params) of csrc/optimize.cuh.
+
+    params: fp32 CUDA tensors. param_groups[i]["lr"] is the learning rate, so torch LR schedulers apply. The host forms
+    lr_t = lr * sqrt(1 - beta2_power) / (1 - beta1_power) in fp32; the powers start at beta1 / beta2 (0 with
+    zero_init_variables) and are multiplied by the betas after every step. They live in each param group, so they travel
+    with state_dict(). They advance even on a step that norm_scale turns into a no-op: the host cannot know.
+
+    gated=True: a param with a `.gate` attribute (fp32 [blocks]) is stepped block by block; blocks whose gate is 0 keep
+    the param and both moments bit for bit. fp16=True: params of at least 8192 elements keep their mean and variance as
+    int16 tensors of the reference's 16-bit codes (8 bytes of state per parameter instead of 12).
+    norm_scale: a one-element fp32 CUDA tensor (e.g. from clip_by_global_norm) read on the device at every step; 0 makes
+    the step a no-op. The *_qspec arguments of the reference's quantize module must be None."""
+
+    def __init__(self, params, learning_rate=3e-4, beta1=0.9, beta2=0.999, epsilon=1e-8, clip_sigmas=0.0,
+                 norm_scale=None, grad_scale=1.0, saturate=0.0, zero_infs=False, zero_nans=False, gated=False,
+                 param_qspec=None, mean_qspec=None, var_qspec=None, fp16=False, zero_init_variables=False, name="Adam"):
+        _check_qspec(param_qspec=param_qspec, mean_qspec=mean_qspec, var_qspec=var_qspec)
+        if norm_scale is not None:
+            _dev_scalar(norm_scale, "norm_scale")
+        b1, b2 = (0.0, 0.0) if zero_init_variables else (float(np.float32(beta1)), float(np.float32(beta2)))
+        super().__init__(params, dict(lr=learning_rate, beta1_power=b1, beta2_power=b2))
+        self.beta1, self.beta2, self.epsilon, self.clip_sigmas = beta1, beta2, epsilon, clip_sigmas
+        self.norm_scale, self.grad_scale, self.saturate = norm_scale, grad_scale, saturate
+        self.zero_infs, self.zero_nans, self.gated, self.fp16, self.name = zero_infs, zero_nans, gated, fp16, name
+        for group in self.param_groups:
+            for p in group["params"]:
+                if not p.is_cuda or p.dtype != torch.float32:
+                    raise ValueError("AdamOptimizer: params must be float32 CUDA tensors, got %s on %s" % (p.dtype, p.device))
+
+    def _moments(self, p):
+        st = self.state[p]
+        if "mean" not in st:
+            dtype = torch.int16 if self.fp16 and p.numel() >= _MIN_CODED else torch.float32
+            st["mean"] = torch.zeros(p.shape, dtype=dtype, device=p.device)
+            st["var"] = torch.zeros(p.shape, dtype=dtype, device=p.device)
+        return st["mean"], st["var"]
+
+    def load_state_dict(self, state_dict):
+        """torch's loader casts every state tensor of a float param to the param's dtype; 16-bit moment codes are
+        restored as the int16 tensors they are."""
+        coded = {i: {k: v for k, v in st.items() if torch.is_tensor(v) and v.dtype == torch.int16}
+                 for i, st in state_dict["state"].items()}
+        super().load_state_dict(state_dict)
+        every = [p for group in self.param_groups for p in group["params"]]
+        for i, st in coded.items():
+            for k, v in st.items():
+                self.state[every[i]][k] = v.to(device=every[i].device, copy=True)
+
+    @torch.no_grad()
+    def step(self, closure=None, norm_scale=None, grads=None):
+        """One Adam step over every param that has a gradient: `grads[i]` (fp32, fp16 or bf16, aligned with the params
+        of all groups in order) when given, else param.grad. norm_scale overrides the constructor's."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        ns = self.norm_scale if norm_scale is None else _dev_scalar(norm_scale, "norm_scale")
+        every = [p for group in self.param_groups for p in group["params"]]
+        if grads is not None and len(grads) != len(every):
+            raise ValueError("AdamOptimizer.step: %d grads for %d params" % (len(grads), len(every)))
+        k = 0
+        lib = _lib.load()
+        f32 = np.float32
+        for group in self.param_groups:
+            gs, ps, ms, vs, gd, codes, sizes, gates, bss = [], [], [], [], [], [], [], [], []
+            for p in group["params"]:
+                g = grads[k] if grads is not None else p.grad
+                k += 1
+                if g is None:
+                    continue
+                if g.shape != p.shape or g.device != p.device:
+                    raise ValueError("AdamOptimizer.step: grad %s on %s for param %s on %s"
+                                     % (tuple(g.shape), g.device, tuple(p.shape), p.device))
+                if not p.is_contiguous():
+                    raise ValueError("AdamOptimizer.step: params must be contiguous")
+                if p.numel() == 0:
+                    continue
+                gd.append(_lib.dtype_code(g.dtype))
+                gate, bs = _gate_of(p, self.gated)
+                m, v = self._moments(p)
+                gs.append(g.contiguous())
+                ps.append(p)
+                ms.append(m)
+                vs.append(v)
+                codes.append(1 if m.dtype == torch.int16 else 0)
+                sizes.append(p.numel())
+                gates.append(gate.data_ptr() if gate is not None else 0)
+                bss.append(bs)
+            b1p, b2p = f32(group["beta1_power"]), f32(group["beta2_power"])
+            lr_t = f32(group["lr"]) * np.sqrt(f32(1) - b2p) / (f32(1) - b1p)           # optimize.py:57
+            if ps:
+                arrs = (_ptrs(gs), _i32(gd), _ptrs(ps), _ptrs(ms), _ptrs(vs), _i32(codes), _i64(sizes),
+                        np.array(gates, dtype=np.uint64), _i32(bss))
+                with torch.cuda.device(ps[0].device):
+                    rc = lib.bsmm_adam(len(ps), *[a.ctypes.data for a in arrs], _lib.ptr(ns), float(lr_t),
+                                       float(self.beta1), float(self.beta2), float(self.epsilon), float(self.grad_scale),
+                                       float(self.clip_sigmas), float(self.saturate), int(self.zero_infs),
+                                       int(self.zero_nans), _lib.stream_ptr())
+                _lib.check(rc, "bsmm_adam")
+            group["beta1_power"] = float(b1p * f32(self.beta1))                        # optimize.py:104-110
+            group["beta2_power"] = float(b2p * f32(self.beta2))
+        return loss
+
+
+def clip_by_global_norm(grads, clip_norm=1.0, grad_scale=1.0, saturate=0.0, zero_infs=False, zero_nans=False):
+    """(global_norm, norm_scale) as 0-dim fp32 CUDA tensors (reference optimize.py:197-225): global_norm =
+    sqrt(sum of (grad_scale * sat(filter(x)))^2) over every element of every grad; norm_scale = clip_norm /
+    max(global_norm, clip_norm), or 0 when the norm is not finite. grads may mix fp32, fp16 and bf16 and include empty
+    tensors. Two launches (one more per 256 tensors), no host synchronisation, bitwise reproducible."""
+    grads = list(grads)
+    for g in grads:
+        if not torch.is_tensor(g) or g.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+            raise ValueError("clip_by_global_norm: unsupported grad dtype %s" % (getattr(g, "dtype", type(g)),))
+        if not g.is_cuda:
+            raise ValueError("clip_by_global_norm: grads must be CUDA tensors (there is no CPU path)")
+    device = grads[0].device if grads else torch.device("cuda", torch.cuda.current_device())
+    live = [g.contiguous() for g in grads if g.numel()]
+    if not live:
+        return torch.zeros((), dtype=torch.float32, device=device), torch.ones((), dtype=torch.float32, device=device)
+    norm = torch.empty((), dtype=torch.float32, device=device)
+    scale = torch.empty((), dtype=torch.float32, device=device)
+    lib = _lib.load()
+    sizes = _i64([g.numel() for g in live])
+    ws = torch.empty(lib.bsmm_global_norm_workspace_bytes(len(live), sizes.ctypes.data) // 4, dtype=torch.float32,
+                     device=device)
+    xs, dts = _ptrs(live), _i32([_lib.dtype_code(g.dtype) for g in live])
+    with torch.cuda.device(device):
+        rc = lib.bsmm_global_norm(len(live), xs.ctypes.data, dts.ctypes.data, sizes.ctypes.data, float(grad_scale),
+                                  float(clip_norm), float(saturate), int(zero_infs), int(zero_nans), norm.data_ptr(),
+                                  scale.data_ptr(), ws.data_ptr(), _lib.stream_ptr())
+    _lib.check(rc, "bsmm_global_norm")
+    return norm, scale
+
+
+def global_norm(grads, grad_scale=1.0, saturate=0.0, zero_infs=False, zero_nans=False):
+    gn, _ = clip_by_global_norm(grads, clip_norm=9e9, grad_scale=grad_scale, saturate=saturate, zero_infs=zero_infs,
+                                zero_nans=zero_nans)
+    return gn
+
+
+def ClipGlobalNorm(grads, clip_norm=1.0, grad_scale=1.0, saturate=0.0, zero_infs=False, zero_nans=False):
+    """Old name of clip_by_global_norm."""
+    return clip_by_global_norm(grads, clip_norm=clip_norm, grad_scale=grad_scale, saturate=saturate,
+                               zero_infs=zero_infs, zero_nans=zero_nans)
+
+
+class Ema(object):
+    """Exponential moving averages of params (reference optimize.py:231-289): apply(params) creates each average on first
+    use as a copy of the param (float16 when fp16), then does ema -= (1 - decay) * (ema - param) for all of them in one
+    launch (per 256). Gated, blocks of a param with a `.gate` whose gate is 0 keep their average."""
+
+    def __init__(self, decay=0.999, gated=False, fp16=False, name="Ema"):
+        self.decay, self.gated, self.fp16, self.name = decay, gated, fp16, name
+        self.averages = dict()           # id(param) -> (param, average)
+
+    @torch.no_grad()
+    def apply(self, params, qspec=None):
+        _check_qspec(qspec=qspec)
+        params = list(params)
+        emas, ps, sizes, gates, bss = [], [], [], [], []
+        for p in params:
+            if not torch.is_tensor(p) or not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous():
+                raise ValueError("Ema.apply: params must be contiguous float32 CUDA tensors")
+            entry = self.averages.get(id(p))
+            if entry is None or entry[0] is not p:
+                entry = self.averages[id(p)] = (p, p.detach().to(torch.float16 if self.fp16 else torch.float32, copy=True))
+            if p.numel() == 0:
+                continue
+            gate, bs = _gate_of(p, self.gated)
+            emas.append(entry[1])
+            ps.append(p)
+            sizes.append(p.numel())
+            gates.append(gate.data_ptr() if gate is not None else 0)
+            bss.append(bs)
+        if not ps:
+            return
+        arrs = (_ptrs(emas), _ptrs(ps), _i64(sizes), np.array(gates, dtype=np.uint64), _i32(bss))
+        with torch.cuda.device(ps[0].device):
+            rc = _lib.load().bsmm_ema(len(ps), arrs[0].ctypes.data, _lib.F16 if self.fp16 else _lib.F32, arrs[1].ctypes.data,
+                                      arrs[2].ctypes.data, arrs[3].ctypes.data, arrs[4].ctypes.data, float(self.decay),
+                                      _lib.stream_ptr())
+        _lib.check(rc, "bsmm_ema")
+
+    def average(self, param):
+        entry = self.averages.get(id(param))
+        return entry[1] if entry is not None and entry[0] is param else None

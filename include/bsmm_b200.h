@@ -36,6 +36,10 @@
  *   bsmm_reduced_dw       <- BlocksparseReducedDWOp: BlocksparseFeatureReduce{CN,NC} + hGemm{NT,TN}
  *                            (src/blocksparse_matmul_op.cc:639-773)
  *   bsmm_gather_rows      <- GatherScatter / ScatterAddMul ops behind SparseProj (blocksparse/matmul.py:835-921)
+ *   bsmm_adam             <- AdamOp: ApplyAdam / ApplyAdamGated, one launch per tensor (src/optimize_op.cc:355-433)
+ *   bsmm_global_norm      <- ClipGlobalNormOp: ReduceSumSquared per tensor + ComputeClipNorm
+ *                            (src/optimize_op.cc:771-858, src/optimize_op_gpu.cu:1102-1238)
+ *   bsmm_ema              <- EmaOp: ApplyEma / ApplyEmaGated (src/optimize_op.cc:463-529)
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer except `err` strings is DEVICE memory
@@ -417,6 +421,52 @@ int bsmm_gather_rows(int dtype, const void* x, const void* y, const int32_t* idx
 int bsmm_pad_blocks(int dtype, int bsize, int blocks_big, const int32_t* sub_map, const void* w_small, const float* gate, void* w_big, void* stream);
 int bsmm_unpad_blocks(int in_dtype, int out_dtype, int bsize, int blocks_small, const int32_t* inv_map, const void* dw_big, const float* gate,
                       void* dw_small, int accumulate, void* stream);
+
+/* ---- optimizer (the reference's optimize module) ------------------------------------------------------------------ */
+
+/*
+ * Multi-tensor entries: tensor i of n is described by entry i of each host array, which is read before the call returns.
+ * Up to 256 non-empty tensors go into one kernel launch (their table travels in the kernel parameters); more tensors take
+ * one more launch per 256. Element offsets are 64-bit; vector accesses of 4 elements (16 bytes of fp32, 8 of 16-bit
+ * data, warp-contiguous) are used on a tensor whose pointers all allow them, scalar ones otherwise. A gated tensor (bsizes[i] in {8, 16, 32, 64}, gates[i] fp32 [size / bs^2]) is handled in the same launch, block
+ * = element / (bs*bs); blocks whose gate is 0 are neither read nor written. bsizes and gates may be NULL (no gates).
+ * n < 0, a bad dtype or moment code, a negative size, a null pointer of a non-empty tensor, bs outside {0, 8, 16, 32, 64}
+ * or a gated size that is not a multiple of bs*bs: BSMM_E_ARG before any launch. Empty tensors are skipped (their
+ * pointers are not read); with nothing left, nothing is launched.
+ */
+
+/*
+ * One Adam step in place, per element (optimize_op_gpu.cu:454-502): g = grad (fp32, fp16 or bf16 by grad_dtypes[i]);
+ * zero_infs, zero_nans, then clamp to +-saturate when saturate != 0; g *= grad_scale * norm_scale;
+ * v = decay_var v + (1 - decay_var) g^2; clamp g to +-clip_sigma sqrt(v) when clip_sigma != 0;
+ * m = decay_mean m + (1 - decay_mean) g; p -= lr m / (sqrt(v) + epsilon).
+ * params are fp32. moment_codes[i] = 0: means / vars fp32; 1: the reference's 16-bit codes (ew_op_gpu.h:332-431),
+ * decoded to fp32, updated and encoded again (see DESIGN.md 7e). norm_scale is a device fp32 scalar read by the kernel
+ * (NULL = 1); when it is 0 the kernel returns without touching anything. lr is the bias-corrected rate the host forms.
+ * Unlike AdamOp, a gated tensor takes exactly one step on its live blocks and none on its pruned ones. Kernel: mt_adam.
+ */
+int bsmm_adam(int n, const void* const* grads, const int* grad_dtypes, float* const* params, void* const* means,
+              void* const* vars, const int* moment_codes, const long long* sizes, const float* const* gates,
+              const int* bsizes, const float* norm_scale, float lr, float decay_mean, float decay_var, float epsilon,
+              float grad_scale, float clip_sigma, float saturate, int zero_infs, int zero_nans, void* stream);
+
+/*
+ * norm = sqrt(sum over every element of every x_i of (grad_scale * sat(filter(x)))^2), with the filters of bsmm_adam;
+ * scale = clip_norm / max(norm, clip_norm) when norm is finite, else 0. norm and scale are device fp32 scalars.
+ * Kernel mt_sumsq writes one fp32 sum of squares per chunk of 8192 elements into workspace (at least
+ * bsmm_global_norm_workspace_bytes(n, sizes) bytes), and mt_norm_finish adds them in fp64 in chunk order: the partition
+ * depends on the sizes only and there are no atomics, so the result is bitwise reproducible. With no element at all
+ * nothing is launched and norm / scale are not written: the caller sets them to 0 and 1.
+ */
+int bsmm_global_norm(int n, const void* const* xs, const int* dtypes, const long long* sizes, float grad_scale,
+                     float clip_norm, float saturate, int zero_infs, int zero_nans, float* norm, float* scale,
+                     void* workspace, void* stream);
+size_t bsmm_global_norm_workspace_bytes(int n, const long long* sizes);
+
+/* ema -= (1 - decay) * (ema - param) in place; emas of ema_dtype (BSMM_F32 or BSMM_F16), params fp32. Kernels
+ * mt_ema (fp32) and mt_ema_f16. */
+int bsmm_ema(int n, void* const* emas, int ema_dtype, const float* const* params, const long long* sizes,
+             const float* const* gates, const int* bsizes, float decay, void* stream);
 
 /* ---- measurement helper (the reference's `bench` op attribute, op.cc:99-106) ---------
  * Records two events around whatever the caller enqueues between begin and end.      */

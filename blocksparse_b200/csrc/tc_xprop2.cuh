@@ -23,7 +23,7 @@ template <int TB, int MI> struct Xp2Shape {
   static constexpr uint32_t STAGE = (XBYTES + TB * WBYTES + 1023) / 1024 * 1024;
   static constexpr size_t SMEM = XP_STAGES * STAGE + SMEM_ALIGN_SLACK;
 };
-constexpr int XP2_REC = 8;           // ints per merged entry: (input block, W block of output 0..3 or -1, pad)
+constexpr int XP2_REC = 16;          // ints per merged entry: (input block, W block of output 0..7 or -1, pad)
 
 struct Xprop2Params {
   const int32_t* tile_off;   // [n_tiles + 1] first merged entry of every tile
@@ -147,12 +147,181 @@ int dispatch_tc_xprop2(const Xprop2Params& p, const XpropTmaps& maps, int n_tile
   return bprop ? launch_tc_xprop2<TB, MI, BF16, false, true>(p, maps, n_tiles, s) : launch_tc_xprop2<TB, MI, BF16, false, false>(p, maps, n_tiles, s);
 }
 
+// ---- grouped tiles: the default for 32 x 32 blocks when lut.py:pick_xprop_tile selects them ---------------------------
+// A CTA owns 128 minibatch rows x G consecutive output blocks and walks the same merged entries, but only the W blocks
+// that exist are fetched (block j of the tile always lands in slot j of the stage; the slot of an absent block keeps
+// stale bytes that nothing reads) and only they are multiplied: one m64n32k16 MMA per K = 16 step into the 16
+// accumulator registers of block j.  Every output element therefore sees exactly the MMAs of tc_xprop_kernel in the same
+// (ascending input block) order, so results are bit-identical to it and an output depends on no block its LUT row does
+// not list.  One warpgroup owns both 64-row halves: 32 G accumulator registers per thread, three CTAs per SM at G = 4.
+template <int G> struct XpgShape {
+  static constexpr uint32_t XBYTES = 128 * 32 * 2;
+  static constexpr uint32_t WBYTES = 32 * 32 * 2;
+  static constexpr uint32_t STAGE = XBYTES + G * WBYTES;
+  static constexpr size_t SMEM = XP_STAGES * STAGE + SMEM_ALIGN_SLACK;
+};
+
+// Merged entries whose records a CTA keeps in shared memory at a time.  The loop below is lock-step (wait, multiply,
+// CTA barrier, refill), so a record read from global memory by the refilling thread would put an L2 round trip into
+// every iteration; the records of up to XPG_LUT entries are copied to shared memory first, and a longer tile drains
+// its pipeline once per XPG_LUT entries to load the next ones.
+constexpr int XPG_LUT = 128;
+
+template <int G, bool BF16, bool AXIS0, bool BPROP>
+__global__ void __launch_bounds__(XP_THREADS)
+tc_xprop_grouped_kernel(const Xprop2Params p, const __grid_constant__ XpropTmaps maps, const int n_tiles) {
+  using Sh = XpgShape<G>;
+  constexpr int ST = XP_STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ uint64_t full[ST];
+  const uint32_t base = aligned_smem_base(smem_raw);
+  const int tid = threadIdx.x, warp = tid / 32, lane = tid % 32;
+  // the output tiles of one minibatch tile are neighbours in the grid, so CTAs that run together share activation tiles
+  // in L2 (with the minibatch tile running fastest an activation tensor larger than L2 is streamed once per output tile)
+  const int nt = blockIdx.x / n_tiles, t = blockIdx.x % n_tiles;
+  const int first = p.tile_off[t], count = p.tile_off[t + 1] - first;
+  const int32_t* ent = p.ent + (size_t)first * XP2_REC;
+  // per entry of the current chunk: input block, W block of output 0..G-1 (or -1), mask of the blocks that exist
+  __shared__ int32_t rec[XPG_LUT][G + 2];
+
+  auto issue = [&](int c0, int e) {                        // one thread: stage merged entry c0 + e (e: index in the chunk)
+    const int32_t* r = rec[e];
+    const int g = c0 + e;
+    const uint32_t st = base + (uint32_t)(g % ST) * Sh::STAGE;
+    uint64_t* bar = &full[g % ST];
+    const uint32_t mask = (uint32_t)r[G + 1];
+    ptx::mbar_expect_tx(bar, Sh::XBYTES + (uint32_t)__popc(mask) * Sh::WBYTES);
+    const int c = r[0];
+    if (!AXIS0) {
+      ptx::tma_load_2d(st, &maps.x, bar, c * 32, nt * 128);                              // [128 n][32 c]
+    } else {                                                                             // [32 c][128 n] as two 64-column boxes
+      ptx::tma_load_2d(st, &maps.x, bar, nt * 128, c * 32);
+      ptx::tma_load_2d(st + Sh::XBYTES / 2, &maps.x, bar, nt * 128 + 64, c * 32);
+    }
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+      if (mask >> j & 1) ptx::tma_load_2d(st + Sh::XBYTES + j * Sh::WBYTES, &maps.w, bar, 0, r[1 + j] * 32);
+  };
+
+  if (tid == 0) {
+    for (int i = 0; i < ST; ++i) ptx::mbar_init(&full[i], 1);
+    ptx::fence_mbar_init();
+    ptx::prefetch_tensormap(&maps.x); ptx::prefetch_tensormap(&maps.w);
+  }
+
+  float acc[2][G][16];
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+#pragma unroll
+      for (int i = 0; i < 16; ++i) acc[m][j][i] = 0.f;
+
+  for (int c0 = 0; c0 < count; c0 += XPG_LUT) {
+    const int n = min(count - c0, XPG_LUT);
+    __syncthreads();                                         // barriers initialized; the previous chunk is consumed and its records are free
+    for (int i = tid; i < n; i += XP_THREADS) {
+      const int32_t* r = ent + (size_t)(c0 + i) * XP2_REC;
+      int32_t mask = 0;
+      rec[i][0] = __ldg(r);
+#pragma unroll
+      for (int j = 0; j < G; ++j) {
+        const int32_t wb = __ldg(r + 1 + j);
+        rec[i][1 + j] = wb;
+        mask |= (int32_t)(wb >= 0) << j;
+      }
+      rec[i][G + 1] = mask;
+    }
+    __syncthreads();
+    if (tid == 0)
+      for (int e = 0; e < n && e < ST; ++e) issue(c0, e);
+    for (int e = 0; e < n; ++e) {
+      const int g = c0 + e;
+      const uint32_t st = base + (uint32_t)(g % ST) * Sh::STAGE;
+      const uint32_t mask = (uint32_t)rec[e][G + 1];         // uniform over the CTA
+      if (!ptx::mbar_wait(&full[g % ST], (uint32_t)(g / ST) & 1)) g_tc_error = 45;
+      ptx::wg_fence();
+#pragma unroll
+      for (int j = 0; j < G; ++j) {
+        if (mask >> j & 1) {
+#pragma unroll
+          for (int ks = 0; ks < 2; ++ks) {                   // descriptors as tc_xprop_kernel<32>: fprop reads W MN-major, bprop K-major
+            const uint32_t wb = st + Sh::XBYTES + j * Sh::WBYTES;
+            const uint64_t bdesc = BPROP ? ptx::make_desc(wb + ks * 32, 16, 512, ptx::SWZ_64B)
+                                         : ptx::make_desc(wb + ks * 1024, Sh::WBYTES, 512, ptx::SWZ_64B);
+#pragma unroll
+            for (int m = 0; m < 2; ++m) {
+              const uint64_t adesc = AXIS0 ? ptx::make_desc(st + m * (Sh::XBYTES / 2) + ks * 2048, Sh::XBYTES / 2, 1024, ptx::SWZ_128B)
+                                           : ptx::make_desc(st + m * 64 * 64 + ks * 32, 16, 512, ptx::SWZ_64B);
+              ptx::wgmma<BF16, AXIS0 ? 1 : 0, BPROP ? 0 : 1, 32>(acc[m][j], adesc, bdesc);
+            }
+          }
+        }
+      }
+      ptx::wg_commit();
+      ptx::wg_wait<1>();                                     // entry e-1 has been consumed by the whole warpgroup ...
+      __syncthreads();
+      if (tid == 0 && e >= 1 && e - 1 + ST < n) issue(c0, e - 1 + ST);   // ... so its buffer can be refilled
+    }
+    ptx::wg_wait<0>();
+  }
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int j = 0; j < G; ++j) ptx::wg_fence_regs(acc[m][j]);
+
+  // epilogue (output blocks with no entry are written as zeros)
+  uint16_t* y = reinterpret_cast<uint16_t*>(p.y);
+#pragma unroll
+  for (int m = 0; m < 2; ++m)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long long n = (long long)nt * 128 + m * 64 + warp * 16 + lane / 4 + 8 * h;
+      if (n >= p.N) continue;
+#pragma unroll
+      for (int j = 0; j < G; ++j) {
+        const int o = t * G + j;
+        if (o >= p.n_out) continue;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int col = o * 32 + 8 * q + 2 * (lane % 4);
+          const float a = acc[m][j][4 * q + 2 * h], b = acc[m][j][4 * q + 2 * h + 1];
+          if (!AXIS0) {
+            *reinterpret_cast<uint32_t*>(y + n * p.y_pitch + col) = pack2<BF16>(a, b);
+          } else {
+            y[(long long)col * p.y_pitch + n] = pack1<BF16>(a);
+            y[(long long)(col + 1) * p.y_pitch + n] = pack1<BF16>(b);
+          }
+        }
+      }
+    }
+}
+
+template <int G, bool BF16, bool AXIS0, bool BPROP>
+int launch_tc_xprop_grouped(const Xprop2Params& p, const XpropTmaps& maps, int n_tiles, cudaStream_t s) {
+  auto kern = tc_xprop_grouped_kernel<G, BF16, AXIS0, BPROP>;
+  constexpr size_t smem = XpgShape<G>::SMEM;
+  static thread_local uint64_t configured = 0;
+  if (int e = ensure_dyn_smem(kern, smem, configured)) return e;
+  const long long ctas = (long long)((p.N + 127) / 128) * n_tiles;
+  if (ctas > 0x7fffffffLL) return fail(BSMM_E_LIMIT, "bsmm_xprop: %lld CTAs exceed the grid limit", ctas);
+  kern<<<dim3((unsigned)ctas), XP_THREADS, smem, s>>>(p, maps, n_tiles);
+  return check_launch("wgmma_xprop_bs32");                 // the default 32 x 32 route keeps one name whatever tile it runs
+}
+
+template <int G, bool BF16>
+int dispatch_tc_xprop_grouped(const Xprop2Params& p, const XpropTmaps& maps, int n_tiles, bool axis0, bool bprop, cudaStream_t s) {
+  if (axis0) return bprop ? launch_tc_xprop_grouped<G, BF16, true, true>(p, maps, n_tiles, s) : launch_tc_xprop_grouped<G, BF16, true, false>(p, maps, n_tiles, s);
+  return bprop ? launch_tc_xprop_grouped<G, BF16, false, true>(p, maps, n_tiles, s) : launch_tc_xprop_grouped<G, BF16, false, false>(p, maps, n_tiles, s);
+}
+
+// variant 4: the grouped kernel with G = 4 output blocks per CTA.
 // sched: lut.py:build_wide_schedule in device memory: tile offsets at int32 index 2, merged entries at ent_off.
 inline int tc_xprop2(int dtype, int axis, int bprop, int n_out, int n_in, int blocks, const void* x, const void* w, void* y,
                      int N, const int32_t* sched, int n_tiles, int variant, int ent_off, cudaStream_t s) {
   if (dtype != BSMM_F16 && dtype != BSMM_BF16) return fail(BSMM_E_ARG, "bsmm_xprop: the wide-tile schedule needs a 16-bit dtype");
-  if (variant < 1 || variant > 3) return fail(BSMM_E_ARG, "bsmm_xprop: wide-tile variant %d (1..3)", variant);
-  const int tb = variant == 3 ? 4 : 2;
+  if (variant < 1 || variant > 4) return fail(BSMM_E_ARG, "bsmm_xprop: wide-tile variant %d (1..4)", variant);
+  const int tb = variant >= 3 ? 4 : 2;
   if (sched == nullptr || n_tiles <= 0 || (long long)n_tiles * tb < n_out || ent_off < n_tiles + 3)
     return fail(BSMM_E_ARG, "bsmm_xprop: inconsistent wide-tile schedule (tiles=%d variant=%d entries at %d)", n_tiles, variant, ent_off);
   if (axis == 0 && (N & 7)) { fail(0, "feature_axis 0 needs N %% 8 == 0 for TMA (row pitch multiple of 16 bytes)"); return TC_NOT_APPLICABLE; }
@@ -175,7 +344,8 @@ inline int tc_xprop2(int dtype, int axis, int bprop, int n_out, int n_in, int bl
   switch (variant) {
     case 1: return bf ? dispatch_tc_xprop2<2, 1, true>(p, maps, n_tiles, a0, bp, s) : dispatch_tc_xprop2<2, 1, false>(p, maps, n_tiles, a0, bp, s);
     case 2: return bf ? dispatch_tc_xprop2<2, 2, true>(p, maps, n_tiles, a0, bp, s) : dispatch_tc_xprop2<2, 2, false>(p, maps, n_tiles, a0, bp, s);
-    default: return bf ? dispatch_tc_xprop2<4, 2, true>(p, maps, n_tiles, a0, bp, s) : dispatch_tc_xprop2<4, 2, false>(p, maps, n_tiles, a0, bp, s);
+    case 3: return bf ? dispatch_tc_xprop2<4, 2, true>(p, maps, n_tiles, a0, bp, s) : dispatch_tc_xprop2<4, 2, false>(p, maps, n_tiles, a0, bp, s);
+    default: return bf ? dispatch_tc_xprop_grouped<4, true>(p, maps, n_tiles, a0, bp, s) : dispatch_tc_xprop_grouped<4, false>(p, maps, n_tiles, a0, bp, s);
   }
 }
 

@@ -187,13 +187,13 @@ class MatmulLuts(object):
         return build_tile_schedule(outs, ins, wids, n_out, blocks_per_tile, bsize, w_per_group, n_tiles, n_ntiles)
 
 
-WIDE_REC = 8             # ints per merged entry of build_wide_schedule (csrc/tc_xprop2.cuh XP2_REC)
+WIDE_REC = 16            # ints per merged entry of build_wide_schedule (csrc/tc_xprop2.cuh XP2_REC)
 
 
 def build_wide_schedule(outs, ins, wids, n_out, blocks_per_tile):
     """Merged LUT rows for the wide-tile xprop kernel (csrc/tc_xprop2.cuh).
 
-    Tile t covers output blocks [t*T, (t+1)*T), T = blocks_per_tile <= 4.  Its entries are the distinct input blocks
+    Tile t covers output blocks [t*T, (t+1)*T), T = blocks_per_tile <= 8.  Its entries are the distinct input blocks
     consumed by any of them, in ascending order, each with the W block of every output block of the tile (-1: none).
 
     int32 layout:
@@ -202,7 +202,7 @@ def build_wide_schedule(outs, ins, wids, n_out, blocks_per_tile):
     Returns (schedule, n_tiles, entry_offset).
     """
     T = int(blocks_per_tile)
-    assert 1 <= T <= WIDE_REC - 1
+    assert 1 <= T <= 8
     outs = np.asarray(outs, dtype=np.int64)
     ins = np.asarray(ins, dtype=np.int64)
     wids = np.asarray(wids, dtype=np.int64)
@@ -220,6 +220,36 @@ def build_wide_schedule(outs, ins, wids, n_out, blocks_per_tile):
     ent[:, 0] = uniq % n_in
     ent[inv, 1 + outs % T] = wids
     return sched, n_tiles, ent_off
+
+
+# Grouped-tile selection for the default 32 x 32 wgmma xprop (csrc/tc_xprop2.cuh: tc_xprop_grouped_kernel).  Both kernels
+# are bound by the bytes they stage from L2 into shared memory, per 128 minibatch rows: the one-block-per-CTA kernel
+# stages an 8 KB activation tile and a 2 KB W block per LUT entry, the grouped kernel an activation tile per MERGED entry
+# and the same W blocks.  The grouped tile is taken when the model says it stages at most XPROP_GROUP_MAX_BYTES of the
+# narrow kernel's bytes and its grid still has XPROP_GROUP_MIN_CTAS_PER_SM CTAs for every SM.  Both thresholds are read
+# off scripts/xprop_tiles.py on an H100 80GB HBM3 at 700 W (DESIGN.md section 5 has the table): at 4096 x 4096 and
+# N = 4096 the grouped tile is 5-6 % faster at 5 % density, where the model says 0.93 of the bytes, and gains from there
+# on; at N = 2048 (3.9 CTAs per SM, three of which run at a time) it is 17-18 % slower in spite of 0.78 of the bytes, at
+# N = 4096 (7.8 per SM) 20 % faster.
+XPROP_GROUP = 4
+XPROP_GROUP_MAX_BYTES = 0.95
+XPROP_GROUP_MIN_CTAS_PER_SM = 6.0
+
+
+def xprop_staged_bytes(nnz, merged_entries, N):
+    """Modelled bytes a 32 x 32, 16-bit xprop call stages into shared memory: (narrow kernel, grouped kernel)."""
+    n_tiles = ceil_div(N, 128)
+    return nnz * 10240 * n_tiles, (merged_entries * 8192 + nnz * 2048) * n_tiles
+
+
+def pick_xprop_tile(nnz, merged_entries, n_out, N, n_sm, group=XPROP_GROUP):
+    """Output blocks per CTA for the default 32 x 32 xprop route: `group` (grouped kernel) or 1 (one block per CTA).
+    merged_entries: entries of build_wide_schedule(..., group) for this layout and direction."""
+    narrow, grouped = xprop_staged_bytes(nnz, merged_entries, N)
+    ctas = ceil_div(N, 128) * ceil_div(n_out, group)
+    if grouped <= XPROP_GROUP_MAX_BYTES * narrow and ctas >= XPROP_GROUP_MIN_CTAS_PER_SM * n_sm:
+        return group
+    return 1
 
 
 GROUP_INTS = 32          # one 128-byte record per schedule group (one coalesced warp load)

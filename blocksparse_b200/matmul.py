@@ -13,14 +13,18 @@ import torch
 
 from . import _lib
 from .checkers import MatmulCheckers
-from .lut import MatmulLuts
+from .lut import MatmulLuts, WIDE_REC, XPROP_GROUP, pick_xprop_tile
 
-# Opt-in xprop variants for 32 x 32 blocks and 16-bit dtypes (the default is csrc/tc.cuh, one output block per CTA):
-# BSMM_XPROP2=1..3 selects a wide-tile kernel (csrc/tc_xprop2.cuh: 2 / 2 / 4 output blocks per CTA, 64 / 128 / 128
-# minibatch rows), BSMM_PAIR_TILES=1 runs csrc/tc.cuh as 2-CTA clusters that share every W block by TMA multicast.
+# 32 x 32 blocks and 16-bit dtypes: the default route picks, per layout, direction and minibatch, between one output block
+# per CTA (csrc/tc.cuh) and the grouped kernel of csrc/tc_xprop2.cuh (lut.pick_xprop_tile); results are bit-identical.
+# Opt-in variants: BSMM_XPROP2=1..3 selects a wide-tile kernel (csrc/tc_xprop2.cuh: 2 / 2 / 4 output blocks per CTA,
+# 64 / 128 / 128 minibatch rows), BSMM_PAIR_TILES=1 runs csrc/tc.cuh as 2-CTA clusters that share every W block by TMA
+# multicast.
 _X2_VARIANTS = {1: 2, 2: 2, 3: 4}          # variant -> output blocks per tile
 _X2_FORCE = int(os.environ.get("BSMM_XPROP2", "0"))
 _PAIR_TILES = int(os.environ.get("BSMM_PAIR_TILES", "0"))
+_GROUPED_VARIANTS = {4: 4}                 # output blocks per CTA -> bsmm_xprop variant of the grouped kernel
+_XPROP_TILE = None                         # tests / scripts: 1 forces one block per CTA, 4 the grouped tile (None: the model)
 # BSMM_PAD8=0: keep 8 x 8 blocks on the CUDA-core FMA kernels instead of the padded 16 x 16 wgmma path
 _PAD8 = int(os.environ.get("BSMM_PAD8", "1"))
 
@@ -182,6 +186,24 @@ class BlocksparseMatMul(MatmulCheckers):
             self._dev[key] = d
         return d
 
+    def _wide_schedule(self, d, device, bprop, blocks_per_tile):
+        key = ("wide", bool(bprop), blocks_per_tile)
+        if key not in d:
+            arr, n_tiles, off = self._luts.wide_schedule(bprop, blocks_per_tile)
+            d[key] = (torch.as_tensor(arr, device=device), n_tiles, off, (len(arr) - off) // WIDE_REC)
+        return d[key]
+
+    def xprop_tile(self, bprop, N, device):
+        """Output blocks per CTA of the default 32 x 32 / 16-bit xprop launch at minibatch N: 1 or the grouped tile."""
+        if _XPROP_TILE is not None:
+            return _XPROP_TILE
+        d = self._device_luts(device)
+        key = ("tile", bool(bprop), N)
+        if key not in d:
+            entries = self._wide_schedule(d, device, bprop, XPROP_GROUP)[3]
+            d[key] = pick_xprop_tile(self.blocks, entries, self.CB if bprop else self.KB, N, _lib.grid_sms(device))
+        return d[key]
+
     # ------------------------------------------------------------------ raw ops
     def fprop(self, x, w, gate=None, flags=0):
         return self._xprop(x, w, False, gate, flags)
@@ -230,14 +252,15 @@ class BlocksparseMatMul(MatmulCheckers):
         sched, sched_tiles, tile_arg, sched_off = None, 0, 0, 0
         if self.bsize == 32 and x.dtype != torch.float32:
             if _X2_FORCE in _X2_VARIANTS:
-                key = ("wide", bool(bprop), _X2_VARIANTS[_X2_FORCE])
-                if key not in d:
-                    arr, n_tiles, off = self._luts.wide_schedule(bprop, _X2_VARIANTS[_X2_FORCE])
-                    d[key] = (torch.as_tensor(arr, device=x.device), n_tiles, off)
-                sched, sched_tiles, sched_off = d[key]
+                sched, sched_tiles, sched_off, _ = self._wide_schedule(d, x.device, bprop, _X2_VARIANTS[_X2_FORCE])
                 tile_arg = (1 << 16) | (_X2_FORCE << 8)
             elif _PAIR_TILES:
                 tile_arg = 1 << 12
+            else:
+                tile = self.xprop_tile(bprop, N, x.device)
+                if tile > 1:
+                    sched, sched_tiles, sched_off, _ = self._wide_schedule(d, x.device, bprop, tile)
+                    tile_arg = (1 << 16) | (_GROUPED_VARIANTS[tile] << 8)
         y2 = torch.empty((feat_out, N) if self.axis == 0 else (N, feat_out), dtype=x.dtype, device=x.device)
         if gate is not None:
             gate = gate.to(torch.float32).contiguous()

@@ -120,10 +120,15 @@ int         bsmm_debug_trace(unsigned long long* out, int n);
  *    (blocksparse/matmul.py:360,369).
  * lut: row LUT grouped by output block (n_out headers).  Output blocks with no entries are
  *    zero-filled (reference behaviour, cn_64.cu:243-253).
- * sched: NULL for the default wgmma kernel (it walks `lut`).  Opt-in variants for 32 x 32 blocks and 16-bit dtypes:
- *    bit 12 of sched_tile_blocks: 2-CTA clusters sharing every W block by TMA multicast (same results, bit for bit);
- *    bit 16: the wide-tile kernel -- sched = lut.py:build_wide_schedule in device memory with sched_tiles tiles, its
- *    entries at int32 index sched_groups_off, bits 8..15 the variant (1, 2, 3).
+ * sched: NULL for the wgmma kernel that gives a CTA one output block (it walks `lut`).  For 32 x 32 blocks and 16-bit
+ *    dtypes, selected through sched_tile_blocks:
+ *    bit 12: 2-CTA clusters sharing every W block by TMA multicast (same results, bit for bit);
+ *    bit 16: a kernel over tiles of consecutive output blocks -- sched = lut.py:build_wide_schedule in device memory with
+ *    sched_tiles tiles, its entries (16 ints each) at int32 index sched_groups_off, bits 8..15 the variant:
+ *      1, 2, 3  wide tiles of 2 / 2 / 4 blocks that multiply absent blocks as zeros (opt-in, launch name wgmma_xprop2_bs32);
+ *      4        grouped tiles of 4 blocks: only the blocks that exist are fetched and multiplied, results bit-identical
+ *               to sched = NULL, launch name wgmma_xprop_bs32.  BlocksparseMatMul picks between this and sched = NULL
+ *               per layout, direction and N (lut.py:pick_xprop_tile).
  * sched_list_off, sched_ctas, sched_ntiles: reserved (ABI compatibility); pass 0.
  * 16-bit dtypes with block size 16 / 32 / 64 (and N % 8 == 0 for axis 0) run on the wgmma kernel; other calls run on
  *    the CUDA-core kernels.

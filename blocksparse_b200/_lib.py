@@ -199,7 +199,7 @@ def guarded(fn):
     @functools.wraps(fn)
     def wrapper(self, *args, **kw):
         dev = None
-        for a in args:
+        for a in (args + tuple(kw.values()) if kw else args):
             if is_tensor(a):
                 if a.is_cuda:
                     if dev is None:

@@ -505,6 +505,8 @@ class _L2NormalizeFunction(torch.autograd.Function):
         g = None if gain is None else gain.to(torch.float32).contiguous()
         if g is not None and g.numel() != bsmm.K:
             raise ValueError("gain must have K = %d entries" % bsmm.K)
+        if g is not None and g.device != W.device:
+            raise ValueError("gain lives on %s, W on %s" % (g.device, W.device))
         y = torch.empty(bsmm.w_shape, dtype=out_dtype, device=W.device)
         ss = torch.empty(bsmm.K, dtype=torch.float32, device=W.device)
         d = bsmm._device_luts(W.device)
@@ -558,7 +560,11 @@ def blocksparse_reduced_dw(xs, dys, scale, dwi=None, bsize=32, norm="max", axis=
     for a, b in zip(xs, dys):
         if a.dtype != x0.dtype or b.dtype != x0.dtype or a.shape[1 - axis] != N or b.shape[1 - axis] != N or a.shape[axis] != C or b.shape[axis] != K:
             raise ValueError("all pairs must share dtype, minibatch and feature sizes")
+        if a.device != x0.device or b.device != x0.device:
+            raise ValueError("all pairs must live on one device, got %s and %s" % (x0.device, a.device if a.device != x0.device else b.device))
     dev = x0.device
+    if dwi is not None and dwi.device != dev:
+        raise ValueError("dwi lives on %s, the pairs on %s" % (dwi.device, dev))
     x_red = torch.empty((bC, P, N) if axis == 0 else (P, N, bC), dtype=x0.dtype, device=dev)
     y_red = torch.empty((bK, P, N) if axis == 0 else (P, N, bK), dtype=x0.dtype, device=dev)
     if dwi is None:
@@ -627,6 +633,8 @@ class _ScatterAddMul(torch.autograd.Function):
 def _gather_rows(x, y, idx, n_out, op):
     if not x.is_cuda:
         raise _lib.BsmmError("SparseProj needs CUDA tensors (no CPU path)")
+    if y is not None and y.device != x.device:
+        raise ValueError("SparseProj: operands live on %s and %s" % (x.device, y.device))
     x2 = x.reshape(x.shape[0], -1).contiguous()
     y2 = None if y is None else y.reshape(y.shape[0], -1).contiguous()
     out = torch.empty((n_out,) + tuple(x.shape[1:]), dtype=x.dtype, device=x.device)

@@ -21,6 +21,8 @@ def _check_param_shape(param, gate=None):
         raise ValueError("param must be (blocks, bsize, bsize) with bsize in {8,16,32,64}, got %s" % (tuple(param.shape),))
     if gate is not None and (gate.dim() != 1 or gate.shape[0] != param.shape[0] or gate.dtype != torch.float32):
         raise ValueError("gate must be a float32 vector with one entry per block")
+    if gate is not None and gate.device != param.device:
+        raise ValueError("gate lives on %s, param on %s" % (gate.device, param.device))
     if not param.is_cuda or not param.is_contiguous():
         raise _lib.BsmmError("block-sparse utilities need contiguous CUDA tensors (no CPU path)")
 
@@ -128,7 +130,15 @@ class AdamOptimizer(torch.optim.Optimizer):
     the param and both moments bit for bit. fp16=True: params of at least 8192 elements keep their mean and variance as
     int16 tensors of the reference's 16-bit codes (8 bytes of state per parameter instead of 12).
     norm_scale: a one-element fp32 CUDA tensor (e.g. from clip_by_global_norm) read on the device at every step; 0 makes
-    the step a no-op. The *_qspec arguments of the reference's quantize module must be None."""
+    the step a no-op. The *_qspec arguments of the reference's quantize module must be None.
+
+    Params may live on several GPUs: each step launches once per device (per 256 params), in param order, with that
+    device current; norm_scale reaches the other devices by a device-to-device copy.
+
+    CUDA graphs: lr_t is a kernel argument, so a captured step replays with the lr_t of the step it captured. That is
+    only right while both beta powers are 0, i.e. with zero_init_variables=True; under capture step() raises ValueError
+    for a group whose powers are not 0 (and a changed param_groups[i]["lr"] takes effect only when the graph is
+    captured again)."""
 
     def __init__(self, params, learning_rate=3e-4, beta1=0.9, beta2=0.999, epsilon=1e-8, clip_sigmas=0.0,
                  norm_scale=None, grad_scale=1.0, saturate=0.0, zero_infs=False, zero_nans=False, gated=False,
@@ -177,11 +187,18 @@ class AdamOptimizer(torch.optim.Optimizer):
         every = [p for group in self.param_groups for p in group["params"]]
         if grads is not None and len(grads) != len(every):
             raise ValueError("AdamOptimizer.step: %d grads for %d params" % (len(grads), len(every)))
+        if torch.cuda.is_current_stream_capturing():
+            for group in self.param_groups:
+                if group["beta1_power"] != 0.0 or group["beta2_power"] != 0.0:
+                    raise ValueError("AdamOptimizer.step under CUDA graph capture: the bias-corrected lr_t is a kernel "
+                                     "argument and would be replayed unchanged while beta1_power / beta2_power (%r, %r) "
+                                     "advance; capture needs zero_init_variables=True"
+                                     % (group["beta1_power"], group["beta2_power"]))
         k = 0
         lib = _lib.load()
         f32 = np.float32
         for group in self.param_groups:
-            gs, ps, ms, vs, gd, codes, sizes, gates, bss = [], [], [], [], [], [], [], [], []
+            per_dev = {}             # device -> the step's tables for the params on it, in param order
             for p in group["params"]:
                 g = grads[k] if grads is not None else p.grad
                 k += 1
@@ -194,6 +211,7 @@ class AdamOptimizer(torch.optim.Optimizer):
                     raise ValueError("AdamOptimizer.step: params must be contiguous")
                 if p.numel() == 0:
                     continue
+                gs, gd, ps, ms, vs, codes, sizes, gates, bss = per_dev.setdefault(p.device, tuple([] for _ in range(9)))
                 gd.append(_lib.dtype_code(g.dtype))
                 gate, bs = _gate_of(p, self.gated)
                 m, v = self._moments(p)
@@ -207,11 +225,12 @@ class AdamOptimizer(torch.optim.Optimizer):
                 bss.append(bs)
             b1p, b2p = f32(group["beta1_power"]), f32(group["beta2_power"])
             lr_t = f32(group["lr"]) * np.sqrt(f32(1) - b2p) / (f32(1) - b1p)           # optimize.py:57
-            if ps:
+            for dev, (gs, gd, ps, ms, vs, codes, sizes, gates, bss) in per_dev.items():
                 arrs = (_ptrs(gs), _i32(gd), _ptrs(ps), _ptrs(ms), _ptrs(vs), _i32(codes), _i64(sizes),
                         np.array(gates, dtype=np.uint64), _i32(bss))
-                with torch.cuda.device(ps[0].device):
-                    rc = lib.bsmm_adam(len(ps), *[a.ctypes.data for a in arrs], _lib.ptr(ns), float(lr_t),
+                with torch.cuda.device(dev):
+                    ns_dev = ns if ns is None or ns.device == dev else ns.to(dev)
+                    rc = lib.bsmm_adam(len(ps), *[a.ctypes.data for a in arrs], _lib.ptr(ns_dev), float(lr_t),
                                        float(self.beta1), float(self.beta2), float(self.epsilon), float(self.grad_scale),
                                        float(self.clip_sigmas), float(self.saturate), int(self.zero_infs),
                                        int(self.zero_nans), _lib.stream_ptr())
@@ -225,13 +244,19 @@ def clip_by_global_norm(grads, clip_norm=1.0, grad_scale=1.0, saturate=0.0, zero
     """(global_norm, norm_scale) as 0-dim fp32 CUDA tensors (reference optimize.py:197-225): global_norm =
     sqrt(sum of (grad_scale * sat(filter(x)))^2) over every element of every grad; norm_scale = clip_norm /
     max(global_norm, clip_norm), or 0 when the norm is not finite. grads may mix fp32, fp16 and bf16 and include empty
-    tensors. Two launches (one more per 256 tensors), no host synchronisation, bitwise reproducible."""
+    tensors. Two launches (one more per 256 tensors), no host synchronisation, bitwise reproducible.
+
+    All grads must be on one device (ValueError otherwise): one norm over several GPUs would need a cross-device
+    reduction, which this op does not do. Clip each device's grads separately, or reduce the squared norms yourself."""
     grads = list(grads)
     for g in grads:
         if not torch.is_tensor(g) or g.dtype not in (torch.float32, torch.float16, torch.bfloat16):
             raise ValueError("clip_by_global_norm: unsupported grad dtype %s" % (getattr(g, "dtype", type(g)),))
         if not g.is_cuda:
             raise ValueError("clip_by_global_norm: grads must be CUDA tensors (there is no CPU path)")
+        if g.device != grads[0].device:
+            raise ValueError("clip_by_global_norm: grads live on %s and %s; one norm over several devices is not "
+                             "computed here" % (grads[0].device, g.device))
     device = grads[0].device if grads else torch.device("cuda", torch.cuda.current_device())
     live = [g.contiguous() for g in grads if g.numel()]
     if not live:
@@ -266,7 +291,8 @@ def ClipGlobalNorm(grads, clip_norm=1.0, grad_scale=1.0, saturate=0.0, zero_infs
 class Ema(object):
     """Exponential moving averages of params (reference optimize.py:231-289): apply(params) creates each average on first
     use as a copy of the param (float16 when fp16), then does ema -= (1 - decay) * (ema - param) for all of them in one
-    launch (per 256). Gated, blocks of a param with a `.gate` whose gate is 0 keep their average."""
+    launch (per 256, and per device for params on several GPUs). Gated, blocks of a param with a `.gate` whose gate is
+    0 keep their average."""
 
     def __init__(self, decay=0.999, gated=False, fp16=False, name="Ema"):
         self.decay, self.gated, self.fp16, self.name = decay, gated, fp16, name
@@ -276,7 +302,7 @@ class Ema(object):
     def apply(self, params, qspec=None):
         _check_qspec(qspec=qspec)
         params = list(params)
-        emas, ps, sizes, gates, bss = [], [], [], [], []
+        per_dev = {}                 # device -> the tables for the params on it, in param order
         for p in params:
             if not torch.is_tensor(p) or not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous():
                 raise ValueError("Ema.apply: params must be contiguous float32 CUDA tensors")
@@ -286,19 +312,19 @@ class Ema(object):
             if p.numel() == 0:
                 continue
             gate, bs = _gate_of(p, self.gated)
+            emas, ps, sizes, gates, bss = per_dev.setdefault(p.device, tuple([] for _ in range(5)))
             emas.append(entry[1])
             ps.append(p)
             sizes.append(p.numel())
             gates.append(gate.data_ptr() if gate is not None else 0)
             bss.append(bs)
-        if not ps:
-            return
-        arrs = (_ptrs(emas), _ptrs(ps), _i64(sizes), np.array(gates, dtype=np.uint64), _i32(bss))
-        with torch.cuda.device(ps[0].device):
-            rc = _lib.load().bsmm_ema(len(ps), arrs[0].ctypes.data, _lib.F16 if self.fp16 else _lib.F32, arrs[1].ctypes.data,
-                                      arrs[2].ctypes.data, arrs[3].ctypes.data, arrs[4].ctypes.data, float(self.decay),
-                                      _lib.stream_ptr())
-        _lib.check(rc, "bsmm_ema")
+        for dev, (emas, ps, sizes, gates, bss) in per_dev.items():
+            arrs = (_ptrs(emas), _ptrs(ps), _i64(sizes), np.array(gates, dtype=np.uint64), _i32(bss))
+            with torch.cuda.device(dev):
+                rc = _lib.load().bsmm_ema(len(ps), arrs[0].ctypes.data, _lib.F16 if self.fp16 else _lib.F32,
+                                          arrs[1].ctypes.data, arrs[2].ctypes.data, arrs[3].ctypes.data,
+                                          arrs[4].ctypes.data, float(self.decay), _lib.stream_ptr())
+            _lib.check(rc, "bsmm_ema")
 
     def average(self, param):
         entry = self.averages.get(id(param))

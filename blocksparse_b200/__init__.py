@@ -5,7 +5,8 @@ updat, group_param_grads) and `BlocksparseTransformer` (NT / NN / TN + masked so
 implemented as hand-written sm_90a CUDA behind the C ABI in include/bsmm_b200.h, plus the dense ops of the
 reference's transformer module (softmax, masked_softmax, masked_top_k_softmax, top_k, rectified_top_k,
 softmax_cross_entropy, transpose_0213, transpose_2d), of its norms module (layer_norm) and of its optimize module
-(AdamOptimizer, clip_by_global_norm, global_norm, Ema).
+(AdamOptimizer, clip_by_global_norm, global_norm, Ema), and of its ewops and embed modules (bias_relu, dropout,
+set_entropy, get_entropy, embedding_lookup; listed in ewops.__all__ and embed.__all__).
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
 from .optimize import (AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay, blocksparse_norm, blocksparse_prune,
@@ -13,6 +14,8 @@ from .optimize import (AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay,
 from .transformer import (BlocksparseTransformer, masked_softmax, masked_top_k_softmax, rectified_top_k, softmax,
                           softmax_cross_entropy, top_k, transpose_0213, transpose_2d)
 from .norms import layer_norm
+from .ewops import bias_relu, dropout, get_entropy, set_entropy
+from .embed import embedding_lookup
 from .lut import z_order_2d
 from . import _lib
 

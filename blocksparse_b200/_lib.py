@@ -50,6 +50,14 @@ SIGNATURES = {
     "bsmm_layer_norm": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _i, _f, _i, _vp]),
     "bsmm_layer_norm_grad": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _i, _f, _i, _vp]),
     "bsmm_layer_norm_workspace_bytes": (_c.c_size_t, [_i, _ll, _i, _i]),
+    "bsmm_bias_relu": (_i, [_i, _i, _i, _vp, _vp, _vp, _ll, _i, _i, _vp]),
+    "bsmm_bias_relu_grad": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
+    "bsmm_bias_grad_workspace_bytes": (_c.c_size_t, [_i, _ll, _i]),
+    "bsmm_dropout_mask": (_i, [_vp, _ll, _c.c_double, _vp, _vp]),
+    "bsmm_dropout_apply": (_i, [_i, _vp, _vp, _vp, _i, _vp, _vp, _ll, _c.c_double, _vp]),
+    "bsmm_embedding_lookup": (_i, [_i, _i, _vp, _vp, _vp, _ll, _i, _i, _vp]),
+    "bsmm_embedding_grad": (_i, [_i, _i, _vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
+    "bsmm_embedding_grad_workspace_bytes": (_c.c_size_t, [_ll, _i, _i]),
     "bsmm_adam": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _i, _i, _vp]),
     "bsmm_global_norm": (_i, [_i, _vp, _vp, _vp, _f, _f, _f, _i, _i, _vp, _vp, _vp, _vp]),
     "bsmm_global_norm_workspace_bytes": (_c.c_size_t, [_i, _vp]),

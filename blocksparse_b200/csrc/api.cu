@@ -4,6 +4,8 @@
 #include <climits>
 #include "common.cuh"
 #include "dense_softmax.cuh"
+#include "embed.cuh"
+#include "ewops.cuh"
 #include "generic.cuh"
 #include "layer_norm.cuh"
 #include "optimize.cuh"
@@ -597,6 +599,138 @@ int bsmm_layer_norm_grad(int dtype, int gdtype, int axis, const void* dy, const 
     const bool vec = aligned16(x) && aligned16(dy) && aligned16(dx) && a.L % V == 0;
     BSMM_DISPATCH_DTYPE(dtype, T, { return launch_layer_norm_nc<T>(a, true, vec, gdtype, dg, db, (cudaStream_t)stream); });
   }
+  return 0;
+}
+
+// ---- bias + activation and dropout (csrc/ewops.cuh) ------------------------------------------------------------------------
+static int br_args(const char* what, int dtype, int bdtype, int axis, long long N, int K, int act) {
+  if (!dense_dtype_ok(dtype) || !dense_dtype_ok(bdtype))
+    return fail(BSMM_E_ARG, "%s: unsupported dtype codes %d, %d", what, dtype, bdtype);
+  if (axis != 0 && axis != 1) return fail(BSMM_E_ARG, "%s: axis must be 0 or 1, got %d", what, axis);
+  if (N < 0 || K <= 0) return fail(BSMM_E_ARG, "%s: bad sizes N %lld, K %d", what, N, K);
+  if (act < ACT_NONE || act > ACT_FAST_GELU) return fail(BSMM_E_ARG, "%s: act must be 0, 1 or 2, got %d", what, act);
+  if (axis == 0 && (N + BR_SEG - 1) / BR_SEG > 0x7fffffffLL) return fail(BSMM_E_LIMIT, "%s: N %lld exceeds the grid", what, N);
+  return 0;
+}
+
+size_t bsmm_bias_grad_workspace_bytes(int axis, long long N, int K) {
+  if ((axis != 0 && axis != 1) || N <= 0 || K <= 0) return 0;
+  return br_workspace_floats(axis, N, K) * sizeof(float);
+}
+
+int bsmm_bias_relu(int dtype, int bdtype, int axis, const void* x, const void* b, void* y, long long N, int K, int act,
+                   void* stream) {
+  if (int e = br_args("bsmm_bias_relu", dtype, bdtype, axis, N, K, act)) return e;
+  if (!x || !b || !y) return fail(BSMM_E_ARG, "bsmm_bias_relu: null pointer");
+  if (N == 0) return 0;
+  BrArgs a = {};
+  a.x = x; a.b = b; a.y = y; a.N = N; a.K = K; a.bdt = bdtype; a.act = act;
+  const bool vec = aligned16(x) && aligned16(y) && (axis ? K : N) % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_bias_act<T>(a, axis, false, vec, nullptr, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_bias_relu_grad(int dtype, int bdtype, int axis, const void* dy, const void* src, const void* b, void* dx,
+                        void* db, void* workspace, long long N, int K, int act, void* stream) {
+  if (int e = br_args("bsmm_bias_relu_grad", dtype, bdtype, axis, N, K, act)) return e;
+  if (!dy || !b || !db || !workspace || (act != ACT_NONE && (!src || !dx)))
+    return fail(BSMM_E_ARG, "bsmm_bias_relu_grad: null pointer");
+  if (N == 0) return 0;
+  BrArgs a = {};
+  a.x = dy; a.src = src; a.b = b; a.y = dx; a.part = (float*)workspace; a.N = N; a.K = K; a.bdt = bdtype; a.act = act;
+  const bool vec = aligned16(dy) && (act == ACT_NONE || (aligned16(src) && aligned16(dx))) &&
+                   (axis ? K : N) % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_bias_act<T>(a, axis, true, vec, db, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_dropout_mask(int32_t* mask, long long M, double keep_prob, long long* state, void* stream) {
+  if (!mask || !state) return fail(BSMM_E_ARG, "bsmm_dropout_mask: null pointer");
+  if (M < 0) return fail(BSMM_E_ARG, "bsmm_dropout_mask: bad size %lld", M);
+  if (!(keep_prob > 0.0 && keep_prob <= 1.0)) return fail(BSMM_E_ARG, "bsmm_dropout_mask: keep_prob must be in (0, 1]");
+  if (M == 0) return 0;
+  const unsigned long long thr = (unsigned long long)floor(keep_prob * 4294967296.0);
+  return launch_dropout_mask((uint32_t*)mask, M, thr, state, (cudaStream_t)stream);
+}
+
+int bsmm_dropout_apply(int dtype, const void* x, const int32_t* mask, void* y, int ndim, const long long* shape,
+                       const long long* mask_strides, long long mask_words, double keep_prob, void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_dropout_apply: unsupported dtype code %d", dtype);
+  if (ndim < 0 || ndim > DROP_MAX_DIMS) return fail(BSMM_E_ARG, "bsmm_dropout_apply: ndim must be in [0, %d]", DROP_MAX_DIMS);
+  if (ndim > 0 && (!shape || !mask_strides)) return fail(BSMM_E_ARG, "bsmm_dropout_apply: null shape or strides");
+  if (!(keep_prob > 0.0 && keep_prob <= 1.0)) return fail(BSMM_E_ARG, "bsmm_dropout_apply: keep_prob must be in (0, 1]");
+  DropArgs a = {};
+  long long n = 1, top = 0;
+  for (int d = 0; d < ndim; ++d) {
+    if (shape[d] < 0 || mask_strides[d] < 0) return fail(BSMM_E_ARG, "bsmm_dropout_apply: negative size or stride in dim %d", d);
+    if (shape[d] == 0) n = 0;
+    else if (n && shape[d] > LLONG_MAX / n) return fail(BSMM_E_LIMIT, "bsmm_dropout_apply: more than 2^63 elements");
+    else n *= shape[d];
+  }
+  if (!x || !mask || !y) return fail(BSMM_E_ARG, "bsmm_dropout_apply: null pointer");
+  if (n == 0) return mask_words < 0 ? fail(BSMM_E_ARG, "bsmm_dropout_apply: bad mask_words") : 0;
+  // drop size-1 dims; merge a dim into the next inner one when both broadcast or both are contiguous in the mask
+  for (int d = 0; d < ndim; ++d) {
+    if (shape[d] == 1) continue;
+    top += (shape[d] - 1) * mask_strides[d];
+    const long long st = mask_strides[d];
+    if (a.nd > 0) {
+      const int i = a.nd - 1;
+      if ((a.mst[i] == 0 && st == 0) || (st != 0 && a.mst[i] == st * shape[d])) {
+        a.size[i] *= shape[d];
+        a.mst[i] = st;
+        continue;
+      }
+    }
+    a.size[a.nd] = shape[d];
+    a.mst[a.nd++] = st;
+  }
+  if (top >= mask_words * 32 || mask_words < 1) return fail(BSMM_E_ARG, "bsmm_dropout_apply: the mask has too few words");
+  if (a.nd > 0 && a.mst[a.nd - 1] > 1) return fail(BSMM_E_ARG, "bsmm_dropout_apply: the innermost mask stride must be 0 or 1");
+  if (a.nd == 1 && a.mst[0] == 1) a.nd = 0;
+  a.x = x; a.mask = (const uint32_t*)mask; a.y = y; a.n = n; a.words = mask_words; a.scale = (float)(1.0 / keep_prob);
+  const int V = 16 / dtype_size(dtype);
+  const bool vec = aligned16(x) && aligned16(y) && (a.nd == 0 ? n : a.size[a.nd - 1]) % V == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_dropout_apply<T>(a, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+// ---- embedding (csrc/embed.cuh) --------------------------------------------------------------------------------------------
+static int emb_args(const char* what, int dtype, int idx_type, long long n, int C, int K) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "%s: unsupported dtype code %d", what, dtype);
+  if (idx_type < BSMM_LABEL_U8 || idx_type > BSMM_LABEL_I64) return fail(BSMM_E_ARG, "%s: unsupported index type %d", what, idx_type);
+  if (n < 0 || C < 0 || K <= 0) return fail(BSMM_E_ARG, "%s: bad sizes n %lld, C %d, K %d", what, n, C, K);
+  return 0;
+}
+
+int bsmm_embedding_lookup(int dtype, int idx_type, const void* emb, const void* idx, void* y, long long n, int C, int K,
+                          void* stream) {
+  if (int e = emb_args("bsmm_embedding_lookup", dtype, idx_type, n, C, K)) return e;
+  if (!idx || !y || (C > 0 && !emb)) return fail(BSMM_E_ARG, "bsmm_embedding_lookup: null pointer");
+  if (n == 0) return 0;
+  const int es = dtype_size(dtype);
+  if (aligned16(emb) && aligned16(y) && (K * es) % 16 == 0)
+    return launch_embedding_lookup<uint4>(emb, idx, idx_type, y, n, C, K * es / 16, (cudaStream_t)stream);
+  if (es == 4) return launch_embedding_lookup<uint32_t>(emb, idx, idx_type, y, n, C, K, (cudaStream_t)stream);
+  return launch_embedding_lookup<uint16_t>(emb, idx, idx_type, y, n, C, K, (cudaStream_t)stream);
+}
+
+size_t bsmm_embedding_grad_workspace_bytes(long long n, int C, int K) {
+  if (n <= 0 || n > 0x7fffffffLL || C <= 0 || C == INT_MAX || K <= 0) return 0;
+  return emb_workspace_bytes(n, C, K);
+}
+
+int bsmm_embedding_grad(int dtype, int idx_type, const void* dy, const void* idx, void* dw, void* workspace, long long n,
+                        int C, int K, void* stream) {
+  if (int e = emb_args("bsmm_embedding_grad", dtype, idx_type, n, C, K)) return e;
+  if (!idx || !dy || !dw || (n > 0 && !workspace)) return fail(BSMM_E_ARG, "bsmm_embedding_grad: null pointer");
+  if (n > 0x7fffffffLL) return fail(BSMM_E_LIMIT, "bsmm_embedding_grad: more than 2^31 - 1 indices");
+  if (C == INT_MAX) return fail(BSMM_E_LIMIT, "bsmm_embedding_grad: C must be below 2^31 - 1");
+  if (C == 0 || n == 0) return 0;
+  const bool vec = aligned16(dy) && aligned16(dw) && K % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, {
+    return launch_embedding_grad<T>(dy, idx, idx_type, dw, workspace, n, C, K, vec, (cudaStream_t)stream);
+  });
   return 0;
 }
 

@@ -27,6 +27,12 @@
  *   bsmm_layer_norm       <- LayerNormForward_NC / LayerNormSegmentedForward_NC / LayerNormForward_CN
  *                            (src/layer_norm_op.cc)
  *   bsmm_layer_norm_grad  <- LayerNormBackward_NC / LayerNormSegmentedBackward_NC / LayerNormBackward_CN
+ *   bsmm_bias_relu        <- EW_Bias_Relu (src/ew_op.cc:741-813)
+ *   bsmm_bias_relu_grad   <- EW_Bias_Relu_Grad and BiasGrad (src/ew_op.cc:832-1002)
+ *   bsmm_dropout_mask     <- GenDropoutMask (src/ew_op.cc:524-591)
+ *   bsmm_dropout_apply    <- ApplyDropoutMask (src/ew_op.cc:593-691)
+ *   bsmm_embedding_lookup <- EmbeddingLookup (src/embedding_op.cc)
+ *   bsmm_embedding_grad   <- EmbeddingLookupGrad (src/embedding_op.cc)
  *   bsmm_block_norm / bsmm_l2_decay / bsmm_threshold_prune / bsmm_prune_topk
  *                         <- BlocksparseNorm / BlocksparseL2Decay / BlocksparseThresholdPrune / BlocksparsePrune
  *                            (src/optimize_op_gpu.cu:794-1098)
@@ -383,6 +389,82 @@ int bsmm_layer_norm_grad(int dtype, int gdtype, int axis, const void* dy, const 
 /* Bytes of device workspace bsmm_layer_norm and bsmm_layer_norm_grad need for (axis, N, K, segments): the fp32 partial
  * sums of the backward (and of the axis-0 forward's row splits). 0 for bad arguments or N = 0. */
 size_t bsmm_layer_norm_workspace_bytes(int axis, long long N, int K, int segments);
+
+/* ---- bias + activation, dropout (the reference's ewops module) and embedding (its embed module) ------------------- */
+
+/*
+ * y = act(x + b), formed in fp32 and rounded once to dtype. act 0: identity, 1: relu, 2: fast_gelu z * sigmoid(1.702 z).
+ *   axis 1: x, y (N, K) of dtype, contiguous, b[k] added to column k;
+ *   axis 0: x, y (K, N), N contiguous (BlocksparseMatMul(feature_axis=0) activations), b[k] added to row k.
+ *   b: K entries of bdtype (F32, F16 or BF16), read as fp32.
+ * Replaces EW_Bias_Relu (src/ew_op_gpu.cu:919-1034, launched from src/ew_op.cc:741-813). Any alignment (16-byte accesses
+ * where every row start allows), 64-bit element offsets. A bad dtype, axis other than 0 / 1, N < 0, K <= 0, act outside
+ * 0..2 or a null pointer: BSMM_E_ARG before any launch. N = 0 launches nothing. Kernels: bias_relu_nc (axis 1),
+ * bias_relu_cn (axis 0).
+ */
+int bsmm_bias_relu(int dtype, int bdtype, int axis, const void* x, const void* b, void* y, long long N, int K, int act,
+                   void* stream);
+
+/*
+ * dx (dtype) and db (K entries of bdtype) of bsmm_bias_relu, given dy and src: y for relu (dx = dy * (y > 0)), x for
+ * fast_gelu (z = x + b recomputed in fp32). With act 0, dx is dy itself: src and dx are not read or written (they may be
+ * NULL) and only db is formed. dx is written in the pass that reads dy, together with fp32 partial sums of db in
+ * `workspace` (bsmm_bias_grad_workspace_bytes), which a second kernel adds in a fixed order: the partition depends on
+ * the shape only and there are no atomics, so db is bitwise reproducible. Replaces EW_Bias_Relu_Grad and BiasGrad
+ * (src/ew_op_gpu.cu:1039-1429, src/ew_op.cc:832-1002), which add db with atomics. Shapes and errors as bsmm_bias_relu.
+ * Kernels: bias_relu_grad_nc, bias_relu_grad_cn.
+ */
+int bsmm_bias_relu_grad(int dtype, int bdtype, int axis, const void* dy, const void* src, const void* b, void* dx,
+                        void* db, void* workspace, long long N, int K, int act, void* stream);
+
+/* Bytes of device workspace bsmm_bias_relu_grad needs for (axis, N, K): 0 for bad arguments or N = 0. */
+size_t bsmm_bias_grad_workspace_bytes(int axis, long long N, int K);
+
+/*
+ * mask: ceil(M / 32) int32 words; bit e % 32 of word e / 32 set means keep element e; bits at or past M are 0. Element e
+ * is kept iff word e % 4 of Philox4x32-10(counter = (e / 4 as 64 bits, call as 64 bits), key = seed) is below
+ * floor(keep_prob * 2^32), compared in 64 bits (keep_prob 1 keeps all). state: device int64 [seed, call]; the kernel
+ * reads it, and a second one-thread kernel then adds 1 to call, in stream order. Calls that share a state must
+ * therefore be stream-ordered. Replaces GenDropoutMask (src/ew_op_gpu.cu:687-733, src/ew_op.cc:524-591), whose
+ * Tausworthe state is sized for 80 V100 SMs. Null pointers, M < 0 or keep_prob outside (0, 1]: BSMM_E_ARG before any
+ * launch; M = 0 launches nothing. Kernel: dropout_mask.
+ */
+int bsmm_dropout_mask(int32_t* mask, long long M, double keep_prob, long long* state, void* stream);
+
+/*
+ * y = bit ? round(fp32(x) * fp32(1 / keep_prob)) : +0 for every element of x, y (shape[0..ndim), dtype, contiguous). The
+ * bit of the element at multi-index i is bit m of mask, m = sum_d i[d] * mask_strides[d]: mask_strides are the
+ * row-major strides of the mask's shape, 0 on the dims it broadcasts over. shape and mask_strides are host arrays read
+ * before the call returns; mask has mask_words words. Replaces ApplyDropoutMask (src/ew_op_gpu.cu:735-814,
+ * src/ew_op.cc:593-691). ndim outside [0, 8], negative sizes or strides, a mask index past mask_words * 32, an innermost
+ * stride other than 0 / 1 (after size-1 dims are dropped), a bad dtype, keep_prob outside (0, 1] or a null pointer:
+ * BSMM_E_ARG before any launch; no element launches nothing. Kernel: dropout_apply.
+ */
+int bsmm_dropout_apply(int dtype, const void* x, const int32_t* mask, void* y, int ndim, const long long* shape,
+                       const long long* mask_strides, long long mask_words, double keep_prob, void* stream);
+
+/*
+ * y[i, :] = emb[idx[i], :] bit for bit, or zeros where idx[i] is outside [0, C). emb (C, K) and y (n, K) of dtype,
+ * contiguous; idx: n integers of idx_type (BSMM_LABEL_*). Replaces EmbeddingLookup (src/embedding_op_gpu.cu, launched from
+ * src/embedding_op.cc). A bad dtype or index type, n < 0, C < 0, K <= 0 or a null pointer: BSMM_E_ARG before any
+ * launch; n = 0 launches nothing. Kernel: embedding_lookup.
+ */
+int bsmm_embedding_lookup(int dtype, int idx_type, const void* emb, const void* idx, void* y, long long n, int C, int K,
+                          void* stream);
+
+/*
+ * dw (C, K) of dtype: dw[c, :] = sum of dy[i, :] over the i with idx[i] == c, in fp32, in ascending i, rounded once;
+ * rows no index hits are 0, out-of-range indices contribute nothing. A stable radix sort of (index, position), then
+ * fixed-size chunks of the sorted order summed per run, groups of 32 chunks inside one run summed once more, and the
+ * partials of a run added in chunk order: deterministic, no
+ * atomics. workspace: bsmm_embedding_grad_workspace_bytes(n, C, K) bytes. Replaces EmbeddingLookupGrad
+ * (src/embedding_op_gpu.cu, src/embedding_op.cc), which adds with atomics (sorted or not). Errors as
+ * bsmm_embedding_lookup, plus a null workspace; n > 2^31 - 1 or C = 2^31 - 1: BSMM_E_LIMIT. n = 0 or C = 0 launches
+ * nothing and leaves dw as it is. Kernel: embedding_grad.
+ */
+int bsmm_embedding_grad(int dtype, int idx_type, const void* dy, const void* idx, void* dw, void* workspace, long long n,
+                        int C, int K, void* stream);
+size_t bsmm_embedding_grad_workspace_bytes(long long n, int C, int K);
 
 /* ---- utilities on the (blocks, bsize, bsize) weight format -------------------------------------- */
 

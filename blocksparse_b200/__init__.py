@@ -5,12 +5,13 @@ updat, group_param_grads) and `BlocksparseTransformer` (NT / NN / TN + masked so
 implemented as hand-written sm_90a CUDA behind the C ABI in include/bsmm_b200.h, plus the dense ops of the
 reference's transformer module (softmax, masked_softmax, masked_top_k_softmax, top_k, rectified_top_k,
 softmax_cross_entropy, transpose_0213, transpose_2d), of its norms module (layer_norm) and of its optimize module
-(AdamOptimizer, clip_by_global_norm, global_norm, Ema), and of its ewops and embed modules (bias_relu, dropout,
+(AdamOptimizer, clip_by_global_norm, global_norm, Ema; AdafactorOptimizer, importable from here and from
+blocksparse_b200.optimize but not listed in __all__), and of its ewops and embed modules (bias_relu, dropout,
 set_entropy, get_entropy, embedding_lookup; listed in ewops.__all__ and embed.__all__).
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
-from .optimize import (AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay, blocksparse_norm, blocksparse_prune,
-                       clip_by_global_norm, global_norm)
+from .optimize import (AdafactorOptimizer, AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay, blocksparse_norm,
+                       blocksparse_prune, clip_by_global_norm, global_norm)
 from .transformer import (BlocksparseTransformer, masked_softmax, masked_top_k_softmax, rectified_top_k, softmax,
                           softmax_cross_entropy, top_k, transpose_0213, transpose_2d)
 from .norms import layer_norm

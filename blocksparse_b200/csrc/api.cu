@@ -1028,4 +1028,62 @@ int bsmm_ema(int n, void* const* emas, int ema_dtype, const float* const* params
         return check_launch("mt_ema_f16");
       });
 }
+
+size_t bsmm_adafactor_workspace_bytes(int n, const long long* rows, const long long* cols) {
+  if (n < 0 || (n && (!rows || !cols))) return 0;
+  long long floats = 0;
+  for (int i = 0; i < n; ++i) {
+    if (rows[i] < 0 || cols[i] < 0) return 0;
+    floats += af_ws_floats(rows[i], cols[i]);
+  }
+  return (size_t)floats * sizeof(float);
+}
+
+int bsmm_adafactor(int n, const void* const* grads, const int* grad_dtypes, float* const* params, float* const* cvs,
+                   float* const* rvs, const long long* rows, const long long* cols, const float* norm_scale, float lr,
+                   float decay, float epsilon, float grad_scale, float clip_thresh, float saturate, int zero_infs,
+                   int zero_nans, void* workspace, void* stream) {
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_adafactor: n = %d", n);
+  if (n && (!grads || !grad_dtypes || !params || !cvs || !rows || !cols))
+    return fail(BSMM_E_ARG, "bsmm_adafactor: null array");
+  bool any = false;
+  for (int i = 0; i < n; ++i) {
+    const long long C = rows[i], K = cols[i];
+    if (C < 0 || K < 0) return fail(BSMM_E_ARG, "bsmm_adafactor: tensor %d has shape (%lld, %lld)", i, C, K);
+    if (!dense_dtype_ok(grad_dtypes[i]))
+      return fail(BSMM_E_ARG, "bsmm_adafactor: tensor %d has unsupported grad dtype code %d", i, grad_dtypes[i]);
+    if (C > 1 && K > LLONG_MAX / C) return fail(BSMM_E_ARG, "bsmm_adafactor: tensor %d: (%lld, %lld) overflows", i, C, K);
+    if (C * K == 0) continue;
+    if (af_tiles(C, K) > 0x7fffffffLL || (C > 1 && (C + K + AF_FIN - 1) / AF_FIN > 0x7fffffffLL))
+      return fail(BSMM_E_LIMIT, "bsmm_adafactor: tensor %d of (%lld, %lld) exceeds the grid", i, C, K);
+    if (!grads[i] || !params[i] || !cvs[i] || (C > 1 && (!rvs || !rvs[i])))
+      return fail(BSMM_E_ARG, "bsmm_adafactor: tensor %d has a null pointer", i);
+    any = true;
+  }
+  if (!any) return 0;
+  if (!workspace) return fail(BSMM_E_ARG, "bsmm_adafactor: null workspace");
+  const AfConsts k = {norm_scale, static_cast<float*>(workspace), lr, decay, epsilon, grad_scale, clip_thresh, saturate,
+                      zero_infs, zero_nans};
+  const cudaStream_t s = (cudaStream_t)stream;
+  return af_for_launches(n, rows, cols,
+      [&](int i, AfTensor& t) {
+        t.g = grads[i]; t.p = params[i]; t.cv = cvs[i]; t.rv = rows[i] > 1 ? rvs[i] : nullptr;
+        t.dtype = (uint8_t)grad_dtypes[i];
+        t.vec = aligned16(t.g) && aligned16(t.p) && aligned16(t.cv) && (rows[i] == 1 || cols[i] % 4 == 0);
+      },
+      [&](const AfTable& tab, int tiles, int fins) {
+        mt_adafactor_stats<<<tiles, AF_THREADS, 0, s>>>(tab, k);
+        if (int e = check_launch("mt_adafactor_stats")) return e;
+        if (fins) {
+          mt_adafactor_finish<<<fins, AF_FIN, 0, s>>>(tab, k);
+          if (int e = check_launch("mt_adafactor_finish")) return e;
+          mt_adafactor_sumsq<<<tiles, AF_THREADS, 0, s>>>(tab, k);
+          if (int e = check_launch("mt_adafactor_sumsq")) return e;
+        }
+        mt_adafactor_rate<<<tab.n, AF_THREADS, 0, s>>>(tab, k);
+        if (int e = check_launch("mt_adafactor_rate")) return e;
+        mt_adafactor_apply<<<tiles, AF_THREADS, 0, s>>>(tab, k);
+        return check_launch("mt_adafactor_apply");
+      });
+}
 }  // extern "C"

@@ -332,4 +332,388 @@ inline int mt_for_launches(int n, const long long* sizes, Fill&& fill, Launch&& 
   return 0;
 }
 
+// ---- Adafactor (the reference's optimize_op_gpu.cu:8-365) -------------------------------------------------------------
+// A (C, K) param with C > 1 keeps rv[C] and cv[K] (factored); any other keeps cv per element. One step is five launches per
+// table of tensors:
+//   1. mt_adafactor_stats   per tile of a factored grad: the tile's row and column sums of g^2 + eps into the workspace;
+//                           per chunk of an unfactored one: cv updated in place and the chunk's sum of x^2
+//   2. mt_adafactor_finish  per entry of rv / cv: its partials added in fp64 in tile order, then the decayed update
+//   3. mt_adafactor_sumsq   per tile of a factored grad: the sum of g^2 / (rv[c] cv[k]), read again from the grad
+//   4. mt_adafactor_rate    per tensor: mean(rv), rms = mean(rv) mean(g^2 / (rv cv)) (or mean(x^2)), the update rate
+//   5. mt_adafactor_apply   per tile: the grad read a third time, x formed again, p -= rate x
+// x is never stored: the workspace holds partial sums and two scalars per tensor. Every sum has a fixed partition and
+// order (no atomics), so two calls give the same bits. A factored tile is AF_TR rows by AF_TK columns; warp w takes rows
+// w, w + 8, ... and each lane 4 columns of them, so a lane keeps its column sums (and 1 / sqrt(cv)) in registers.
+constexpr int AF_MAX = 384;          // tensors per launch: 384 * 72 bytes of table + AfConsts stay under 32,764 bytes
+constexpr int AF_THREADS = 256;
+constexpr int AF_WARPS = AF_THREADS / 32;
+constexpr int AF_TR = 64;
+constexpr int AF_TK = 128;
+constexpr int AF_CHUNK = AF_TR * AF_TK;       // elements per CTA of an unfactored tensor
+constexpr int AF_FIN = 256;                   // rv / cv entries per CTA of the finish pass
+
+struct AfTensor {
+  const void* g;
+  float* p;
+  float* cv;
+  float* rv;                         // NULL: unfactored
+  long long rows, cols;              // factored: C > 1 and K; unfactored: 1 and the size
+  long long ws;                      // first workspace float of this tensor
+  int tile0;                         // first tile (passes 1, 3 and 5) of this tensor within the launch
+  int fin0;                          // first CTA of the finish pass (factored tensors only)
+  uint8_t dtype, vec, pad[6];        // dtype of g; 16-byte accesses (every pointer aligned and K % 4 == 0)
+};
+static_assert(sizeof(AfTensor) == 72, "table entry layout");
+
+struct AfTable {
+  AfTensor t[AF_MAX];
+  int n;
+};
+
+struct AfConsts {
+  const float* norm_scale;
+  float* ws;
+  float lr, decay, epsilon, grad_scale, clip_thresh, saturate;
+  int zero_infs, zero_nans;
+};
+static_assert(sizeof(AfTable) + sizeof(AfConsts) <= 32764, "the table must fit the kernel parameters");
+
+// Workspace floats of a tensor, from its first: [0] mean(rv), [1] update rate, then one sum of squares per tile, then
+// (factored) the row partials [tile column][C] and the column partials [tile row][K].
+__host__ __device__ inline long long af_tile_rows(long long C) { return (C + AF_TR - 1) / AF_TR; }
+__host__ __device__ inline long long af_tile_cols(long long K) { return (K + AF_TK - 1) / AF_TK; }
+__host__ __device__ inline long long af_tiles(long long rows, long long cols) {
+  return rows > 1 ? af_tile_rows(rows) * af_tile_cols(cols) : (cols + AF_CHUNK - 1) / AF_CHUNK;
+}
+__host__ __device__ inline long long af_ws_floats(long long rows, long long cols) {
+  if (rows * cols == 0) return 0;
+  const long long tiles = af_tiles(rows, cols);
+  return 2 + tiles + (rows > 1 ? rows * af_tile_cols(cols) + af_tile_rows(rows) * cols : 0);
+}
+
+__device__ __forceinline__ int af_find_tile(const AfTable& tab, int b) {
+  int lo = 0, hi = tab.n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (tab.t[mid].tile0 <= b) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+// Unfactored tensors have no finish CTAs and share fin0 with the next tensor: the last tensor at or below b owns b.
+__device__ __forceinline__ int af_find_fin(const AfTable& tab, int b) {
+  int lo = 0, hi = tab.n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (tab.t[mid].fin0 <= b) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+__device__ __forceinline__ float af_norm_scale(const AfConsts& k) { return k.norm_scale ? *k.norm_scale : 1.f; }
+
+// Column of a lane's j-th element in a factored tile: 4 adjacent ones with 16-byte accesses, a stride of 32 without.
+template <bool VEC>
+__device__ __forceinline__ long long af_col(long long k0, int lane, int j) { return VEC ? k0 + 4 * lane + j : k0 + lane + 32 * j; }
+
+// The 4 elements of row `row` a lane owns (0 past the last column), converted to fp32.
+template <typename T, bool VEC>
+__device__ __forceinline__ void af_ld_row(const void* p, long long row, long long K, long long k0, int lane, float* v) {
+  if constexpr (VEC) {
+    if (af_col<true>(k0, lane, 0) < K) { Io<T>::ldv(p, row * K + af_col<true>(k0, lane, 0), v); return; }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = 0.f;
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long long c = af_col<false>(k0, lane, j);
+      v[j] = c < K ? Io<T>::ld1(p, row * K + c) : 0.f;
+    }
+  }
+}
+
+template <bool VEC>
+__device__ __forceinline__ void af_st_row(float* p, long long row, long long K, long long k0, int lane, const float* v) {
+  if constexpr (VEC) {
+    if (af_col<true>(k0, lane, 0) < K) Io<float>::stv(p, row * K + af_col<true>(k0, lane, 0), v);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long long c = af_col<false>(k0, lane, j);
+      if (c < K) p[row * K + c] = v[j];
+    }
+  }
+}
+
+// Elements [c0, c1) of an unfactored chunk: MT_VEC at a time with 16-byte accesses, then the scalar tail.
+template <bool VEC, typename F>
+__device__ __forceinline__ void af_walk(long long c0, long long c1, F&& body) {
+  long long i = c0 + (long long)threadIdx.x * (VEC ? MT_VEC : 1);
+  if (VEC) {
+    const long long body_end = c0 + ((c1 - c0) & ~(long long)(MT_VEC - 1));
+    for (; i < body_end; i += AF_THREADS * MT_VEC) body(i, std::integral_constant<int, MT_VEC>());
+    i = body_end + threadIdx.x;
+  }
+  for (; i < c1; i += AF_THREADS) body(i, std::integral_constant<int, 1>());
+}
+
+// pass 1
+template <typename TG, bool VEC>
+__device__ __forceinline__ void af_stats(const AfTensor& t, long long tile, const AfConsts& k, float scale, float* red) {
+  float* ws = k.ws + t.ws;
+  if (!t.rv) {
+    const long long c0 = tile * AF_CHUNK, c1 = min(c0 + AF_CHUNK, t.cols);
+    float acc = 0.f;
+    af_walk<VEC>(c0, c1, [&](long long i, auto w) {
+      constexpr int W = decltype(w)::value;
+      float g[W], v[W];
+      mt_ld<TG, W>(t.g, i, g);
+      mt_ld<float, W>(t.cv, i, v);
+#pragma unroll
+      for (int j = 0; j < W; ++j) {
+        const float gj = mt_condition(g[j], k.saturate, k.zero_infs, k.zero_nans) * scale;
+        v[j] = k.decay * v[j] + (1.f - k.decay) * (gj * gj + k.epsilon);
+        const float x = gj * rsqrtf(v[j]);
+        acc = fmaf(x, x, acc);
+      }
+      mt_st<float, W>(t.cv, i, v);
+    });
+    acc = block_sum_fixed<float, AF_THREADS>(acc, red);
+    if (threadIdx.x == 0) ws[2 + tile] = acc;
+    return;
+  }
+  const long long C = t.rows, K = t.cols, ntc = af_tile_cols(K);
+  const long long tr = tile / ntc, tc = tile - tr * ntc;
+  const long long r0 = tr * AF_TR, r1 = min(r0 + AF_TR, C), k0 = tc * AF_TK;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float* rowpart = ws + 2 + af_tiles(C, K) + tc * C;
+  float* colpart = ws + 2 + af_tiles(C, K) + C * ntc + tr * K;
+  float col[4] = {0.f, 0.f, 0.f, 0.f};
+  for (long long r = r0 + warp; r < r1; r += AF_WARPS) {
+    float g[4];
+    af_ld_row<TG, VEC>(t.g, r, K, k0, lane, g);
+    float rs = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float gj = mt_condition(g[j], k.saturate, k.zero_infs, k.zero_nans) * scale;
+      const float s = af_col<VEC>(k0, lane, j) < K ? gj * gj + k.epsilon : 0.f;
+      col[j] += s;
+      rs += s;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) rs += __shfl_xor_sync(0xffffffffu, rs, o);
+    if (lane == 0) rowpart[r] = rs;
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) red[warp * AF_TK + (int)(af_col<VEC>(0, lane, j))] = col[j];
+  __syncthreads();
+  if (threadIdx.x < AF_TK && k0 + threadIdx.x < K) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < AF_WARPS; ++w) s += red[w * AF_TK + threadIdx.x];
+    colpart[k0 + threadIdx.x] = s;
+  }
+}
+
+template <typename TG>
+__device__ __forceinline__ void af_stats_vec(const AfTensor& t, long long tile, const AfConsts& k, float scale, float* red) {
+  if (t.vec) af_stats<TG, true>(t, tile, k, scale, red); else af_stats<TG, false>(t, tile, k, scale, red);
+}
+
+__global__ void __launch_bounds__(AF_THREADS) mt_adafactor_stats(const __grid_constant__ AfTable tab, const AfConsts k) {
+  __shared__ float red[AF_WARPS * AF_TK];
+  const float ns = af_norm_scale(k);
+  if (ns == 0.f) return;                             // a non-finite global norm skips the step
+  const AfTensor& t = tab.t[af_find_tile(tab, blockIdx.x)];
+  const long long tile = blockIdx.x - t.tile0;
+  const float scale = k.grad_scale * ns;
+  switch (t.dtype) {
+    case BSMM_F32: af_stats_vec<float>(t, tile, k, scale, red); break;
+    case BSMM_F16: af_stats_vec<__half>(t, tile, k, scale, red); break;
+    default:       af_stats_vec<__nv_bfloat16>(t, tile, k, scale, red); break;
+  }
+}
+
+// pass 2: rv[c] = decay rv[c] + (1 - decay) (row sum) / K, cv[k] = decay cv[k] + (1 - decay) (column sum) / C
+__global__ void __launch_bounds__(AF_FIN) mt_adafactor_finish(const __grid_constant__ AfTable tab, const AfConsts k) {
+  if (af_norm_scale(k) == 0.f) return;
+  const AfTensor& t = tab.t[af_find_fin(tab, blockIdx.x)];
+  const long long C = t.rows, K = t.cols, ntc = af_tile_cols(K), ntr = af_tile_rows(C);
+  const long long e = (long long)(blockIdx.x - t.fin0) * AF_FIN + threadIdx.x;
+  const float* part = k.ws + t.ws + 2 + af_tiles(C, K);
+  if (e < C) {
+    double s = 0.0;
+    for (long long j = 0; j < ntc; ++j) s += (double)part[j * C + e];
+    t.rv[e] = k.decay * t.rv[e] + (1.f - k.decay) * (float)(s / (double)K);
+  } else if (e < C + K) {
+    const long long c = e - C;
+    part += C * ntc;
+    double s = 0.0;
+    for (long long i = 0; i < ntr; ++i) s += (double)part[i * K + c];
+    t.cv[c] = k.decay * t.cv[c] + (1.f - k.decay) * (float)(s / (double)C);
+  }
+}
+
+// pass 3: sum of (g / sqrt(rv[c] cv[k]))^2 over a factored tile
+template <typename TG, bool VEC>
+__device__ __forceinline__ float af_sumsq(const AfTensor& t, long long tile, const AfConsts& k, float scale) {
+  const long long C = t.rows, K = t.cols, ntc = af_tile_cols(K);
+  const long long tr = tile / ntc, tc = tile - tr * ntc;
+  const long long r0 = tr * AF_TR, r1 = min(r0 + AF_TR, C), k0 = tc * AF_TK;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float rc[4];
+  af_ld_row<float, VEC>(t.cv, 0, K, k0, lane, rc);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) rc[j] = af_col<VEC>(k0, lane, j) < K ? rsqrtf(rc[j]) : 0.f;
+  float acc = 0.f;
+  for (long long r = r0 + warp; r < r1; r += AF_WARPS) {
+    float g[4];
+    af_ld_row<TG, VEC>(t.g, r, K, k0, lane, g);
+    const float rr = rsqrtf(t.rv[r]);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float y = mt_condition(g[j], k.saturate, k.zero_infs, k.zero_nans) * scale * rr * rc[j];
+      acc = fmaf(y, y, acc);
+    }
+  }
+  return acc;
+}
+
+__global__ void __launch_bounds__(AF_THREADS) mt_adafactor_sumsq(const __grid_constant__ AfTable tab, const AfConsts k) {
+  __shared__ float red[AF_WARPS];
+  const float ns = af_norm_scale(k);
+  if (ns == 0.f) return;
+  const AfTensor& t = tab.t[af_find_tile(tab, blockIdx.x)];
+  if (!t.rv) return;                                 // unfactored: pass 1 wrote the partials
+  const long long tile = blockIdx.x - t.tile0;
+  const float scale = k.grad_scale * ns;
+  float acc;
+  switch (t.dtype * 2 + t.vec) {
+    case BSMM_F32 * 2:      acc = af_sumsq<float, false>(t, tile, k, scale); break;
+    case BSMM_F32 * 2 + 1:  acc = af_sumsq<float, true>(t, tile, k, scale); break;
+    case BSMM_F16 * 2:      acc = af_sumsq<__half, false>(t, tile, k, scale); break;
+    case BSMM_F16 * 2 + 1:  acc = af_sumsq<__half, true>(t, tile, k, scale); break;
+    case BSMM_BF16 * 2:     acc = af_sumsq<__nv_bfloat16, false>(t, tile, k, scale); break;
+    default:                acc = af_sumsq<__nv_bfloat16, true>(t, tile, k, scale); break;
+  }
+  acc = block_sum_fixed<float, AF_THREADS>(acc, red);
+  if (threadIdx.x == 0) k.ws[t.ws + 2 + tile] = acc;
+}
+
+// pass 4: one CTA per tensor. rate = lr / max(1, sqrt(rms) / clip_thresh), rms = mean(x^2).
+__global__ void __launch_bounds__(AF_THREADS) mt_adafactor_rate(const __grid_constant__ AfTable tab, const AfConsts k) {
+  __shared__ double red[AF_WARPS];
+  if (af_norm_scale(k) == 0.f) return;
+  const AfTensor& t = tab.t[blockIdx.x];
+  float* ws = k.ws + t.ws;
+  const long long tiles = af_tiles(t.rows, t.cols);
+  double sq = 0.0, rvs = 0.0;
+  for (long long i = threadIdx.x; i < tiles; i += AF_THREADS) sq += (double)ws[2 + i];
+  sq = block_sum_fixed<double, AF_THREADS>(sq, red);
+  __syncthreads();                                   // red is reused
+  if (t.rv) {
+    for (long long i = threadIdx.x; i < t.rows; i += AF_THREADS) rvs += (double)t.rv[i];
+    rvs = block_sum_fixed<double, AF_THREADS>(rvs, red);
+  }
+  if (threadIdx.x == 0) {
+    const double n = (double)t.rows * (double)t.cols;
+    const float rv_mean = t.rv ? (float)(rvs / (double)t.rows) : 1.f;
+    const double rms = t.rv ? (double)rv_mean * sq / n : sq / n;
+    ws[0] = rv_mean;
+    ws[1] = (float)((double)k.lr / fmax(1.0, sqrt(rms) / (double)k.clip_thresh));
+  }
+}
+
+// pass 5: p -= rate * x, x = g / sqrt(rv[c] / mean(rv)) / sqrt(cv[k]) or g / sqrt(cv)
+template <typename TG, bool VEC>
+__device__ __forceinline__ void af_apply(const AfTensor& t, long long tile, const AfConsts& k, float scale) {
+  const float* ws = k.ws + t.ws;
+  const float rate = ws[1];
+  if (!t.rv) {
+    const long long c0 = tile * AF_CHUNK, c1 = min(c0 + AF_CHUNK, t.cols);
+    af_walk<VEC>(c0, c1, [&](long long i, auto w) {
+      constexpr int W = decltype(w)::value;
+      float g[W], v[W], p[W];
+      mt_ld<TG, W>(t.g, i, g);
+      mt_ld<float, W>(t.cv, i, v);
+      mt_ld<float, W>(t.p, i, p);
+#pragma unroll
+      for (int j = 0; j < W; ++j) {
+        const float gj = mt_condition(g[j], k.saturate, k.zero_infs, k.zero_nans) * scale;
+        p[j] -= rate * (gj * rsqrtf(v[j]));
+      }
+      mt_st<float, W>(t.p, i, p);
+    });
+    return;
+  }
+  const float rv_mean = ws[0];
+  const long long C = t.rows, K = t.cols, ntc = af_tile_cols(K);
+  const long long tr = tile / ntc, tc = tile - tr * ntc;
+  const long long r0 = tr * AF_TR, r1 = min(r0 + AF_TR, C), k0 = tc * AF_TK;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float rc[4];
+  af_ld_row<float, VEC>(t.cv, 0, K, k0, lane, rc);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) rc[j] = af_col<VEC>(k0, lane, j) < K ? rsqrtf(rc[j]) : 0.f;
+  for (long long r = r0 + warp; r < r1; r += AF_WARPS) {
+    float g[4], p[4];
+    af_ld_row<TG, VEC>(t.g, r, K, k0, lane, g);
+    af_ld_row<float, VEC>(t.p, r, K, k0, lane, p);
+    const float rr = rsqrtf(t.rv[r] / rv_mean);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float gj = mt_condition(g[j], k.saturate, k.zero_infs, k.zero_nans) * scale;
+      p[j] -= rate * (gj * rr * rc[j]);
+    }
+    af_st_row<VEC>(t.p, r, K, k0, lane, p);
+  }
+}
+
+__global__ void __launch_bounds__(AF_THREADS) mt_adafactor_apply(const __grid_constant__ AfTable tab, const AfConsts k) {
+  const float ns = af_norm_scale(k);
+  if (ns == 0.f) return;
+  const AfTensor& t = tab.t[af_find_tile(tab, blockIdx.x)];
+  const long long tile = blockIdx.x - t.tile0;
+  const float scale = k.grad_scale * ns;
+  switch (t.dtype * 2 + t.vec) {
+    case BSMM_F32 * 2:      af_apply<float, false>(t, tile, k, scale); break;
+    case BSMM_F32 * 2 + 1:  af_apply<float, true>(t, tile, k, scale); break;
+    case BSMM_F16 * 2:      af_apply<__half, false>(t, tile, k, scale); break;
+    case BSMM_F16 * 2 + 1:  af_apply<__half, true>(t, tile, k, scale); break;
+    case BSMM_BF16 * 2:     af_apply<__nv_bfloat16, false>(t, tile, k, scale); break;
+    default:                af_apply<__nv_bfloat16, true>(t, tile, k, scale); break;
+  }
+}
+
+// Splits the non-empty tensors into tables of at most AF_MAX tensors, 2^31 - 1 tiles and 2^31 - 1 finish CTAs;
+// fill(i, entry) sets the pointers and flags of tensor i, launch(table, tiles, finish CTAs) enqueues the five passes.
+template <typename Fill, typename Launch>
+inline int af_for_launches(int n, const long long* rows, const long long* cols, Fill&& fill, Launch&& launch) {
+  AfTable tab;
+  tab.n = 0;
+  long long tiles = 0, fins = 0, ws = 0;
+  for (int i = 0; i <= n; ++i) {
+    const bool live = i < n && rows[i] * cols[i] > 0;
+    const long long c = live ? af_tiles(rows[i], cols[i]) : 0;
+    const long long f = live && rows[i] > 1 ? (rows[i] + cols[i] + AF_FIN - 1) / AF_FIN : 0;
+    if (tab.n && (i == n || tab.n == AF_MAX || tiles + c > 0x7fffffffLL || fins + f > 0x7fffffffLL)) {
+      if (int e = launch(tab, (int)tiles, (int)fins)) return e;
+      tab.n = 0;
+      tiles = fins = 0;
+    }
+    if (!live) continue;
+    AfTensor& t = tab.t[tab.n++];
+    t = AfTensor{};
+    t.rows = rows[i];
+    t.cols = cols[i];
+    t.ws = ws;
+    t.tile0 = (int)tiles;
+    t.fin0 = (int)fins;
+    fill(i, t);
+    tiles += c;
+    fins += f;
+    ws += af_ws_floats(rows[i], cols[i]);
+  }
+  return 0;
+}
+
 }  // namespace bsmm

@@ -1,6 +1,7 @@
 """The reference's blocksparse/optimize.py on torch tensors.
 
   AdamOptimizer(params, learning_rate, beta1, beta2, ...)   torch optimizer; gated and 16-bit-moment Adam (:20-110)
+  AdafactorOptimizer(params, learning_rate, beta2, ...)     torch optimizer; factored second moments (:113-191)
   clip_by_global_norm(grads, clip_norm, ...) / global_norm / ClipGlobalNorm   device norm and clip scale (:197-225)
   Ema(decay, gated, fp16)                                   parameter moving averages (:231-289)
 
@@ -111,6 +112,15 @@ def _gate_of(p, gated):
     return gate, p.shape[1]
 
 
+def _check_capture(opt, rate, group, *powers):
+    """Under CUDA graph capture, refuses a group whose powers are not all 0: the bias-corrected `rate` the host forms
+    from them is a kernel argument and would be replayed unchanged while they advance."""
+    if torch.cuda.is_current_stream_capturing() and any(group[k] != 0.0 for k in powers):
+        raise ValueError("%s.step under CUDA graph capture: the bias-corrected %s is a kernel argument and would be "
+                         "replayed unchanged while %s (%s) advance; capture needs zero_init_variables=True"
+                         % (opt, rate, " / ".join(powers), ", ".join(repr(group[k]) for k in powers)))
+
+
 def _check_qspec(**qspecs):
     for k, v in qspecs.items():
         if v is not None:
@@ -187,13 +197,8 @@ class AdamOptimizer(torch.optim.Optimizer):
         every = [p for group in self.param_groups for p in group["params"]]
         if grads is not None and len(grads) != len(every):
             raise ValueError("AdamOptimizer.step: %d grads for %d params" % (len(grads), len(every)))
-        if torch.cuda.is_current_stream_capturing():
-            for group in self.param_groups:
-                if group["beta1_power"] != 0.0 or group["beta2_power"] != 0.0:
-                    raise ValueError("AdamOptimizer.step under CUDA graph capture: the bias-corrected lr_t is a kernel "
-                                     "argument and would be replayed unchanged while beta1_power / beta2_power (%r, %r) "
-                                     "advance; capture needs zero_init_variables=True"
-                                     % (group["beta1_power"], group["beta2_power"]))
+        for group in self.param_groups:
+            _check_capture("AdamOptimizer", "lr_t", group, "beta1_power", "beta2_power")
         k = 0
         lib = _lib.load()
         f32 = np.float32
@@ -237,6 +242,124 @@ class AdamOptimizer(torch.optim.Optimizer):
                 _lib.check(rc, "bsmm_adam")
             group["beta1_power"] = float(b1p * f32(self.beta1))                        # optimize.py:104-110
             group["beta2_power"] = float(b2p * f32(self.beta2))
+        return loss
+
+
+class AdafactorOptimizer(torch.optim.Optimizer):
+    """The reference's AdafactorOptimizer (optimize.py:113-191) as a torch optimizer, on the multi-tensor kernels of
+    csrc/optimize.cuh: five launches per device (per 384 params) whatever the number of params.
+
+    params: fp32 contiguous CUDA tensors of rank 1 or 2. A (C, K) param with C > 1 keeps one fp32 second moment per row
+    and one per column (state "rv" [C] and "cv" [K]); rank 1 and (1, K) keep one per element (state "cv"). Any other
+    rank raises ValueError, so block-sparse (blocks, bs, bs) weights are refused. Each step, per element:
+        g = grad_scale * norm_scale * sat(zero_nans(zero_infs(grad)))
+        factored:   rv = decay rv + (1 - decay) mean_k(g^2 + eps);  cv = decay cv + (1 - decay) mean_c(g^2 + eps)
+                    x = g / sqrt(rv[c] / mean(rv)) / sqrt(cv[k])
+        unfactored: cv = decay cv + (1 - decay) (g^2 + eps);  x = g / sqrt(cv)
+        p -= lr x / max(1, sqrt(mean(x^2)) / clip_thresh)
+    decay = beta2 (1 - decay1_power) / (1 - decay2_power) is formed on the host in fp32; the powers start at beta2 and
+    beta2^2 (0 with zero_init_variables), are multiplied by beta2 after every step and live in each param group next to
+    "lr", so they travel with state_dict(). param_groups[i]["lr"] is the learning rate, so torch LR schedulers apply.
+
+    x is never stored: the kernels form it again from the grad, and the only temporary is a workspace of partial sums
+    (about 2.4 % of the grad's element count for a factored param). Every sum has a fixed order, so a step is bitwise
+    reproducible. norm_scale, step(grads=...), multi-device params and CUDA graph capture work as in AdamOptimizer:
+    norm_scale 0 leaves params and state unchanged bit for bit (the powers still advance), and a step under capture
+    needs zero_init_variables=True."""
+
+    def __init__(self, params, learning_rate=5e-4, beta2=0.999, epsilon=1e-30, clip_thresh=1.0, norm_scale=None,
+                 grad_scale=1.0, saturate=0.0, zero_infs=False, zero_nans=False, name="Adafactor",
+                 zero_init_variables=False):
+        if norm_scale is not None:
+            _dev_scalar(norm_scale, "norm_scale")
+        b2 = np.float32(beta2)
+        d1, d2 = (0.0, 0.0) if zero_init_variables else (float(b2), float(b2 * b2))
+        super().__init__(params, dict(lr=learning_rate, decay1_power=d1, decay2_power=d2))
+        self.beta2, self.epsilon, self.clip_thresh = beta2, epsilon, clip_thresh
+        self.norm_scale, self.grad_scale, self.saturate = norm_scale, grad_scale, saturate
+        self.zero_infs, self.zero_nans, self.name = zero_infs, zero_nans, name
+        for group in self.param_groups:
+            for p in group["params"]:
+                if not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous():
+                    raise ValueError("AdafactorOptimizer: params must be contiguous float32 CUDA tensors, got %s on %s"
+                                     % (p.dtype, p.device))
+                if p.dim() not in (1, 2):
+                    raise ValueError("AdafactorOptimizer: only 1 or 2-d params are supported, got shape %s"
+                                     % (tuple(p.shape),))
+
+    @staticmethod
+    def _rows(p):
+        """C of a factored param, 1 otherwise."""
+        return p.shape[0] if p.dim() == 2 and p.shape[0] > 1 else 1
+
+    def _moments(self, p):
+        st = self.state[p]
+        if "cv" not in st:
+            if self._rows(p) > 1:
+                st["cv"] = torch.zeros(p.shape[1], dtype=torch.float32, device=p.device)
+                st["rv"] = torch.zeros(p.shape[0], dtype=torch.float32, device=p.device)
+            else:
+                st["cv"] = torch.zeros(p.numel(), dtype=torch.float32, device=p.device)
+        return st["cv"], st.get("rv")
+
+    @torch.no_grad()
+    def step(self, closure=None, norm_scale=None, grads=None):
+        """One Adafactor step over every param that has a gradient: `grads[i]` (fp32, fp16 or bf16, aligned with the
+        params of all groups in order) when given, else param.grad. norm_scale overrides the constructor's. Every
+        argument is checked before anything is launched."""
+        loss = None
+        if closure is not None:
+            with torch.enable_grad():
+                loss = closure()
+        ns = self.norm_scale if norm_scale is None else _dev_scalar(norm_scale, "norm_scale")
+        every = [p for group in self.param_groups for p in group["params"]]
+        if grads is not None and len(grads) != len(every):
+            raise ValueError("AdafactorOptimizer.step: %d grads for %d params" % (len(grads), len(every)))
+        for group in self.param_groups:
+            _check_capture("AdafactorOptimizer", "decay", group, "decay1_power", "decay2_power")
+        k = 0
+        plan = []                    # per group: device -> the step's tables for the params on it, in param order
+        for group in self.param_groups:
+            per_dev = {}
+            for p in group["params"]:
+                g = grads[k] if grads is not None else p.grad
+                k += 1
+                if g is None:
+                    continue
+                if not torch.is_tensor(g) or g.shape != p.shape or g.device != p.device:
+                    raise ValueError("AdafactorOptimizer.step: grad %s on %s for param %s on %s"
+                                     % (tuple(getattr(g, "shape", ())), getattr(g, "device", None), tuple(p.shape),
+                                        p.device))
+                gd = _lib.dtype_code(g.dtype)
+                if p.numel() == 0:
+                    continue
+                per_dev.setdefault(p.device, []).append((p, g, gd))
+            plan.append((group, per_dev))
+        lib = _lib.load()
+        f32 = np.float32
+        for group, per_dev in plan:
+            d1, d2 = f32(group["decay1_power"]), f32(group["decay2_power"])
+            b2 = f32(self.beta2)
+            decay = b2 * (f32(1) - d1) / (f32(1) - d2)                               # optimize.py:140
+            for dev, items in per_dev.items():
+                gs = [g.contiguous() for _, g, _ in items]
+                ps = [p for p, _, _ in items]
+                cvs, rvs = zip(*[self._moments(p) for p in ps])
+                rows = _i64([self._rows(p) for p in ps])
+                cols = _i64([p.numel() // self._rows(p) for p in ps])
+                arrs = (_ptrs(gs), _i32([gd for _, _, gd in items]), _ptrs(ps), _ptrs(cvs),
+                        np.array([0 if r is None else r.data_ptr() for r in rvs], dtype=np.uint64), rows, cols)
+                with torch.cuda.device(dev):
+                    ns_dev = ns if ns is None or ns.device == dev else ns.to(dev)
+                    nbytes = lib.bsmm_adafactor_workspace_bytes(len(ps), rows.ctypes.data, cols.ctypes.data)
+                    ws = torch.empty(nbytes // 4, dtype=torch.float32, device=dev)
+                    rc = lib.bsmm_adafactor(len(ps), *[a.ctypes.data for a in arrs], _lib.ptr(ns_dev), float(group["lr"]),
+                                            float(decay), float(self.epsilon), float(self.grad_scale),
+                                            float(self.clip_thresh), float(self.saturate), int(self.zero_infs),
+                                            int(self.zero_nans), ws.data_ptr(), _lib.stream_ptr())
+                _lib.check(rc, "bsmm_adafactor")
+            group["decay1_power"] = float(d1 * b2)                                    # optimize.py:185-191
+            group["decay2_power"] = float(d2 * b2)
         return loss
 
 

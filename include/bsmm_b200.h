@@ -46,6 +46,8 @@
  *   bsmm_global_norm      <- ClipGlobalNormOp: ReduceSumSquared per tensor + ComputeClipNorm
  *                            (src/optimize_op.cc:771-858, src/optimize_op_gpu.cu:1102-1238)
  *   bsmm_ema              <- EmaOp: ApplyEma / ApplyEmaGated (src/optimize_op.cc:463-529)
+ *   bsmm_adafactor        <- Adafactor2dOp / Adafactor1dOp: Adafactor<T,V> per tensor
+ *                            (src/optimize_op.cc:21-212, src/optimize_op_gpu.cu:8-365)
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer except `err` strings is DEVICE memory
@@ -554,6 +556,33 @@ size_t bsmm_global_norm_workspace_bytes(int n, const long long* sizes);
  * mt_ema (fp32) and mt_ema_f16. */
 int bsmm_ema(int n, void* const* emas, int ema_dtype, const float* const* params, const long long* sizes,
              const float* const* gates, const int* bsizes, float decay, void* stream);
+
+/*
+ * One Adafactor step in place (optimize_op.cc Adafactor2dOp / Adafactor1dOp, launcher Adafactor in
+ * optimize_op_gpu.cu:311-359). Tensor i is a (rows[i], cols[i]) fp32 param with a grad of grad_dtypes[i]. Every element
+ * is conditioned as in bsmm_adam: g = grad_scale * norm_scale * sat(zero_nans(zero_infs(grad))).
+ *   rows[i] > 1 (factored; rvs[i] has rows[i] floats, cvs[i] cols[i]):
+ *     rv[c] = decay rv[c] + (1 - decay) mean_k(g^2 + epsilon);  cv[k] = decay cv[k] + (1 - decay) mean_c(g^2 + epsilon)
+ *     x = g / sqrt(rv[c] / mean_c(rv)) / sqrt(cv[k])
+ *   rows[i] == 1 (unfactored; cvs[i] has cols[i] floats, rvs[i] is not read):
+ *     cv = decay cv + (1 - decay) (g^2 + epsilon);  x = g / sqrt(cv)
+ *   then rms = mean(x^2) over the tensor and p -= lr x / max(1, sqrt(rms) / clip_thresh).
+ * decay is the bias-corrected rate the host forms. norm_scale is a device fp32 scalar (NULL = 1); when it is 0 the
+ * kernels return without touching anything. rvs may be NULL when no tensor is factored.
+ * Five launches per table of up to 384 tensors (mt_adafactor_stats, _finish, _sumsq, _rate, _apply; see DESIGN.md 7e):
+ * x is formed again from the grad where needed, never stored. workspace (at least bsmm_adafactor_workspace_bytes(n, rows,
+ * cols) bytes, uninitialised) takes per-tile row, column and square sums and two scalars per tensor; every sum is added
+ * in an order fixed by the shapes, without atomics, so the result is bitwise reproducible. Element offsets are 64-bit;
+ * 16-byte accesses are used where every pointer of a tensor is 16-byte aligned and cols[i] % 4 == 0 (or rows[i] == 1).
+ * n < 0, a negative rows / cols, a bad dtype, a null array or a null pointer of a non-empty tensor: BSMM_E_ARG before any
+ * launch. Empty tensors are skipped; with nothing left, nothing is launched and workspace may be NULL.
+ */
+int bsmm_adafactor(int n, const void* const* grads, const int* grad_dtypes, float* const* params, float* const* cvs,
+                   float* const* rvs, const long long* rows, const long long* cols, const float* norm_scale, float lr,
+                   float decay, float epsilon, float grad_scale, float clip_thresh, float saturate, int zero_infs,
+                   int zero_nans, void* workspace, void* stream);
+/* Bytes of workspace bsmm_adafactor needs for these shapes; 0 for bad arguments. */
+size_t bsmm_adafactor_workspace_bytes(int n, const long long* rows, const long long* cols);
 
 /* ---- measurement helper (the reference's `bench` op attribute, op.cc:99-106) ---------
  * Records two events around whatever the caller enqueues between begin and end.      */

@@ -7,7 +7,8 @@ reference's transformer module (softmax, masked_softmax, masked_top_k_softmax, t
 softmax_cross_entropy, transpose_0213, transpose_2d), of its norms module (layer_norm) and of its optimize module
 (AdamOptimizer, clip_by_global_norm, global_norm, Ema; AdafactorOptimizer, importable from here and from
 blocksparse_b200.optimize but not listed in __all__), and of its ewops and embed modules (bias_relu, dropout,
-set_entropy, get_entropy, embedding_lookup; listed in ewops.__all__ and embed.__all__).
+set_entropy, get_entropy, embedding_lookup; listed in ewops.__all__ and embed.__all__), and of its lstm module
+(fused_lstm_gates, split4, concat4, sparse_relu; listed in lstm.__all__).
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
 from .optimize import (AdafactorOptimizer, AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay, blocksparse_norm,
@@ -17,6 +18,7 @@ from .transformer import (BlocksparseTransformer, masked_softmax, masked_top_k_s
 from .norms import layer_norm
 from .ewops import bias_relu, dropout, get_entropy, set_entropy
 from .embed import embedding_lookup
+from .lstm import concat4, fused_lstm_gates, sparse_relu, split4
 from .lut import z_order_2d
 from . import _lib
 

@@ -55,6 +55,11 @@ SIGNATURES = {
     "bsmm_bias_grad_workspace_bytes": (_c.c_size_t, [_i, _ll, _i]),
     "bsmm_dropout_mask": (_i, [_vp, _ll, _c.c_double, _vp, _vp]),
     "bsmm_dropout_apply": (_i, [_i, _vp, _vp, _vp, _i, _vp, _vp, _ll, _c.c_double, _vp]),
+    "bsmm_lstm_gates": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp, _vp, _vp, _ll, _i, _f, _vp]),
+    "bsmm_lstm_gates_grad": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i,
+                                  _f, _vp]),
+    "bsmm_sparse_relu": (_i, [_i, _vp, _vp, _ll, _i, _f, _vp]),
+    "bsmm_relu_mask_grad": (_i, [_i, _vp, _vp, _vp, _ll, _vp]),
     "bsmm_embedding_lookup": (_i, [_i, _i, _vp, _vp, _vp, _ll, _i, _i, _vp]),
     "bsmm_embedding_grad": (_i, [_i, _i, _vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
     "bsmm_embedding_grad_workspace_bytes": (_c.c_size_t, [_ll, _i, _i]),

@@ -261,3 +261,11 @@ def layer_norm_grad_test(dy, x, g, b, axis=1, segments=1, epsilon=1e-6, relu=Fal
     shape = (-1, 1) if axis == 0 else (1, -1)
     dt = np.result_type(x, np.float32)
     return (_segment_unview(dx, np.shape(x), axis).astype(dt), dg.reshape(shape).astype(dt), db.reshape(shape).astype(dt))
+
+
+def sparse_relu_test(x, alpha=1.0):
+    """y = max(x - (mean + alpha * std), 0) along the last axis, std the population standard deviation (the reference's
+    checker, lstm.py:111-117)."""
+    x = np.asarray(x)
+    cutoff = x.mean(axis=-1, keepdims=True) + alpha * x.std(axis=-1, keepdims=True)
+    return np.maximum(x - cutoff, 0.0)

@@ -8,6 +8,7 @@
 #include "ewops.cuh"
 #include "generic.cuh"
 #include "layer_norm.cuh"
+#include "lstm.cuh"
 #include "optimize.cuh"
 #include "softmax.cuh"
 #include "tc.cuh"
@@ -692,6 +693,77 @@ int bsmm_dropout_apply(int dtype, const void* x, const int32_t* mask, void* y, i
   const int V = 16 / dtype_size(dtype);
   const bool vec = aligned16(x) && aligned16(y) && (a.nd == 0 ? n : a.size[a.nd - 1]) % V == 0;
   BSMM_DISPATCH_DTYPE(dtype, T, { return launch_dropout_apply<T>(a, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+// ---- LSTM gates and sparse relu (csrc/lstm.cuh) ----------------------------------------------------------------------------
+static int lstm_args(const char* what, int dtype, int bdtype, long long N, int K, long long stride) {
+  if (!dense_dtype_ok(dtype) || !dense_dtype_ok(bdtype))
+    return fail(BSMM_E_ARG, "%s: unsupported dtype codes %d, %d", what, dtype, bdtype);
+  if (N < 0 || K <= 0 || stride < K) return fail(BSMM_E_ARG, "%s: bad sizes N %lld, K %d, stride %lld", what, N, K, stride);
+  if (N > LLONG_MAX / stride) return fail(BSMM_E_LIMIT, "%s: more than 2^63 elements", what);
+  return 0;
+}
+
+// 16-byte accesses when every pointer given is aligned and every row start stays so
+static bool lstm_vec(int dtype, int K, long long stride, std::initializer_list<const void*> ptrs) {
+  const int V = 16 / dtype_size(dtype);
+  if (K % V || stride % V) return false;
+  for (const void* p : ptrs)
+    if (p && !aligned16(p)) return false;
+  return true;
+}
+
+int bsmm_lstm_gates(int dtype, int bdtype, const void* c, const void* i, const void* u, const void* f, const void* o,
+                    long long stride, const void* bias, void* c_next, void* h_next, long long N, int K,
+                    float forget_bias, void* stream) {
+  if (int e = lstm_args("bsmm_lstm_gates", dtype, bdtype, N, K, stride)) return e;
+  if (!c || !i || !u || !f || !o || !c_next || !h_next) return fail(BSMM_E_ARG, "bsmm_lstm_gates: null pointer");
+  if (N == 0) return 0;
+  LstmArgs a = {};
+  a.c = c; a.g[0] = i; a.g[1] = u; a.g[2] = f; a.g[3] = o; a.bias = bias; a.c_out = c_next; a.h_out = h_next;
+  a.N = N; a.gs = stride; a.K = K; a.bdt = bdtype; a.forget_bias = forget_bias;
+  const bool vec = lstm_vec(dtype, K, stride, {c, i, u, f, o, c_next, h_next});
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_lstm_gates<T>(a, false, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_lstm_gates_grad(int dtype, int bdtype, const void* c, const void* i, const void* u, const void* f,
+                         const void* o, long long stride, const void* bias, const void* ec, const void* eh, void* dc,
+                         void* di, void* du, void* df, void* d_o, long long N, int K, float forget_bias, void* stream) {
+  if (int e = lstm_args("bsmm_lstm_gates_grad", dtype, bdtype, N, K, stride)) return e;
+  if (!c || !i || !u || !f || !o || !dc || !di || !du || !df || !d_o)
+    return fail(BSMM_E_ARG, "bsmm_lstm_gates_grad: null pointer");
+  if (N == 0) return 0;
+  LstmArgs a = {};
+  a.c = c; a.g[0] = i; a.g[1] = u; a.g[2] = f; a.g[3] = o; a.bias = bias; a.ec = ec; a.eh = eh; a.c_out = dc;
+  a.dg[0] = di; a.dg[1] = du; a.dg[2] = df; a.dg[3] = d_o;
+  a.N = N; a.gs = stride; a.K = K; a.bdt = bdtype; a.forget_bias = forget_bias;
+  const bool vec = lstm_vec(dtype, K, stride, {c, i, u, f, o, ec, eh, dc, di, du, df, d_o});
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_lstm_gates<T>(a, true, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_sparse_relu(int dtype, const void* x, void* y, long long N, int K, float alpha, void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_sparse_relu: unsupported dtype code %d", dtype);
+  if (N < 0 || K <= 0) return fail(BSMM_E_ARG, "bsmm_sparse_relu: bad sizes N %lld, K %d", N, K);
+  if (!x || !y) return fail(BSMM_E_ARG, "bsmm_sparse_relu: null pointer");
+  if (N > LLONG_MAX / K) return fail(BSMM_E_LIMIT, "bsmm_sparse_relu: more than 2^63 elements");
+  if (N == 0) return 0;
+  SreluArgs a = {};
+  a.x = x; a.y = y; a.N = N; a.K = K; a.alpha = alpha;
+  const bool vec = aligned16(x) && aligned16(y) && K % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_sparse_relu<T>(a, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_relu_mask_grad(int dtype, const void* dy, const void* y, void* dx, long long n, void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_relu_mask_grad: unsupported dtype code %d", dtype);
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_relu_mask_grad: bad size %lld", n);
+  if (!dy || !y || !dx) return fail(BSMM_E_ARG, "bsmm_relu_mask_grad: null pointer");
+  if (n == 0) return 0;
+  const bool vec = aligned16(dy) && aligned16(y) && aligned16(dx) && n % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_relu_mask_grad<T>(dy, y, dx, n, vec, (cudaStream_t)stream); });
   return 0;
 }
 

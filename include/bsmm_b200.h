@@ -31,6 +31,9 @@
  *   bsmm_bias_relu_grad   <- EW_Bias_Relu_Grad and BiasGrad (src/ew_op.cc:832-1002)
  *   bsmm_dropout_mask     <- GenDropoutMask (src/ew_op.cc:524-591)
  *   bsmm_dropout_apply    <- ApplyDropoutMask (src/ew_op.cc:593-691)
+ *   bsmm_lstm_gates(_grad) <- LSTMGates / LSTMGates4 and their gradients (src/lstm_op.cc)
+ *   bsmm_sparse_relu      <- SparseRelu (src/lstm_op.cc:430-467)
+ *   bsmm_relu_mask_grad   <- ew_dx_dzza with RELU_OP, sparse_relu's gradient (blocksparse/lstm.py:106-109)
  *   bsmm_embedding_lookup <- EmbeddingLookup (src/embedding_op.cc)
  *   bsmm_embedding_grad   <- EmbeddingLookupGrad (src/embedding_op.cc)
  *   bsmm_block_norm / bsmm_l2_decay / bsmm_threshold_prune / bsmm_prune_topk
@@ -444,6 +447,51 @@ int bsmm_dropout_mask(int32_t* mask, long long M, double keep_prob, long long* s
  */
 int bsmm_dropout_apply(int dtype, const void* x, const int32_t* mask, void* y, int ndim, const long long* shape,
                        const long long* mask_strides, long long mask_words, double keep_prob, void* stream);
+
+/* ---- LSTM gates and sparse relu (the reference's lstm module) --------------------------------------------------------- */
+
+/*
+ * Per element of the (N, K) cell state c (dtype, contiguous):
+ *   c_next = sig(f + b_f + forget_bias) c + sig(i + b_i) tanh(u + b_u),   h_next = sig(o + b_o) tanh(c_next),
+ * with the gates i, u, f, o of row n read at gate + n * stride (elements). The fused (N, 4K) gate tensor h of
+ * LSTM_Forward is i = h, u = h + K, f = h + 2K, o = h + 3K with stride 4K; four separate tensors have stride K. bias:
+ * NULL, or 4K entries of bdtype (F32, F16 or BF16) read as fp32, in the same i, u, f, o blocks. Formed in fp32 with
+ * expf / tanhf, each output rounded once. Replaces LSTM_Gates_Forward / LSTM4_Gates_Forward (src/lstm_op_gpu.cu:283-339,
+ * launched from src/lstm_op.cc), which take int offsets and put N on grid.y (N <= 65535). Any alignment (16-byte accesses
+ * where every pointer and row start allows), 64-bit offsets, no row limit. A bad dtype, N < 0, K <= 0, stride < K or a
+ * null pointer other than bias: BSMM_E_ARG before any launch. N = 0 launches nothing. Kernel: lstm_gates.
+ */
+int bsmm_lstm_gates(int dtype, int bdtype, const void* c, const void* i, const void* u, const void* f, const void* o,
+                    long long stride, const void* bias, void* c_next, void* h_next, long long N, int K,
+                    float forget_bias, void* stream);
+
+/*
+ * dc (N, K) and the gate gradients di, du, df, do (laid out as the gates, same stride) of bsmm_lstm_gates, given its
+ * inputs and the incoming gradients ec of c_next and eh of h_next; either may be NULL and reads as zero. The gates are
+ * recomputed from the inputs; nothing of the forward is saved. Replaces LSTM_Gates_Backward / LSTM4_Gates_Backward
+ * (src/lstm_op_gpu.cu:340-404). The bias gradient is not formed here: it is the column sum of the fused (N, 4K) gate
+ * gradient, which bsmm_bias_relu_grad (act 0, axis 1) gives. Errors as bsmm_lstm_gates. Kernel: lstm_gates_grad.
+ */
+int bsmm_lstm_gates_grad(int dtype, int bdtype, const void* c, const void* i, const void* u, const void* f,
+                         const void* o, long long stride, const void* bias, const void* ec, const void* eh, void* dc,
+                         void* di, void* du, void* df, void* d_o, long long N, int K, float forget_bias, void* stream);
+
+/*
+ * y = max(x - (mean + alpha std), 0) along each row of x, y (N, K) of dtype, contiguous; std is the population standard
+ * deviation. mean and std are formed in fp32 in two passes (never E[x^2] - E[x]^2) and a fixed order, so y is bitwise
+ * reproducible; a row whose entries are all equal gives zeros. Replaces SparseReluForward (src/lstm_op_gpu.cu:554-664),
+ * which forms the variance as E[x^2] - E[x]^2 and puts N on grid.x. A bad dtype, N < 0, K <= 0 or a null pointer:
+ * BSMM_E_ARG before any launch. N = 0 launches nothing. Kernels: sparse_relu_warp (K <= 1024), sparse_relu_cta
+ * (<= 8192), sparse_relu_long.
+ */
+int bsmm_sparse_relu(int dtype, const void* x, void* y, long long N, int K, float alpha, void* stream);
+
+/*
+ * dx = y > 0 ? dy : +0 over n elements of dtype: relu's gradient given its output, the gradient the reference gives
+ * sparse_relu (ew_dx_dzza with RELU_OP). A bad dtype, n < 0 or a null pointer: BSMM_E_ARG before any launch; n = 0
+ * launches nothing. Kernel: relu_mask_grad.
+ */
+int bsmm_relu_mask_grad(int dtype, const void* dy, const void* y, void* dx, long long n, void* stream);
 
 /*
  * y[i, :] = emb[idx[i], :] bit for bit, or zeros where idx[i] is outside [0, C). emb (C, K) and y (n, K) of dtype,

@@ -8,7 +8,9 @@ softmax_cross_entropy, transpose_0213, transpose_2d), of its norms module (layer
 (AdamOptimizer, clip_by_global_norm, global_norm, Ema; AdafactorOptimizer, importable from here and from
 blocksparse_b200.optimize but not listed in __all__), and of its ewops and embed modules (bias_relu, dropout,
 set_entropy, get_entropy, embedding_lookup; listed in ewops.__all__ and embed.__all__), and of its lstm module
-(fused_lstm_gates, split4, concat4, sparse_relu; listed in lstm.__all__).
+(fused_lstm_gates, split4, concat4, sparse_relu; listed in lstm.__all__), and the rest of its ewops module (add,
+multiply, sigmoid, tanh, float_cast, filter_tensor, add_n, concrete_gate, fancy_gather, reduce_max, assign_add, ...;
+listed in elementwise.__all__ and also reachable as blocksparse_b200.ewops.<name>).
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
 from .optimize import (AdafactorOptimizer, AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay, blocksparse_norm,
@@ -19,6 +21,10 @@ from .norms import layer_norm
 from .ewops import bias_relu, dropout, get_entropy, set_entropy
 from .embed import embedding_lookup
 from .lstm import concat4, fused_lstm_gates, sparse_relu, split4
+from .elementwise import (add, add_n, add_n8, assign_add, concrete_gate, concrete_gate_infer, divide, elu, exp,
+                          fancy_gather, fast_gelu, filter_tensor, float_cast, gelu, log, maximum, minimum, multiply,
+                          negative, reciprocal, reduce_max, relu, scale_tensor, sigmoid, sqrt, square, subtract, swish,
+                          tanh)
 from .lut import z_order_2d
 from . import _lib
 

@@ -60,7 +60,20 @@ SIGNATURES = {
                                   _f, _vp]),
     "bsmm_sparse_relu": (_i, [_i, _vp, _vp, _ll, _i, _f, _vp]),
     "bsmm_relu_mask_grad": (_i, [_i, _vp, _vp, _vp, _ll, _vp]),
-    "bsmm_embedding_lookup": (_i, [_i, _i, _vp, _vp, _vp, _ll, _i, _i, _vp]),
+    "bsmm_ew_forward": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _ll, _ll, _f, _vp]),
+    "bsmm_ew_backward": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _f, _vp]),
+    "bsmm_gain_mul_grad": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _vp]),
+    "bsmm_float_cast": (_i, [_i, _i, _vp, _vp, _ll, _vp]),
+    "bsmm_filter_tensor": (_i, [_i, _vp, _vp, _ll, _f, _vp, _f, _i, _i, _vp]),
+    "bsmm_add_n": (_i, [_i, _c.POINTER(_vp), _i, _vp, _ll, _vp]),
+    "bsmm_concrete_gate": (_i, [_i, _vp, _vp, _vp, _ll, _f, _f, _f, _f, _vp, _vp]),
+    "bsmm_concrete_gate_grad": (_i, [_i, _vp, _vp, _vp, _ll, _f, _f, _f, _vp]),
+    "bsmm_concrete_gate_infer": (_i, [_i, _vp, _vp, _ll, _f, _f, _vp]),
+    "bsmm_fancy_gather": (_i, [_i, _vp, _vp, _vp, _ll, _ll, _ll, _vp]),
+    "bsmm_fancy_gather_grad": (_i, [_i, _vp, _vp, _vp, _ll, _ll, _ll, _vp]),
+    "bsmm_reduce_max": (_i, [_i, _i, _vp, _vp, _vp, _ll, _ll, _ll, _vp]),
+    "bsmm_reduce_max_grad": (_i, [_i, _i, _vp, _vp, _vp, _ll, _ll, _ll, _vp]),
+    "bsmm_embedding_lookup":(_i, [_i, _i, _vp, _vp, _vp, _ll, _i, _i, _vp]),
     "bsmm_embedding_grad": (_i, [_i, _i, _vp, _vp, _vp, _vp, _ll, _i, _i, _vp]),
     "bsmm_embedding_grad_workspace_bytes": (_c.c_size_t, [_ll, _i, _i]),
     "bsmm_adam": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _i, _i, _vp]),

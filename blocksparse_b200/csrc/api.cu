@@ -4,6 +4,7 @@
 #include <climits>
 #include "common.cuh"
 #include "dense_softmax.cuh"
+#include "elementwise.cuh"
 #include "embed.cuh"
 #include "ewops.cuh"
 #include "generic.cuh"
@@ -764,6 +765,203 @@ int bsmm_relu_mask_grad(int dtype, const void* dy, const void* y, void* dx, long
   if (n == 0) return 0;
   const bool vec = aligned16(dy) && aligned16(y) && aligned16(dx) && n % (16 / dtype_size(dtype)) == 0;
   BSMM_DISPATCH_DTYPE(dtype, T, { return launch_relu_mask_grad<T>(dy, y, dx, n, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+// ---- elementwise math, casts, filters, sums, gates, gathers, column maxima (csrc/elementwise.cuh) -----------------------
+static bool all_aligned16(std::initializer_list<const void*> ptrs) {
+  for (const void* p : ptrs)
+    if (p && !aligned16(p)) return false;
+  return true;
+}
+
+int bsmm_ew_forward(int dtype, int bdtype, int op, const void* x, const void* y, const void* b, void* z, long long n,
+                    long long K, float alpha, void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_ew_forward: unsupported dtype code %d", dtype);
+  if (op < 0 || op >= EW_NOPS) return fail(BSMM_E_ARG, "bsmm_ew_forward: unknown op code %d", op);
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_ew_forward: bad size %lld", n);
+  if (!x || !z || (ew_binary(op) && !y)) return fail(BSMM_E_ARG, "bsmm_ew_forward: null pointer");
+  if (ew_bcast(op)) {
+    if (!b) return fail(BSMM_E_ARG, "bsmm_ew_forward: null vector");
+    if (!dense_dtype_ok(bdtype)) return fail(BSMM_E_ARG, "bsmm_ew_forward: unsupported vector dtype code %d", bdtype);
+    if (K <= 0 || n % K) return fail(BSMM_E_ARG, "bsmm_ew_forward: n %lld is not a multiple of K %lld", n, K);
+  }
+  if (n == 0) return 0;
+  EwArgs a = {};
+  a.x = x; a.y = y; a.b = b; a.z = z; a.n = n; a.K = K; a.bdt = bdtype; a.alpha = alpha;
+  const bool vec = all_aligned16({x, ew_binary(op) ? y : nullptr, z}) && (!ew_bcast(op) || K % (16 / dtype_size(dtype)) == 0);
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_ew<T>(a, op, false, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_ew_backward(int dtype, int op, const void* dz, const void* x, const void* y, void* dx, void* dy, long long n,
+                     float alpha, void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_ew_backward: unsupported dtype code %d", dtype);
+  if (op < 0 || op >= EW_NOPS || op == EW_ADD || op == EW_SUB || op == EW_NEG || ew_bcast(op))
+    return fail(BSMM_E_ARG, "bsmm_ew_backward: op code %d has no backward kernel", op);
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_ew_backward: bad size %lld", n);
+  if (!dz || !x || !dx || (ew_binary(op) && (!y || !dy))) return fail(BSMM_E_ARG, "bsmm_ew_backward: null pointer");
+  if (n == 0) return 0;
+  EwArgs a = {};
+  a.dz = dz; a.x = x; a.y = y; a.z = dx; a.dy = dy; a.n = n; a.alpha = alpha;
+  const bool vec = all_aligned16({dz, x, dx, ew_binary(op) ? y : nullptr, ew_binary(op) ? dy : nullptr});
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_ew<T>(a, op, true, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_gain_mul_grad(int dtype, int gdtype, const void* dz, const void* x, const void* g, void* dx, void* dg,
+                       void* workspace, long long N, int K, void* stream) {
+  if (!dense_dtype_ok(dtype) || !dense_dtype_ok(gdtype))
+    return fail(BSMM_E_ARG, "bsmm_gain_mul_grad: unsupported dtype codes %d, %d", dtype, gdtype);
+  if (N < 0 || K <= 0) return fail(BSMM_E_ARG, "bsmm_gain_mul_grad: bad sizes N %lld, K %d", N, K);
+  if (!dz || !x || !g || !dx || !dg || !workspace) return fail(BSMM_E_ARG, "bsmm_gain_mul_grad: null pointer");
+  if (N > LLONG_MAX / K) return fail(BSMM_E_LIMIT, "bsmm_gain_mul_grad: more than 2^63 elements");
+  if (N == 0) return 0;
+  BrArgs a = {};
+  a.x = x; a.b = g; a.y = dx; a.part = (float*)workspace; a.N = N; a.K = K; a.bdt = gdtype;
+  const bool vec = all_aligned16({dz, x, dx}) && K % (16 / dtype_size(dtype)) == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_gain_mul_grad<T>(a, dz, dg, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_float_cast(int xdtype, int ydtype, const void* x, void* y, long long n, void* stream) {
+  if (!dense_dtype_ok(xdtype) || !dense_dtype_ok(ydtype))
+    return fail(BSMM_E_ARG, "bsmm_float_cast: unsupported dtype codes %d, %d", xdtype, ydtype);
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_float_cast: bad size %lld", n);
+  if (!x || !y) return fail(BSMM_E_ARG, "bsmm_float_cast: null pointer");
+  if (n == 0) return 0;
+  return launch_float_cast(xdtype, ydtype, x, y, n, all_aligned16({x, y}), (cudaStream_t)stream);
+}
+
+int bsmm_filter_tensor(int dtype, const void* x, void* y, long long n, float scale, const float* scale_ptr,
+                       float saturate, int zero_infs, int zero_nans, void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_filter_tensor: unsupported dtype code %d", dtype);
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_filter_tensor: bad size %lld", n);
+  if (!x || !y) return fail(BSMM_E_ARG, "bsmm_filter_tensor: null pointer");
+  if (n == 0) return 0;
+  FilterArgs a = {};
+  a.x = x; a.y = y; a.scale_ptr = scale_ptr; a.n = n; a.scale = scale; a.saturate = saturate;
+  a.zero_infs = zero_infs != 0; a.zero_nans = zero_nans != 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_filter<T>(a, all_aligned16({x, y}), (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_add_n(int dtype, const void* const* xs, int count, void* y, long long n, void* stream) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_add_n: unsupported dtype code %d", dtype);
+  if (count < 1 || count > ADDN_MAX) return fail(BSMM_E_ARG, "bsmm_add_n: count must be in [1, %d], got %d", ADDN_MAX, count);
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_add_n: bad size %lld", n);
+  if (!xs || !y) return fail(BSMM_E_ARG, "bsmm_add_n: null pointer");
+  AddNArgs a = {};
+  bool vec = aligned16(y);
+  for (int i = 0; i < count; ++i) {
+    if (!xs[i]) return fail(BSMM_E_ARG, "bsmm_add_n: null input %d", i);
+    a.x[i] = xs[i];
+    vec = vec && aligned16(xs[i]);
+  }
+  if (n == 0) return 0;
+  a.y = y; a.n = n; a.count = count;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_add_n<T>(a, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+static int gate_args(const char* what, int dtype, long long n, float limit_a, float limit_b) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "%s: unsupported dtype code %d", what, dtype);
+  if (n < 0) return fail(BSMM_E_ARG, "%s: bad size %lld", what, n);
+  if (!(limit_a < limit_b)) return fail(BSMM_E_ARG, "%s: limit_a %g must be below limit_b %g", what, limit_a, limit_b);
+  return 0;
+}
+
+int bsmm_concrete_gate(int dtype, const void* loga, void* gate, float* concrete, long long n, float rcp_temp,
+                       float limit_a, float limit_b, float epsilon, long long* state, void* stream) {
+  if (int e = gate_args("bsmm_concrete_gate", dtype, n, limit_a, limit_b)) return e;
+  if (!loga || !gate || !concrete || !state) return fail(BSMM_E_ARG, "bsmm_concrete_gate: null pointer");
+  if (!(epsilon >= 0.f && epsilon < 0.5f)) return fail(BSMM_E_ARG, "bsmm_concrete_gate: epsilon must be in [0, 0.5)");
+  if (n == 0) return 0;
+  GateArgs a = {};
+  a.loga = loga; a.gate = gate; a.concrete = concrete; a.state = state; a.n = n; a.rcp_temp = rcp_temp;
+  a.limit_a = limit_a; a.limit_b = limit_b; a.epsilon = epsilon;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_concrete_gate<T>(a, 0, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_concrete_gate_grad(int dtype, const void* dgate, const float* concrete, void* dloga, long long n,
+                            float rcp_temp, float limit_a, float limit_b, void* stream) {
+  if (int e = gate_args("bsmm_concrete_gate_grad", dtype, n, limit_a, limit_b)) return e;
+  if (!dgate || !concrete || !dloga) return fail(BSMM_E_ARG, "bsmm_concrete_gate_grad: null pointer");
+  if (n == 0) return 0;
+  GateArgs a = {};
+  a.loga = dgate; a.gate = dloga; a.concrete = (float*)concrete; a.n = n; a.rcp_temp = rcp_temp;
+  a.limit_a = limit_a; a.limit_b = limit_b;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_concrete_gate<T>(a, 1, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_concrete_gate_infer(int dtype, const void* loga, void* gate, long long n, float limit_a, float limit_b,
+                             void* stream) {
+  if (int e = gate_args("bsmm_concrete_gate_infer", dtype, n, limit_a, limit_b)) return e;
+  if (!loga || !gate) return fail(BSMM_E_ARG, "bsmm_concrete_gate_infer: null pointer");
+  if (n == 0) return 0;
+  GateArgs a = {};
+  a.loga = loga; a.gate = gate; a.n = n; a.limit_a = limit_a; a.limit_b = limit_b;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_concrete_gate<T>(a, 2, (cudaStream_t)stream); });
+  return 0;
+}
+
+static int dims3(const char* what, long long d0, long long d1, long long d2) {
+  if (d0 < 0 || d1 < 0 || d2 < 0) return fail(BSMM_E_ARG, "%s: bad dims %lld, %lld, %lld", what, d0, d1, d2);
+  if (d0 && d1 && d2 && (d1 > LLONG_MAX / d2 || d0 > LLONG_MAX / (d1 * d2)))
+    return fail(BSMM_E_LIMIT, "%s: more than 2^63 elements", what);
+  return 0;
+}
+
+int bsmm_fancy_gather(int esize, const void* x, const int32_t* idx, void* y, long long d0, long long d1, long long d2,
+                      void* stream) {
+  if (esize != 2 && esize != 4) return fail(BSMM_E_ARG, "bsmm_fancy_gather: element size must be 2 or 4, got %d", esize);
+  if (int e = dims3("bsmm_fancy_gather", d0, d1, d2)) return e;
+  if (!x || !idx || !y) return fail(BSMM_E_ARG, "bsmm_fancy_gather: null pointer");
+  if (d0 * d2 == 0) return 0;
+  return launch_fancy_gather(esize, false, x, idx, y, d0, d1, d2, (cudaStream_t)stream);
+}
+
+int bsmm_fancy_gather_grad(int esize, const void* dy, const int32_t* idx, void* dx, long long d0, long long d1,
+                           long long d2, void* stream) {
+  if (esize != 2 && esize != 4) return fail(BSMM_E_ARG, "bsmm_fancy_gather_grad: element size must be 2 or 4, got %d", esize);
+  if (int e = dims3("bsmm_fancy_gather_grad", d0, d1, d2)) return e;
+  if (!dy || !idx || !dx) return fail(BSMM_E_ARG, "bsmm_fancy_gather_grad: null pointer");
+  if (d0 * d1 * d2 == 0) return 0;
+  return launch_fancy_gather(esize, true, dy, idx, dx, d0, d1, d2, (cudaStream_t)stream);
+}
+
+static int rmax_args(const char* what, int dtype, int idx_type, long long d0, long long d1, long long d2) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "%s: unsupported dtype code %d", what, dtype);
+  if (idx_type != BSMM_LABEL_U8 && idx_type != BSMM_LABEL_U16 && idx_type != BSMM_LABEL_I32)
+    return fail(BSMM_E_ARG, "%s: index type %d is not U8, U16 or I32", what, idx_type);
+  if (int e = dims3(what, d0, d1, d2)) return e;
+  if (d1 < 1) return fail(BSMM_E_ARG, "%s: the reduced dim must have at least one entry", what);
+  const long long cap = idx_type == BSMM_LABEL_U8 ? 256 : idx_type == BSMM_LABEL_U16 ? 65536 : 2147483648LL;
+  if (d1 > cap) return fail(BSMM_E_ARG, "%s: %lld entries do not fit index type %d", what, d1, idx_type);
+  return 0;
+}
+
+int bsmm_reduce_max(int dtype, int idx_type, const void* x, void* y, void* argmax, long long d0, long long d1,
+                    long long d2, void* stream) {
+  if (int e = rmax_args("bsmm_reduce_max", dtype, idx_type, d0, d1, d2)) return e;
+  if (!x || !y || !argmax) return fail(BSMM_E_ARG, "bsmm_reduce_max: null pointer");
+  if (d0 * d2 == 0) return 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, {
+    return launch_reduce_max<T>(idx_type, false, x, argmax, nullptr, y, d0, d1, d2, (cudaStream_t)stream);
+  });
+  return 0;
+}
+
+int bsmm_reduce_max_grad(int dtype, int idx_type, const void* dy, const void* argmax, void* dx, long long d0,
+                         long long d1, long long d2, void* stream) {
+  if (int e = rmax_args("bsmm_reduce_max_grad", dtype, idx_type, d0, d1, d2)) return e;
+  if (!dy || !argmax || !dx) return fail(BSMM_E_ARG, "bsmm_reduce_max_grad: null pointer");
+  if (d0 * d2 == 0) return 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, {
+    return launch_reduce_max<T>(idx_type, true, dy, (void*)argmax, dx, nullptr, d0, d1, d2, (cudaStream_t)stream);
+  });
   return 0;
 }
 

@@ -2,8 +2,10 @@
 :207-242) and of its entropy state (blocksparse/utils.py:21-39), on torch tensors, calling the sm_90a kernels of
 csrc/ewops.cuh through bsmm_bias_relu / bsmm_bias_relu_grad / bsmm_dropout_mask / bsmm_dropout_apply.
 
-The reference's other elementwise ops (add, float_cast, scale_tensor, filter_tensor, ...) are one torch expression each
-and are not carried here.
+The reference's other elementwise ops (add, multiply, sigmoid, float_cast, filter_tensor, add_n, concrete_gate,
+fancy_gather, reduce_max, assign_add, ...) live in blocksparse_b200/elementwise.py, which also sets them as attributes of
+this module, so that `from blocksparse_b200 import ewops as ew; ew.add(x, b)` reads as the reference does; they are not
+listed in this module's __all__.
 """
 import ctypes
 import math

@@ -34,6 +34,11 @@
  *   bsmm_lstm_gates(_grad) <- LSTMGates / LSTMGates4 and their gradients (src/lstm_op.cc)
  *   bsmm_sparse_relu      <- SparseRelu (src/lstm_op.cc:430-467)
  *   bsmm_relu_mask_grad   <- ew_dx_dzza with RELU_OP, sparse_relu's gradient (blocksparse/lstm.py:106-109)
+ *   bsmm_ew_forward / bsmm_ew_backward / bsmm_gain_mul_grad <- EW_Forward / EW_Backward (src/ew_op_gpu.cu:306-536)
+ *   bsmm_float_cast       <- FloatCast (src/ew_op_gpu.cu:537-576)
+ *   bsmm_concrete_gate(_grad, _infer) <- ConcreteGate / ConcreteGateGrad / ConcreteGateInfer (src/ew_op_gpu.cu:578-685)
+ *   bsmm_filter_tensor / bsmm_add_n <- FilterTensor / AddN (src/ew_op_gpu.cu:816-915)
+ *   bsmm_fancy_gather(_grad) / bsmm_reduce_max(_grad) <- EW_Fancy_Gather / EW_Reduce_Max (src/ew_op_gpu.cu:1434-1676)
  *   bsmm_embedding_lookup <- EmbeddingLookup (src/embedding_op.cc)
  *   bsmm_embedding_grad   <- EmbeddingLookupGrad (src/embedding_op.cc)
  *   bsmm_block_norm / bsmm_l2_decay / bsmm_threshold_prune / bsmm_prune_topk
@@ -492,6 +497,118 @@ int bsmm_sparse_relu(int dtype, const void* x, void* y, long long N, int K, floa
  * launches nothing. Kernel: relu_mask_grad.
  */
 int bsmm_relu_mask_grad(int dtype, const void* dy, const void* y, void* dx, long long n, void* stream);
+
+/* ---- elementwise math, casts, filters, sums, gates, gathers and column maxima (the reference's ewops module) --------- */
+
+/*
+ * z = op(x, y) over n elements of dtype, formed in fp32 and rounded once. op is the reference's code
+ * (blocksparse/ewops.py:25-44): 0 add, 1 sub, 2 mul, 3 div, 4 maximum, 5 minimum (binary, y of n elements), 6 neg,
+ * 7 rcp, 8 sqr, 9 sqrt, 10 exp, 11 log, 12 sigmoid, 13 tanh, 14 relu, 15 elu, 16 gelu, 17 swish (unary, y unused;
+ * alpha for 15-17), 18 bias-add z = x + b, 19 gain-mul z = x * b (x viewed as (n / K, K), b K entries of bdtype read
+ * as fp32). Replaces EW_Forward (src/ew_op_gpu.cu:306-399), which approximates div, rcp, sqrt, exp, log and sigmoid
+ * with the PTX .approx instructions and takes int sizes; here IEEE division and square root, expf / logf / tanhf /
+ * expm1f, 64-bit offsets, any alignment (16-byte accesses when x, y and z are 16-byte aligned, and K a multiple of the
+ * vector width for 18 / 19). z may alias x (assign_add). A bad dtype or op code, n < 0, a null pointer the op reads, or
+ * for 18 / 19 K <= 0 or n % K != 0: BSMM_E_ARG before any launch. n = 0 launches nothing. Kernel: ew_forward.
+ */
+int bsmm_ew_forward(int dtype, int bdtype, int op, const void* x, const void* y, const void* b, void* z, long long n,
+                    long long K, float alpha, void* stream);
+
+/*
+ * The gradient of bsmm_ew_forward: dx (and dy for ops 2-5) from dz and x, where x is the forward's output z for
+ * sigmoid, tanh and relu (the reference's ew_dx_dzza) and its input otherwise (ew_dx_dzxa, ew_dxdy_dzxy); y the
+ * forward's y for ops 2-5. maximum / minimum give dz to every operand that equals the result. Replaces EW_Backward
+ * (src/ew_op_gpu.cu:400-536) except for the vector gradients. add, sub and neg have no kernel (their gradients are dz
+ * and -dz: bsmm_ew_forward op 6), and bias-add / gain-mul have bsmm_bias_relu_grad (act 0, axis 1) and
+ * bsmm_gain_mul_grad; those op codes give BSMM_E_ARG, as do the errors of bsmm_ew_forward. Kernel: ew_backward.
+ */
+int bsmm_ew_backward(int dtype, int op, const void* dz, const void* x, const void* y, void* dx, void* dy, long long n,
+                     float alpha, void* stream);
+
+/*
+ * Gain-mul gradient: dx = dz * g and dg[k] = sum over rows of dz * x, for dz, x, dx (N, K) of dtype and g K entries of
+ * gdtype (read as fp32; dg comes back in gdtype). The partials of dg follow bsmm_bias_relu_grad's axis-1 partition into
+ * `workspace` (bsmm_bias_grad_workspace_bytes(1, N, K) bytes), added in a fixed order: bitwise reproducible. Replaces
+ * GainMulGrad of EW_Backward (src/ew_op_gpu.cu:217-256), which switches to 4-wide loads only from 16384 elements.
+ * A bad dtype, N < 0, K <= 0 or a null pointer: BSMM_E_ARG before any launch. Kernel: gain_mul_grad.
+ */
+int bsmm_gain_mul_grad(int dtype, int gdtype, const void* dz, const void* x, const void* g, void* dx, void* dg,
+                       void* workspace, long long N, int K, void* stream);
+
+/*
+ * y = x converted from xdtype to ydtype (any pair of F32, F16, BF16), through fp32 and rounded once to nearest even.
+ * Replaces FloatCast (src/ew_op_gpu.cu:537-576), which has only the fp32 <-> 16-bit pairs and int sizes. A bad dtype,
+ * n < 0 or a null pointer: BSMM_E_ARG before any launch. Kernel: float_cast.
+ */
+int bsmm_float_cast(int xdtype, int ydtype, const void* x, void* y, long long n, void* stream);
+
+/*
+ * y = saturate(scale * zero_nans(zero_infs(x))) over n elements: zero_infs / zero_nans replace +-inf / NaN by 0, scale
+ * is *scale_ptr (an fp32 device scalar, read on the device) when scale_ptr is given and `scale` otherwise, and a nonzero
+ * saturate clamps to [-saturate, saturate] with fminf / fmaxf (a NaN left in becomes +saturate). Replaces FilterTensor
+ * (src/ew_op_gpu.cu:816-860). A bad dtype, n < 0 or a null x / y: BSMM_E_ARG before any launch. Kernel: filter_tensor.
+ */
+int bsmm_filter_tensor(int dtype, const void* x, void* y, long long n, float scale, const float* scale_ptr,
+                       float saturate, int zero_infs, int zero_nans, void* stream);
+
+/*
+ * y = xs[0] + xs[1] + ... + xs[count - 1], 1 <= count <= 8 tensors of n elements of dtype, added in fp32 in that order
+ * starting from +0 and rounded once. Replaces AddN (src/ew_op_gpu.cu:862-915). A bad dtype or count, n < 0 or a null
+ * pointer: BSMM_E_ARG before any launch. Kernel: add_n.
+ */
+int bsmm_add_n(int dtype, const void* const* xs, int count, void* y, long long n, void* stream);
+
+/*
+ * Hard-concrete gate (L0 pruning), per element of loga (n of dtype): u is word e % 4 of Philox4x32-10 keyed by
+ * state[0] at counter (e / 4, state[1]), f = fp32(u) 2^-32 (1 - 2 epsilon) + epsilon, c = sigmoid((log f - log(1 - f) +
+ * loga) rcp_temp) -> concrete (fp32), gate = clamp(c (limit_b - limit_a) + limit_a, 0, 1) -> gate (dtype). state is the
+ * device int64 [seed, call] of bsmm_dropout_mask; a one-thread kernel adds 1 to call afterwards. Replaces ConcreteGate
+ * (src/ew_op_gpu.cu:578-663), whose uniforms come from a Tausworthe state sized by the grid. A bad dtype, n < 0,
+ * limit_a >= limit_b, epsilon outside [0, 0.5) or a null pointer: BSMM_E_ARG before any launch. Kernel: concrete_gate.
+ */
+int bsmm_concrete_gate(int dtype, const void* loga, void* gate, float* concrete, long long n, float rcp_temp,
+                       float limit_a, float limit_b, float epsilon, long long* state, void* stream);
+
+/*
+ * dloga = [0 <= c (limit_b - limit_a) + limit_a <= 1] dgate (limit_b - limit_a) c (1 - c) rcp_temp, from the concrete
+ * values c of bsmm_concrete_gate. Replaces ConcreteGateGrad (src/ew_op_gpu.cu:616-674). Errors as bsmm_concrete_gate.
+ * Kernel: concrete_gate_grad.
+ */
+int bsmm_concrete_gate_grad(int dtype, const void* dgate, const float* concrete, void* dloga, long long n,
+                            float rcp_temp, float limit_a, float limit_b, void* stream);
+
+/*
+ * gate = clamp(sigmoid(loga) (limit_b - limit_a) + limit_a, 0, 1), no noise. Replaces ConcreteGateInfer
+ * (src/ew_op_gpu.cu:636-685). Errors as bsmm_concrete_gate. Kernel: concrete_gate_infer.
+ */
+int bsmm_concrete_gate_infer(int dtype, const void* loga, void* gate, long long n, float limit_a, float limit_b,
+                             void* stream);
+
+/*
+ * x (d0, d1, d2) and idx (d0) int32: y[i, j] = x[i, max(idx[i], 0), j], or 0 where max(idx[i], 0) >= d1. Elements of
+ * esize bytes (2 or 4: fp16 / bf16, fp32 / int32) are copied bit for bit. The gradient writes all of dx (d0, d1, d2):
+ * dy[i, j] at row max(idx[i], 0) of block i and 0 elsewhere. Replaces EW_Fancy_Gather(_Grad) (src/ew_op_gpu.cu:
+ * 1434-1542), which takes d2 <= 1024 and uint sizes; here any d2 and 64-bit offsets. A bad esize, negative dims or a null
+ * pointer: BSMM_E_ARG before any launch. Kernels: fancy_gather, fancy_gather_grad.
+ */
+int bsmm_fancy_gather(int esize, const void* x, const int32_t* idx, void* y, long long d0, long long d1, long long d2,
+                      void* stream);
+int bsmm_fancy_gather_grad(int esize, const void* dy, const int32_t* idx, void* dx, long long d0, long long d1,
+                           long long d2, void* stream);
+
+/*
+ * x (d0, d1, d2) -> y (d0, d2) of dtype and argmax (d0, d2) of idx_type (BSMM_LABEL_U8 for d1 <= 256, U16 for
+ * <= 65536, I32): the maximum over d1, by the reference kernel's rule: start from (-FLT_MAX, 0) and take an entry only
+ * when it is strictly greater, so the first maximum wins, NaN is never taken and a column of NaNs (or of -inf) gives
+ * -FLT_MAX (rounded to dtype) at index 0. The gradient writes all of dx (d0, d1, d2): dy at the stored index, 0
+ * elsewhere. Replaces EW_Reduce_Max(_Grad) (src/ew_op_gpu.cu:1544-1636), which has uint sizes and U8 / U16 indices only.
+ * d2 == 1 runs a warp per row. A bad dtype or idx_type, an index type too narrow for d1, d1 < 1, negative dims or a null
+ * pointer: BSMM_E_ARG before any launch. Kernels: reduce_max_row, reduce_max_col, reduce_max_grad.
+ */
+int bsmm_reduce_max(int dtype, int idx_type, const void* x, void* y, void* argmax, long long d0, long long d1,
+                    long long d2, void* stream);
+int bsmm_reduce_max_grad(int dtype, int idx_type, const void* dy, const void* argmax, void* dx, long long d0,
+                         long long d1, long long d2, void* stream);
 
 /*
  * y[i, :] = emb[idx[i], :] bit for bit, or zeros where idx[i] is outside [0, C). emb (C, K) and y (n, K) of dtype,

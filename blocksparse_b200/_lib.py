@@ -82,6 +82,9 @@ SIGNATURES = {
     "bsmm_ema": (_i, [_i, _vp, _i, _vp, _vp, _vp, _vp, _f, _vp]),
     "bsmm_adafactor": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _i, _i, _vp, _vp]),
     "bsmm_adafactor_workspace_bytes": (_c.c_size_t, [_i, _vp, _vp]),
+    "bsmm_quantize": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "bsmm_quantize_stats": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _vp]),
+    "bsmm_quantize_stats_workspace_bytes": (_c.c_size_t, [_i, _vp]),
     "bsmm_block_norm":(_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),

@@ -11,6 +11,7 @@
 #include "layer_norm.cuh"
 #include "lstm.cuh"
 #include "optimize.cuh"
+#include "quantize.cuh"
 #include "softmax.cuh"
 #include "tc.cuh"
 #include "transpose.cuh"
@@ -1354,6 +1355,105 @@ int bsmm_adafactor(int n, const void* const* grads, const int* grad_dtypes, floa
         if (int e = check_launch("mt_adafactor_rate")) return e;
         mt_adafactor_apply<<<tiles, AF_THREADS, 0, s>>>(tab, k);
         return check_launch("mt_adafactor_apply");
+      });
+}
+static int q_format_args(const char* what, int ebits, int fbits, int denorm) {
+  if (ebits < 1 || ebits > 8) return fail(BSMM_E_ARG, "%s: ebits %d outside 1..8", what, ebits);
+  if (fbits < 0 || fbits > 23) return fail(BSMM_E_ARG, "%s: fbits %d outside 0..23", what, fbits);
+  if (denorm != 0 && denorm != 1) return fail(BSMM_E_ARG, "%s: denorm %d (0 or 1)", what, denorm);
+  return 0;
+}
+
+// Checks tensor i of a multi-tensor quantize entry: size >= 0, a grid that fits, non-null pointers when not empty.
+static int q_check(const char* what, int i, long long size, const void* const* ptrs, int nptr) {
+  if (size < 0) return fail(BSMM_E_ARG, "%s: tensor %d has negative size %lld", what, i, size);
+  if (q_chunks(size) > 0x7fffffffLL) return fail(BSMM_E_LIMIT, "%s: tensor %d of %lld elements exceeds the grid", what, i, size);
+  if (size == 0) return 0;
+  for (int j = 0; j < nptr; ++j)
+    if (!ptrs[j]) return fail(BSMM_E_ARG, "%s: tensor %d has a null pointer", what, i);
+  return 0;
+}
+
+int bsmm_quantize(int n, int dtype, const void* const* xs, void* const* ys, long long* const* exps, const long long* sizes,
+                  int ebits, int fbits, int denorm, int stochastic, long long* entropy, void* stream) {
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_quantize: n = %d", n);
+  if (dtype != BSMM_F32 && dtype != BSMM_BF16) return fail(BSMM_E_ARG, "bsmm_quantize: dtype %d (F32 or BF16)", dtype);
+  if (int e = q_format_args("bsmm_quantize", ebits, fbits, denorm)) return e;
+  if (dtype == BSMM_BF16 && fbits > 7) return fail(BSMM_E_ARG, "bsmm_quantize: bf16 holds at most 7 fraction bits, got %d", fbits);
+  if (stochastic < 0 || stochastic > 2) return fail(BSMM_E_ARG, "bsmm_quantize: stochastic %d (0, 1 or 2)", stochastic);
+  if (stochastic && !entropy) return fail(BSMM_E_ARG, "bsmm_quantize: stochastic rounding without an entropy state");
+  if (n && (!xs || !ys || !exps || !sizes)) return fail(BSMM_E_ARG, "bsmm_quantize: null array");
+  bool any = false;
+  for (int i = 0; i < n; ++i) {
+    const void* ptrs[3] = {xs[i], ys[i], exps[i]};
+    if (int e = q_check("bsmm_quantize", i, sizes[i], ptrs, 3)) return e;
+    any = any || sizes[i] > 0;
+  }
+  if (!any) return 0;
+  const QConsts k = {entropy, ebits, fbits, denorm, stochastic ? 1 : 0};
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (int e = q_for_launches(n, sizes,
+          [&](int i, QTensor& t) {
+            t.x = xs[i]; t.y = ys[i]; t.exp = exps[i];
+            t.vec = aligned16(t.x) && aligned16(t.y);
+          },
+          [&](const QTable& tab, int chunks, long long) {
+            if (dtype == BSMM_F32) {
+              if (k.stoch) q_quantize<float, true><<<chunks, Q_THREADS, 0, s>>>(tab, k);
+              else         q_quantize<float, false><<<chunks, Q_THREADS, 0, s>>>(tab, k);
+            } else {
+              if (k.stoch) q_quantize<__nv_bfloat16, true><<<chunks, Q_THREADS, 0, s>>>(tab, k);
+              else         q_quantize<__nv_bfloat16, false><<<chunks, Q_THREADS, 0, s>>>(tab, k);
+            }
+            return check_launch(k.stoch ? "quantize_stochastic" : "quantize");
+          }))
+    return e;
+  if (!k.stoch) return 0;
+  q_advance<<<1, 1, 0, s>>>(entropy, (long long)n);
+  return check_launch("quantize_stochastic");
+}
+
+size_t bsmm_quantize_stats_workspace_bytes(int n, const long long* sizes) {
+  if (n < 0 || (n && !sizes)) return 0;
+  long long chunks = 0;
+  for (int i = 0; i < n; ++i) {
+    if (sizes[i] < 0) return 0;
+    chunks += q_chunks(sizes[i]);
+  }
+  return (size_t)chunks * sizeof(QPart);
+}
+
+int bsmm_quantize_stats(int n, int dtype, const void* const* xs, const long long* sizes, long long* const* exps,
+                        float* stats, int ebits, int fbits, int denorm, int mode, int bias_pad, float stdv_mul,
+                        float sat_val, float ftz_val, void* workspace, void* stream) {
+  if (n < 0) return fail(BSMM_E_ARG, "bsmm_quantize_stats: n = %d", n);
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_quantize_stats: unsupported dtype code %d", dtype);
+  if (exps) {
+    if (int e = q_format_args("bsmm_quantize_stats", ebits, fbits, denorm)) return e;
+    if (mode != 0 && mode != 1) return fail(BSMM_E_ARG, "bsmm_quantize_stats: mode %d (0 or 1)", mode);
+  }
+  if (n && (!xs || !sizes)) return fail(BSMM_E_ARG, "bsmm_quantize_stats: null array");
+  long long total = 0;
+  for (int i = 0; i < n; ++i) {
+    const void* ptrs[2] = {xs[i], exps ? exps[i] : xs[i]};
+    if (int e = q_check("bsmm_quantize_stats", i, sizes[i], ptrs, 2)) return e;
+    total += q_chunks(sizes[i]);
+  }
+  if (total == 0) return 0;
+  if (!stats || !workspace) return fail(BSMM_E_ARG, "bsmm_quantize_stats: null stats or workspace");
+  QStatConsts k = {stats, workspace, sat_val, ftz_val, stdv_mul, ebits, fbits, denorm, mode, bias_pad, dtype == BSMM_F16};
+  const cudaStream_t s = (cudaStream_t)stream;
+  QPart* parts = static_cast<QPart*>(workspace);
+  return q_for_launches(n, sizes,
+      [&](int i, QTensor& t) {
+        t.x = xs[i]; t.exp = exps ? exps[i] : nullptr;
+        t.vec = aligned16(t.x);
+      },
+      [&](const QTable& tab, int chunks, long long base) {
+        BSMM_DISPATCH_DTYPE(dtype, T, { q_stats<T><<<chunks, Q_THREADS, 0, s>>>(tab, k, parts + base); });
+        if (int e = check_launch("quantize_stats")) return e;
+        q_stats_finish<<<tab.n, Q_THREADS, 0, s>>>(tab, k, parts + base);
+        return check_launch("quantize_stats");
       });
 }
 }  // extern "C"

@@ -122,9 +122,30 @@ def _check_capture(opt, rate, group, *powers):
 
 
 def _check_qspec(**qspecs):
+    from .quantize import QuantizeSpec, _check_spec
     for k, v in qspecs.items():
-        if v is not None:
-            raise ValueError("%s: the quantize module is not carried here; only None is accepted" % k)
+        if v is None:
+            continue
+        if not isinstance(v, QuantizeSpec):
+            raise ValueError("%s must be None or a blocksparse_b200.quantize.QuantizeSpec, got %r" % (k, v))
+        _check_spec(v, k)
+
+
+def _quantize_in_place(st_of, kind, spec, tensors, names):
+    """Rounds tensors (fp32, on the current device) in place to spec: one multi-tensor quantize launch (per 256), plus
+    one statistics launch on the calls their schedules pick. Tensor i's exponent record and schedule live in st_of(i) as
+    "<kind>_qexp" (0-dim int64) and "<kind>_qsched"."""
+    from .quantize import new_exponent, new_schedule, quantize_tensors
+    exps, scheds = [], []
+    for i in range(len(tensors)):
+        st = st_of(i)
+        if kind + "_qexp" not in st:
+            st[kind + "_qexp"] = new_exponent(spec.emax, tensors[i].device)
+            st[kind + "_qsched"] = new_schedule()
+        exps.append(st[kind + "_qexp"])
+        scheds.append(st[kind + "_qsched"])
+    if tensors:
+        quantize_tensors(tensors, tensors, exps, scheds, spec, names)
 
 
 class AdamOptimizer(torch.optim.Optimizer):
@@ -140,7 +161,14 @@ class AdamOptimizer(torch.optim.Optimizer):
     the param and both moments bit for bit. fp16=True: params of at least 8192 elements keep their mean and variance as
     int16 tensors of the reference's 16-bit codes (8 bytes of state per parameter instead of 12).
     norm_scale: a one-element fp32 CUDA tensor (e.g. from clip_by_global_norm) read on the device at every step; 0 makes
-    the step a no-op. The *_qspec arguments of the reference's quantize module must be None.
+    the step a no-op.
+
+    param_qspec / mean_qspec / var_qspec: None or a QuantizeSpec (blocksparse_b200.quantize). After the Adam launch the
+    stepped params, means and variances are rounded in place to their spec (reference optimize.py:88-97): one
+    multi-tensor quantize launch per spec and device (per 256 params), plus one statistics launch on the steps the
+    schedules pick. Each (param, spec) pair has its own exponent and schedule in self.state[p] ("param_qexp",
+    "param_qsched", "mean_qexp", ...), so they travel with state_dict(). mean_qspec / var_qspec with fp16=True raise
+    ValueError: the moments are then 16-bit codes. Anything else than None or a QuantizeSpec raises ValueError.
 
     Params may live on several GPUs: each step launches once per device (per 256 params), in param order, with that
     device current; norm_scale reaches the other devices by a device-to-device copy.
@@ -154,6 +182,9 @@ class AdamOptimizer(torch.optim.Optimizer):
                  norm_scale=None, grad_scale=1.0, saturate=0.0, zero_infs=False, zero_nans=False, gated=False,
                  param_qspec=None, mean_qspec=None, var_qspec=None, fp16=False, zero_init_variables=False, name="Adam"):
         _check_qspec(param_qspec=param_qspec, mean_qspec=mean_qspec, var_qspec=var_qspec)
+        if fp16 and (mean_qspec is not None or var_qspec is not None):
+            raise ValueError("AdamOptimizer: mean_qspec / var_qspec need fp32 moments; fp16=True keeps them as 16-bit codes")
+        self.param_qspec, self.mean_qspec, self.var_qspec = param_qspec, mean_qspec, var_qspec
         if norm_scale is not None:
             _dev_scalar(norm_scale, "norm_scale")
         b1, b2 = (0.0, 0.0) if zero_init_variables else (float(np.float32(beta1)), float(np.float32(beta2)))
@@ -175,9 +206,9 @@ class AdamOptimizer(torch.optim.Optimizer):
         return st["mean"], st["var"]
 
     def load_state_dict(self, state_dict):
-        """torch's loader casts every state tensor of a float param to the param's dtype; 16-bit moment codes are
-        restored as the int16 tensors they are."""
-        coded = {i: {k: v for k, v in st.items() if torch.is_tensor(v) and v.dtype == torch.int16}
+        """torch's loader casts every state tensor of a float param to the param's dtype; 16-bit moment codes and the
+        int64 quantize exponents are restored as the integer tensors they are."""
+        coded = {i: {k: v for k, v in st.items() if torch.is_tensor(v) and v.dtype in (torch.int16, torch.int64)}
                  for i, st in state_dict["state"].items()}
         super().load_state_dict(state_dict)
         every = [p for group in self.param_groups for p in group["params"]]
@@ -202,6 +233,7 @@ class AdamOptimizer(torch.optim.Optimizer):
         k = 0
         lib = _lib.load()
         f32 = np.float32
+        index = {}                   # id(param) -> its position over all groups, for the quantize log names
         for group in self.param_groups:
             per_dev = {}             # device -> the step's tables for the params on it, in param order
             for p in group["params"]:
@@ -217,6 +249,7 @@ class AdamOptimizer(torch.optim.Optimizer):
                 if p.numel() == 0:
                     continue
                 gs, gd, ps, ms, vs, codes, sizes, gates, bss = per_dev.setdefault(p.device, tuple([] for _ in range(9)))
+                index[id(p)] = k - 1
                 gd.append(_lib.dtype_code(g.dtype))
                 gate, bs = _gate_of(p, self.gated)
                 m, v = self._moments(p)
@@ -239,7 +272,12 @@ class AdamOptimizer(torch.optim.Optimizer):
                                        float(self.beta1), float(self.beta2), float(self.epsilon), float(self.grad_scale),
                                        float(self.clip_sigmas), float(self.saturate), int(self.zero_infs),
                                        int(self.zero_nans), _lib.stream_ptr())
-                _lib.check(rc, "bsmm_adam")
+                    _lib.check(rc, "bsmm_adam")
+                    for kind, spec, ts in (("param", self.param_qspec, ps), ("mean", self.mean_qspec, ms),
+                                           ("var", self.var_qspec, vs)):
+                        if spec is not None:
+                            _quantize_in_place(lambda i: self.state[ps[i]], kind, spec, ts,
+                                               ["%s/%s_%d" % (self.name, kind, index[id(p)]) for p in ps])
             group["beta1_power"] = float(b1p * f32(self.beta1))                        # optimize.py:104-110
             group["beta2_power"] = float(b2p * f32(self.beta2))
         return loss
@@ -415,15 +453,22 @@ class Ema(object):
     """Exponential moving averages of params (reference optimize.py:231-289): apply(params) creates each average on first
     use as a copy of the param (float16 when fp16), then does ema -= (1 - decay) * (ema - param) for all of them in one
     launch (per 256, and per device for params on several GPUs). Gated, blocks of a param with a `.gate` whose gate is
-    0 keep their average."""
+    0 keep their average.
+
+    apply(params, qspec=QuantizeSpec(...)) then rounds every updated average in place to qspec, in one multi-tensor
+    quantize launch per device (per 256), each average with its own exponent and schedule (self.qstate[id(param)]). With
+    fp16=True a qspec raises ValueError (the averages are float16)."""
 
     def __init__(self, decay=0.999, gated=False, fp16=False, name="Ema"):
         self.decay, self.gated, self.fp16, self.name = decay, gated, fp16, name
         self.averages = dict()           # id(param) -> (param, average)
+        self.qstate = dict()             # id(param) -> {"param", "ema_qexp", "ema_qsched"} of its average
 
     @torch.no_grad()
     def apply(self, params, qspec=None):
         _check_qspec(qspec=qspec)
+        if qspec is not None and self.fp16:
+            raise ValueError("Ema.apply: qspec needs fp32 averages; this Ema keeps them in float16")
         params = list(params)
         per_dev = {}                 # device -> the tables for the params on it, in param order
         for p in params:
@@ -447,7 +492,14 @@ class Ema(object):
                 rc = _lib.load().bsmm_ema(len(ps), arrs[0].ctypes.data, _lib.F16 if self.fp16 else _lib.F32,
                                           arrs[1].ctypes.data, arrs[2].ctypes.data, arrs[3].ctypes.data,
                                           arrs[4].ctypes.data, float(self.decay), _lib.stream_ptr())
-            _lib.check(rc, "bsmm_ema")
+                _lib.check(rc, "bsmm_ema")
+                if qspec is not None:
+                    for p in ps:
+                        st = self.qstate.get(id(p))
+                        if st is None or st["param"] is not p:
+                            self.qstate[id(p)] = {"param": p}
+                    _quantize_in_place(lambda i: self.qstate[id(ps[i])], "ema", qspec, emas,
+                                       ["%s/ema_%d" % (self.name, i) for i in range(len(ps))])
 
     def average(self, param):
         entry = self.averages.get(id(param))

@@ -56,6 +56,9 @@
  *   bsmm_ema              <- EmaOp: ApplyEma / ApplyEmaGated (src/optimize_op.cc:463-529)
  *   bsmm_adafactor        <- Adafactor2dOp / Adafactor1dOp: Adafactor<T,V> per tensor
  *                            (src/optimize_op.cc:21-212, src/optimize_op_gpu.cu:8-365)
+ *   bsmm_quantize         <- Quantize<T> (src/quantize_op_gpu.cu:192-220), launched by QuantizeOp (src/quantize_op.cc)
+ *   bsmm_quantize_stats   <- QuantizationStats<T> (src/quantize_op_gpu.cu:222-239) with QuantizeOp::UpdateExponent
+ *                            and LogStatsOp (src/quantize_op.cc:84-111,217-301)
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer except `err` strings is DEVICE memory
@@ -748,6 +751,43 @@ int bsmm_adafactor(int n, const void* const* grads, const int* grad_dtypes, floa
                    int zero_nans, void* workspace, void* stream);
 /* Bytes of workspace bsmm_adafactor needs for these shapes; 0 for bad arguments. */
 size_t bsmm_adafactor_workspace_bytes(int n, const long long* rows, const long long* cols);
+
+/* ---- quantization to narrow float formats (the reference's quantize module) --------------------------------------- */
+
+/*
+ * Multi-tensor, like the optimizer entries: tensor i of n is entry i of each host array, read before the call returns;
+ * up to 256 non-empty tensors per kernel launch, 64-bit element offsets, 16-byte accesses on a tensor whose pointers
+ * allow them. exps[i] is tensor i's exponent record, one int64 in device memory holding exp_max (unbiased); the kernels
+ * derive the format from it on the device (see csrc/quantize.cuh and DESIGN.md 7i), clamping it so that the largest
+ * value stays finite, and the host never reads it.
+ *
+ * bsmm_quantize: ys[i] = xs[i] rounded to the format (ebits 1..8, fbits 0..23, denorm 0 / 1): the reference kernel's
+ * arithmetic, bit for bit on every non-NaN input; NaN gives NaN (the reference gives -max_float). ys[i] may be xs[i].
+ * dtype BSMM_F32 or BSMM_BF16 (fbits <= 7). stochastic 0 rounds half away from zero; 1 or 2 adds a uniform fraction of
+ * one ulp before truncating, drawn from entropy ([seed, call], int64, device; the dropout state): element e of tensor i
+ * takes word e % 4 of Philox4x32-10 at key seed and counter (e / 4, call + i), and a one-thread kernel then adds n to
+ * call. Errors (BSMM_E_ARG before any launch): n < 0, a bad dtype or format, bf16 with fbits > 7, stochastic outside
+ * 0..2 or without entropy, a null array, a negative size, a null pointer of a non-empty tensor. Empty tensors are
+ * skipped. Kernels: q_quantize ("quantize" / "quantize_stochastic"), q_advance.
+ */
+int bsmm_quantize(int n, int dtype, const void* const* xs, void* const* ys, long long* const* exps, const long long* sizes,
+                  int ebits, int fbits, int denorm, int stochastic, long long* entropy, void* stream);
+
+/*
+ * bsmm_quantize_stats: stats[5 i .. 5 i + 4] = mean |x|, stdv = sqrt(max(E[x^2] - mean^2, 0)), the percentages of
+ * elements with |x| >= sat and of non-zero ones with |x| < ftz, and max |x|, over tensor i (fp32, fp16 or bf16; NaN
+ * counts as inf, and fp16 values are clamped to +-65504 first, as in QuantizationStats). Sums are fp64 and counts
+ * integers, in an order fixed by the sizes, so the result is bitwise reproducible (the reference adds with fp32
+ * atomics). Log mode (exps == NULL): sat = sat_val, ftz = ftz_val. Quantize mode: sat = max_float and ftz = the
+ * format's flush threshold, both from exps[i], and exps[i] is then set to exponent(m) + bias_pad clamped to the format
+ * (m = max |x| in mode 0, mean + stdv * stdv_mul in fp32 in mode 1), ready for a bsmm_quantize later on the stream.
+ * workspace: bsmm_quantize_stats_workspace_bytes(n, sizes) bytes. Errors as bsmm_quantize (any dtype; the format and
+ * mode 0 / 1 are checked in quantize mode only) plus a null stats or workspace. Kernels: q_stats, q_stats_finish.
+ */
+int bsmm_quantize_stats(int n, int dtype, const void* const* xs, const long long* sizes, long long* const* exps,
+                        float* stats, int ebits, int fbits, int denorm, int mode, int bias_pad, float stdv_mul,
+                        float sat_val, float ftz_val, void* workspace, void* stream);
+size_t bsmm_quantize_stats_workspace_bytes(int n, const long long* sizes);
 
 /* ---- measurement helper (the reference's `bench` op attribute, op.cc:99-106) ---------
  * Records two events around whatever the caller enqueues between begin and end.      */

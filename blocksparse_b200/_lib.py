@@ -85,6 +85,12 @@ SIGNATURES = {
     "bsmm_quantize": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "bsmm_quantize_stats": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _f, _f, _vp, _vp]),
     "bsmm_quantize_stats_workspace_bytes": (_c.c_size_t, [_i, _vp]),
+    "bsmm_conv_xprop": (_i, [_i, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _ll, _i, _ll, _i, _ll, _i, _vp]),
+    "bsmm_conv_updat": (_i, [_i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _ll, _i, _ll, _i, _ll, _ll,
+                             _i, _vp]),
+    "bsmm_conv_updat_workspace_bytes": (_c.c_size_t, [_ll, _ll]),
+    "bsmm_conv_l2_normalize": (_i, [_i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _vp]),
+    "bsmm_conv_l2_normalize_grad": (_i, [_i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _f, _vp]),
     "bsmm_block_norm":(_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),

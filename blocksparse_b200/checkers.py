@@ -269,3 +269,93 @@ def sparse_relu_test(x, alpha=1.0):
     x = np.asarray(x)
     cutoff = x.mean(axis=-1, keepdims=True) + alpha * x.std(axis=-1, keepdims=True)
     return np.maximum(x - cutoff, 0.0)
+
+
+class ConvCheckers(object):
+    """Mixin for BlocksparseConv / BlocksparseDeconv (conv.py:540-661, 746-801): needs BCK, blocks, C, K, DHW, MPQ, trs,
+    sizeF, f_shape and the spatial tables _lut_f / _lut_b ([positions][trs], -1 where a tap reads nothing). F and U
+    are lists of per-block arrays of f_shape(block), as in the reference; results are float64, updat's and l2's
+    collapsed to [sizeF] as the reference's are (in float32 there)."""
+
+    @staticmethod
+    def _gather(a, lut):
+        """a (N, C, P) -> (N, C, P_out, trs), zero where lut is -1."""
+        a = np.asarray(a, dtype=np.float64)
+        N, C = a.shape[:2]
+        a = np.concatenate([a.reshape(N, C, -1), np.zeros((N, C, 1))], axis=2)
+        return a[:, :, np.where(lut < 0, a.shape[2] - 1, lut)]
+
+    def _f3(self, block, f):
+        return np.asarray(f, dtype=np.float64).reshape(len(self.BCK[block][1]), len(self.BCK[block][0]), self.trs)
+
+    def _conv_fprop(self, F, I):
+        N = I.shape[0]
+        cols = self._gather(I, self._lut_f)
+        O = np.zeros((N, self.K, int(np.prod(self.MPQ))))
+        for b, (lutC, lutK) in enumerate(self.BCK):
+            O[:, lutK] += np.einsum("ncpt,kct->nkp", cols[:, lutC], self._f3(b, F[b]))
+        return O.reshape([N, self.K] + list(self.MPQ))
+
+    def _conv_bprop(self, F, E):
+        N = E.shape[0]
+        cols = self._gather(E, self._lut_b)
+        O = np.zeros((N, self.C, int(np.prod(self.DHW))))
+        for b, (lutC, lutK) in enumerate(self.BCK):
+            O[:, lutC] += np.einsum("nkpt,kct->ncp", cols[:, lutK], self._f3(b, F[b]))
+        return O.reshape([N, self.C] + list(self.DHW))
+
+    def _conv_updat(self, E, I):
+        N = I.shape[0]
+        cols = self._gather(I, self._lut_f)
+        E = np.asarray(E, dtype=np.float64).reshape(N, self.K, -1)
+        return np.concatenate([np.einsum("nkp,ncpt->kct", E[:, lutK], cols[:, lutC]).ravel()
+                               for lutC, lutK in self.BCK])
+
+    def fprop_test(self, F, I, alpha=1.0):
+        """O = conv(I, F) (conv.py:540-563); the deconv's is the conv's bprop (conv.py:746-747)."""
+        return (self._conv_bprop(F, I) if self.deconv else self._conv_fprop(F, I)) * alpha
+
+    def bprop_test(self, F, I, alpha=1.0):
+        """dI from dO = I (conv.py:565-589); the deconv's is the conv's fprop."""
+        return (self._conv_fprop(F, I) if self.deconv else self._conv_bprop(F, I)) * alpha
+
+    def updat_test(self, E, I, alpha=1.0, transpose=False):
+        """dF, collapsed to [sizeF] (conv.py:591-615); the deconv swaps E and I (conv.py:752-753)."""
+        return (self._conv_updat(I, E) if self.deconv else self._conv_updat(E, I)) * alpha
+
+    def _l2_axes(self):
+        return (0, 2) if self.deconv else (1, 2)
+
+    def l2_normalize_test(self, F, gain=None, epsilon=1e-12):
+        """Each block's rows (KCTRS: per output channel; CKTRS for the deconv: per input channel) scaled to unit l2
+        norm and by gain (conv.py:617-631, 756-772)."""
+        out, off = [], 0
+        for b, f in enumerate(F):
+            f = self._f3(b, f)
+            ax = self._l2_axes()
+            nrm = np.sqrt(np.maximum(np.sum(f * f, axis=ax, keepdims=True), epsilon))
+            y = f / nrm
+            if gain is not None:
+                n = f.shape[1 if self.deconv else 0]
+                g = np.asarray(gain, dtype=np.float64)[off:off + n]
+                y = y * (g.reshape(1, n, 1) if self.deconv else g.reshape(n, 1, 1))
+                off += n
+            out.append(y.ravel())
+        return np.concatenate(out)
+
+    def l2_normalize_grad_test(self, F, U, gain=None, epsilon=1e-12):
+        """(dF collapsed to [sizeF], dgain or None) (conv.py:633-661, 774-801)."""
+        D, dg, off = [], [], 0
+        for b, (f, u) in enumerate(zip(F, U)):
+            f, u = self._f3(b, f), self._f3(b, u)
+            ax = self._l2_axes()
+            n = f.shape[1 if self.deconv else 0]
+            shape = (1, n, 1) if self.deconv else (n, 1, 1)
+            g = np.ones(shape) if gain is None else np.asarray(gain, dtype=np.float64)[off:off + n].reshape(shape)
+            ss = np.sum(f * f, axis=ax, keepdims=True)
+            mx = np.maximum(ss, epsilon)
+            rn = 1.0 / np.sqrt(mx)
+            dg.append(np.sum(u * f * rn, axis=ax).ravel())
+            D.append(((u * g + f * (ss >= epsilon) * np.sum(-u * f * g / mx, axis=ax, keepdims=True)) * rn).ravel())
+            off += n
+        return np.concatenate(D), (None if gain is None else np.concatenate(dg))

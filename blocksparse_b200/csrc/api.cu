@@ -3,6 +3,7 @@
 #include <atomic>
 #include <climits>
 #include "common.cuh"
+#include "conv.cuh"
 #include "dense_softmax.cuh"
 #include "elementwise.cuh"
 #include "embed.cuh"
@@ -1455,5 +1456,153 @@ int bsmm_quantize_stats(int n, int dtype, const void* const* xs, const long long
         q_stats_finish<<<tab.n, Q_THREADS, 0, s>>>(tab, k, parts + base);
         return check_launch("quantize_stats");
       });
+}
+// ---- block-sparse convolution (csrc/conv.cuh) ------------------------------------------------------------------------
+static bool conv_pair_ok(int a, int b) {
+  return dense_dtype_ok(a) && dense_dtype_ok(b) && !((a == BSMM_F16 && b == BSMM_BF16) || (a == BSMM_BF16 && b == BSMM_F16));
+}
+
+// Instantiates body with TA / TB for every supported (a, b) dtype pair (fp16 never meets bf16).
+#define BSMM_CONV_PAIR(a, b, TA, TB, ...)                                                                               \
+  BSMM_DISPATCH_DTYPE(a, TA, {                                                                                        \
+    if ((b) == BSMM_F32) { using TB = float; __VA_ARGS__; }                                                           \
+    else if ((b) == BSMM_F16 && (a) != BSMM_BF16) { using TB = __half; __VA_ARGS__; }                                 \
+    else if ((b) == BSMM_BF16 && (a) != BSMM_F16) { using TB = __nv_bfloat16; __VA_ARGS__; }                          \
+  })
+
+static int conv_common_args(const char* what, const int32_t* blocks, const int32_t* channels, const int32_t* lut,
+                            int trs, const void* x, const void* f, const void* y, long long N, int C_in, long long P_in,
+                            int C_out, long long P_out, int max_out) {
+  if (!blocks || !channels || !lut || !x || !f || !y) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (N < 0 || C_in <= 0 || C_out <= 0 || P_in <= 0 || P_out <= 0 || trs <= 0 || max_out <= 0)
+    return fail(BSMM_E_ARG, "%s: bad sizes (N %lld, C_in %d, P_in %lld, C_out %d, P_out %lld, trs %d, max_out %d)", what, N,
+                C_in, P_in, C_out, P_out, trs, max_out);
+  if (P_out * trs > INT_MAX || P_in > INT_MAX)
+    return fail(BSMM_E_LIMIT, "%s: %lld output positions x %d taps exceed the int32 spatial table", what, P_out, trs);
+  // xprop puts the 64-row tiles of N * P_out on grid.x (at most 2^31 - 1 CTAs)
+  if (N > ((1LL << 37) - 64) / P_out)
+    return fail(BSMM_E_LIMIT, "%s: N * P_out = %lld x %lld reaches 2^37 rows", what, N, P_out);
+  return 0;
+}
+
+int bsmm_conv_xprop(int x_dtype, int f_dtype, const int32_t* blocks, const int* pass_offsets, int passes, int max_out,
+                    const int32_t* channels, const int32_t* lut, int trs, const void* x, const void* f, void* y, float* acc,
+                    long long N, int C_in, long long P_in, int C_out, long long P_out, int flags, void* stream) {
+  const char* what = "bsmm_conv_xprop";
+  if (!conv_pair_ok(x_dtype, f_dtype)) return fail(BSMM_E_ARG, "%s: dtype pair (%d, %d)", what, x_dtype, f_dtype);
+  if (int e = conv_common_args(what, blocks, channels, lut, trs, x, f, y, N, C_in, P_in, C_out, P_out, max_out)) return e;
+  if (passes <= 0 || !pass_offsets) return fail(BSMM_E_ARG, "%s: %d passes", what, passes);
+  for (int i = 0; i < passes; ++i)
+    if (pass_offsets[i] < 0 || pass_offsets[i + 1] <= pass_offsets[i]) return fail(BSMM_E_ARG, "%s: pass %d is empty", what, i);
+  const int col_tiles = (max_out + CONV_T - 1) / CONV_T;
+  const long long rows = N * P_out, row_tiles = (rows + CONV_T - 1) / CONV_T;
+  for (int i = 0; i < passes; ++i)
+    if ((long long)(pass_offsets[i + 1] - pass_offsets[i]) * col_tiles > 65535)
+      return fail(BSMM_E_LIMIT, "%s: pass %d has %d blocks of up to %d outputs (at most 65535 64-wide column tiles)", what,
+                  i, pass_offsets[i + 1] - pass_offsets[i], max_out);
+  const bool multi = passes > 1, y32 = x_dtype == BSMM_F32;
+  if (multi && !y32 && !acc) return fail(BSMM_E_ARG, "%s: %d passes into a 16-bit output need an fp32 accumulator", what, passes);
+  if (rows == 0) return 0;
+  const bool tc = !(flags & BSMM_FLAG_FORCE_GENERIC) && x_dtype == f_dtype && x_dtype != BSMM_F32;
+  const cudaStream_t s = (cudaStream_t)stream;
+  float* accum = multi ? (y32 ? static_cast<float*>(y) : acc) : nullptr;
+  const long long out_elems = N * C_out * P_out;
+  if (accum && cudaMemsetAsync(accum, 0, out_elems * sizeof(float), s) != cudaSuccess) return check_launch(what);
+  ConvArgs a = {nullptr, channels, lut, x, f, accum ? (void*)accum : y, N, P_in, P_out, rows, C_in, C_out, trs,
+                col_tiles, 0, accum ? 1 : 0, 0};
+  const char* name = tc ? "wgmma_conv_xprop" : "fma_conv_xprop";
+  for (int i = 0; i < passes; ++i) {
+    a.blk = reinterpret_cast<const ConvBlk*>(blocks) + pass_offsets[i];
+    const dim3 grid((unsigned)row_tiles, (unsigned)((pass_offsets[i + 1] - pass_offsets[i]) * col_tiles));
+    if (tc) {
+      if (x_dtype == BSMM_BF16) conv_tc_kernel<true, XpropOp<__nv_bfloat16, __nv_bfloat16, CONV_TC_BK>><<<grid, 128, 0, s>>>(a);
+      else conv_tc_kernel<false, XpropOp<__half, __half, CONV_TC_BK>><<<grid, 128, 0, s>>>(a);
+    } else {
+      BSMM_CONV_PAIR(x_dtype, f_dtype, TX, TF, { conv_fma_kernel<XpropOp<TX, TF, 16>><<<grid, 256, 0, s>>>(a); });
+    }
+    if (int e = check_launch(name)) return e;
+  }
+  if (multi && !y32) {
+    if (int e = launch_float_cast(BSMM_F32, x_dtype, acc, y, out_elems, aligned16(acc) && aligned16(y), s)) return e;
+    kernel_name_slot() = name;
+  }
+  return 0;
+}
+
+size_t bsmm_conv_updat_workspace_bytes(long long rows, long long size_f) {
+  if (rows < 0 || size_f < 0) return 0;
+  return (size_t)((rows + CONV_CHUNK - 1) / CONV_CHUNK) * (size_t)size_f * sizeof(float);
+}
+
+int bsmm_conv_updat(int e_dtype, int x_dtype, int f_dtype, const int32_t* blocks, int n_blocks, int max_out, int max_red,
+                    const int32_t* channels, const int32_t* lut, int trs, const void* e, const void* x, void* df,
+                    float* workspace, long long N, int C_in, long long P_in, int C_out, long long P_out, long long size_f,
+                    int flags, void* stream) {
+  const char* what = "bsmm_conv_updat";
+  if (!conv_pair_ok(e_dtype, x_dtype) || !dense_dtype_ok(f_dtype))
+    return fail(BSMM_E_ARG, "%s: dtypes (%d, %d, %d)", what, e_dtype, x_dtype, f_dtype);
+  if (int r = conv_common_args(what, blocks, channels, lut, trs, x, e, df, N, C_in, P_in, C_out, P_out, max_out)) return r;
+  if (n_blocks <= 0 || max_red <= 0 || size_f <= 0 || size_f > INT_MAX)
+    return fail(size_f > INT_MAX ? BSMM_E_LIMIT : BSMM_E_ARG, "%s: %d blocks, max_red %d, size_f %lld", what, n_blocks,
+                max_red, size_f);
+  const long long rows = N * P_out, chunks = (rows + CONV_CHUNK - 1) / CONV_CHUNK;
+  const int row_tiles = (max_out + CONV_T - 1) / CONV_T, col_tiles = (int)(((long long)max_red * trs + CONV_T - 1) / CONV_T);
+  if (chunks > 65535) return fail(BSMM_E_LIMIT, "%s: %lld rows exceed 65535 chunks of %d", what, rows, CONV_CHUNK);
+  if ((long long)n_blocks * row_tiles * col_tiles > INT_MAX) return fail(BSMM_E_LIMIT, "%s: too many tiles", what);
+  if (rows > 0 && !workspace) return fail(BSMM_E_ARG, "%s: null workspace", what);
+  const cudaStream_t s = (cudaStream_t)stream;
+  const bool tc = !(flags & BSMM_FLAG_FORCE_GENERIC) && e_dtype == x_dtype && x_dtype != BSMM_F32;
+  const char* name = tc ? "wgmma_conv_updat" : "fma_conv_updat";
+  if (rows > 0) {
+    const ConvArgs a = {reinterpret_cast<const ConvBlk*>(blocks), channels, lut, x, e, workspace, N, P_in, P_out, rows,
+                        C_in, C_out, trs, col_tiles, row_tiles, 0, size_f};
+    const dim3 grid((unsigned)(n_blocks * row_tiles * col_tiles), (unsigned)chunks);
+    if (tc) {
+      if (x_dtype == BSMM_BF16) conv_tc_kernel<true, UpdatOp<__nv_bfloat16, __nv_bfloat16, CONV_TC_BK>><<<grid, 128, 0, s>>>(a);
+      else conv_tc_kernel<false, UpdatOp<__half, __half, CONV_TC_BK>><<<grid, 128, 0, s>>>(a);
+    } else {
+      BSMM_CONV_PAIR(e_dtype, x_dtype, TE, TX, { conv_fma_kernel<UpdatOp<TE, TX, 16>><<<grid, 256, 0, s>>>(a); });
+    }
+    if (int r = check_launch(name)) return r;
+  }
+  const int grid = (int)((size_f + 255) / 256 < 4096 ? (size_f + 255) / 256 : 4096);
+  BSMM_DISPATCH_DTYPE(f_dtype, TF, {
+    conv_updat_reduce<TF><<<grid, 256, 0, s>>>(workspace, static_cast<TF*>(df), size_f, rows > 0 ? (int)chunks : 0);
+  });
+  if (int r = check_launch(name)) return r;
+  return 0;
+}
+
+int bsmm_conv_l2_normalize(int x_dtype, int y_dtype, const int32_t* rows, int n_rows, int trs, const void* x,
+                           const float* gain, void* y, float* sum_sqr, float epsilon, void* stream) {
+  if (!dense_dtype_ok(x_dtype) || (y_dtype != x_dtype && y_dtype != BSMM_F32))
+    return fail(BSMM_E_ARG, "bsmm_conv_l2_normalize: dtypes (%d, %d): y is x's dtype or fp32", x_dtype, y_dtype);
+  if (!rows || !x || !y || !sum_sqr || n_rows <= 0 || trs <= 0 || !(epsilon >= 0.f))
+    return fail(BSMM_E_ARG, "bsmm_conv_l2_normalize: bad arguments");
+  const cudaStream_t s = (cudaStream_t)stream;
+  const auto* r = reinterpret_cast<const ConvNormRow*>(rows);
+  const int grid = (n_rows + CN_WARPS - 1) / CN_WARPS;
+  BSMM_DISPATCH_DTYPE(x_dtype, T, {
+    if (y_dtype == BSMM_F32) conv_l2n_kernel<T, float><<<grid, 32 * CN_WARPS, 0, s>>>(r, n_rows, trs, (const T*)x, gain, (float*)y, sum_sqr, epsilon);
+    else                     conv_l2n_kernel<T, T><<<grid, 32 * CN_WARPS, 0, s>>>(r, n_rows, trs, (const T*)x, gain, (T*)y, sum_sqr, epsilon);
+  });
+  return check_launch("conv_l2_normalize");
+}
+
+int bsmm_conv_l2_normalize_grad(int x_dtype, int dy_dtype, const int32_t* rows, int n_rows, int trs, const void* dy,
+                                const void* x, const float* gain, const float* sum_sqr, void* dx, float* dgain,
+                                float epsilon, void* stream) {
+  if (!dense_dtype_ok(x_dtype) || (dy_dtype != x_dtype && dy_dtype != BSMM_F32))
+    return fail(BSMM_E_ARG, "bsmm_conv_l2_normalize_grad: dtypes (%d, %d): dy is x's dtype or fp32", x_dtype, dy_dtype);
+  if (!rows || !dy || !x || !sum_sqr || !dx || n_rows <= 0 || trs <= 0 || !(epsilon >= 0.f))
+    return fail(BSMM_E_ARG, "bsmm_conv_l2_normalize_grad: bad arguments");
+  const cudaStream_t s = (cudaStream_t)stream;
+  const auto* r = reinterpret_cast<const ConvNormRow*>(rows);
+  const int grid = (n_rows + CN_WARPS - 1) / CN_WARPS;
+  BSMM_DISPATCH_DTYPE(x_dtype, T, {
+    if (dy_dtype == BSMM_F32) conv_l2n_grad_kernel<T, float><<<grid, 32 * CN_WARPS, 0, s>>>(r, n_rows, trs, (const float*)dy, (const T*)x, gain, sum_sqr, (T*)dx, dgain, epsilon);
+    else                      conv_l2n_grad_kernel<T, T><<<grid, 32 * CN_WARPS, 0, s>>>(r, n_rows, trs, (const T*)dy, (const T*)x, gain, sum_sqr, (T*)dx, dgain, epsilon);
+  });
+  return check_launch("conv_l2_normalize_grad");
 }
 }  // extern "C"

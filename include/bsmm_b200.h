@@ -59,6 +59,11 @@
  *   bsmm_quantize         <- Quantize<T> (src/quantize_op_gpu.cu:192-220), launched by QuantizeOp (src/quantize_op.cc)
  *   bsmm_quantize_stats   <- QuantizationStats<T> (src/quantize_op_gpu.cu:222-239) with QuantizeOp::UpdateExponent
  *                            and LogStatsOp (src/quantize_op.cc:84-111,217-301)
+ *   bsmm_conv_xprop       <- BlocksparseConv / BlocksparseDeconv fprop and bprop: the xconv_blocksparse_* fprop /
+ *                            bprop cubins launched by BlocksparseConvOp (src/blocksparse_conv_op.cc:170-282)
+ *   bsmm_conv_updat       <- the xconv_blocksparse_* updat cubins of the same op (src/blocksparse_conv_op.cc:284-360)
+ *   bsmm_conv_l2_normalize(_grad) <- L2NormalizeKCTRS / L2NormalizeCKTRS, their Gain variants and gradients
+ *                            (src/blocksparse_l2_norm_op_gpu.cu:27-147,378-394,428-586,893-909)
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer except `err` strings is DEVICE memory
@@ -788,6 +793,64 @@ int bsmm_quantize_stats(int n, int dtype, const void* const* xs, const long long
                         float* stats, int ebits, int fbits, int denorm, int mode, int bias_pad, float stdv_mul,
                         float sat_val, float ftz_val, void* workspace, void* stream);
 size_t bsmm_quantize_stats_workspace_bytes(int n, const long long* sizes);
+
+/* ---- block-sparse convolution (the reference's conv module; csrc/conv.cuh, DESIGN.md 7j) ------------------------ */
+
+/*
+ * Tables, all int32 in device memory and built by the host layer (blocksparse_b200/conv.py):
+ *   blocks    [n][8]  per block: out_len, red_len, out channel list offset, red channel list offset, filter offset,
+ *                     so, sr, 0 -- filter element (out c, red j, tap t) is f[offset + c * so + j * sr + t];
+ *   channels          the channel lists the offsets point into (absolute channel ids);
+ *   lut       [P_out][trs]  input position that output position p reads through tap t, or -1 (padding or a stride
+ *                     hole): for a conv's fprop and updat the fprop table, for its bprop the bprop table.
+ * Activations are [N][C][P] contiguous (P = D * H * W); element offsets are 64-bit.
+ *
+ * bsmm_conv_xprop: y[n][out_ch][p] = sum over the block's red channels j and taps t of
+ * x[n][red_ch[j]][lut[p][t]] * f[...], for every block; y has x's dtype. f may be fp32, fp16 or bf16, x likewise, but
+ * fp16 never meets bf16. Blocks come grouped in passes (pass i = blocks [pass_offsets[i], pass_offsets[i + 1]), a host
+ * array) so that no two blocks of one pass share an output channel; every output channel must be covered. One pass is
+ * written straight to y; several are added in pass order into an fp32 buffer (y itself when fp32, else acc, N * C_out
+ * * P_out floats) that is then rounded once into y. fp16 / bf16 x and f of one dtype run wgmma_conv_xprop unless flags
+ * has BSMM_FLAG_FORCE_GENERIC; every other case runs fma_conv_xprop (fp32 FMA). Bitwise reproducible.
+ * Errors before any launch: null pointers, a bad dtype pair, non-positive sizes or passes, an empty pass, a 16-bit y
+ * with several passes and no acc (BSMM_E_ARG); P_out * trs or P_in past 2^31 - 1, N * P_out of 2^37 - 64 or more (its 64-row tiles fill grid.x), or a pass whose
+ * blocks x ceil(max_out / 64) exceeds 65535 (BSMM_E_LIMIT). N = 0 launches nothing.
+ */
+int bsmm_conv_xprop(int x_dtype, int f_dtype, const int32_t* blocks, const int* pass_offsets, int passes, int max_out,
+                    const int32_t* channels, const int32_t* lut, int trs, const void* x, const void* f, void* y, float* acc,
+                    long long N, int C_in, long long P_in, int C_out, long long P_out, int flags, void* stream);
+
+/*
+ * bsmm_conv_updat: df[offset + o * so + j * sr + t] = sum over n, p of e[n][out_ch[o]][p] * x[n][red_ch[j]][lut[p][t]],
+ * for every block (the fprop tables: out = the conv's K, red = its C), rounded once into df's dtype (size_f elements).
+ * The N * P_out rows are cut into chunks of 8192 (a constant, so the sum order does not depend on the GPU); each chunk
+ * writes fp32 partials to workspace (bsmm_conv_updat_workspace_bytes(N * P_out, size_f) bytes) and conv_updat_reduce
+ * adds them in chunk order. e and x: one dtype each of fp32 / fp16 / bf16, fp16 never with bf16; the kernel is
+ * wgmma_conv_updat for e and x both fp16 or both bf16 without BSMM_FLAG_FORCE_GENERIC, else fma_conv_updat. Errors as
+ * bsmm_conv_xprop, plus a null workspace with N > 0, more than 65535 chunks or size_f past 2^31 - 1 (BSMM_E_LIMIT).
+ * N = 0 writes zeros.
+ */
+int bsmm_conv_updat(int e_dtype, int x_dtype, int f_dtype, const int32_t* blocks, int n_blocks, int max_out, int max_red,
+                    const int32_t* channels, const int32_t* lut, int trs, const void* e, const void* x, void* df,
+                    float* workspace, long long N, int C_in, long long P_in, int C_out, long long P_out, long long size_f,
+                    int flags, void* stream);
+size_t bsmm_conv_updat_workspace_bytes(long long rows, long long size_f);
+
+/*
+ * bsmm_conv_l2_normalize: for each row r of rows (int32 [n_rows][4]: base, outer, stride, 0; the row's elements are
+ * x[base + i * stride + t], i < outer, t < trs), sum_sqr[r] = sum x^2 (fp32, fixed order) and
+ * y = x * gain[r] / sqrt(max(sum_sqr[r], epsilon)); gain may be NULL (1). KCTRS rows are one output channel of a block
+ * (stride = trs), CKTRS rows one input channel (stride = C_b * trs). y is x's dtype or fp32. Kernel conv_l2_normalize.
+ * bsmm_conv_l2_normalize_grad: with s = sum dy * x over the row and m = max(sum_sqr, epsilon),
+ * dx = (dy * g - x * [sum_sqr >= epsilon] * s * g / m) / sqrt(m) in x's dtype, and dgain[r] = s / sqrt(m) when dgain
+ * is not NULL; dy is x's dtype or fp32. Kernel conv_l2_normalize_grad. Both: a bad dtype, a null pointer, n_rows <= 0,
+ * trs <= 0 or a negative epsilon give BSMM_E_ARG before any launch.
+ */
+int bsmm_conv_l2_normalize(int x_dtype, int y_dtype, const int32_t* rows, int n_rows, int trs, const void* x,
+                           const float* gain, void* y, float* sum_sqr, float epsilon, void* stream);
+int bsmm_conv_l2_normalize_grad(int x_dtype, int dy_dtype, const int32_t* rows, int n_rows, int trs, const void* dy,
+                                const void* x, const float* gain, const float* sum_sqr, void* dx, float* dgain,
+                                float epsilon, void* stream);
 
 /* ---- measurement helper (the reference's `bench` op attribute, op.cc:99-106) ---------
  * Records two events around whatever the caller enqueues between begin and end.      */

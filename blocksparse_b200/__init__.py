@@ -11,7 +11,9 @@ set_entropy, get_entropy, embedding_lookup; listed in ewops.__all__ and embed.__
 (fused_lstm_gates, split4, concat4, sparse_relu; listed in lstm.__all__), and the rest of its ewops module (add,
 multiply, sigmoid, tanh, float_cast, filter_tensor, add_n, concrete_gate, fancy_gather, reduce_max, assign_add, ...;
 listed in elementwise.__all__ and also reachable as blocksparse_b200.ewops.<name>), and of its quantize module
-(QuantizeSpec, quantize, log_stats, with quantize_state and reset_quantize_states; listed in quantize.__all__), and of its conv module (BlocksparseConv, BlocksparseDeconv; listed in conv.__all__).
+(QuantizeSpec, quantize, log_stats, with quantize_state and reset_quantize_states; listed in quantize.__all__), and of its conv module (BlocksparseConv, BlocksparseDeconv; listed in conv.__all__; ConvEdgeBias,
+conv_edge_bias_init, deconv_edge_bias_init, cwise_linear; listed in conv_bias.__all__ and also reachable as
+blocksparse_b200.conv.<name>).
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
 from .optimize import (AdafactorOptimizer, AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay, blocksparse_norm,
@@ -28,6 +30,7 @@ from .elementwise import (add, add_n, add_n8, assign_add, concrete_gate, concret
                           tanh)
 from .quantize import QuantizeSpec, log_stats, quantize, quantize_state, reset_quantize_states
 from .conv import BlocksparseConv, BlocksparseDeconv
+from .conv_bias import ConvEdgeBias, conv_edge_bias_init, cwise_linear, deconv_edge_bias_init
 from .lut import z_order_2d
 from . import _lib
 

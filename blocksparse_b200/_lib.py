@@ -91,6 +91,12 @@ SIGNATURES = {
     "bsmm_conv_updat_workspace_bytes": (_c.c_size_t, [_ll, _ll]),
     "bsmm_conv_l2_normalize": (_i, [_i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _vp]),
     "bsmm_conv_l2_normalize_grad": (_i, [_i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _f, _vp]),
+    "bsmm_edge_bias": (_i, [_i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _ll, _ll, _i, _i, _vp]),
+    "bsmm_edge_bias_grad": (_i, [_i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _i, _vp]),
+    "bsmm_edge_bias_grad_workspace_bytes": (_c.c_size_t, [_ll, _i, _i, _i]),
+    "bsmm_cwise_linear": (_i, [_i, _vp, _vp, _vp, _vp, _ll, _i, _ll, _i, _i, _vp]),
+    "bsmm_cwise_linear_grad": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _ll, _i, _i, _vp]),
+    "bsmm_cwise_linear_grad_workspace_bytes": (_c.c_size_t, [_ll, _i, _ll]),
     "bsmm_block_norm":(_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),

@@ -359,3 +359,49 @@ class ConvCheckers(object):
             D.append(((u * g + f * (ss >= epsilon) * np.sum(-u * f * g / mx, axis=ax, keepdims=True)) * rn).ravel())
             off += n
         return np.concatenate(D), (None if gain is None else np.concatenate(dg))
+
+
+class EdgeBiasCheckers(object):
+    """Mixin for ConvEdgeBias (conv.py:163-214): needs layout, shape, edgeBiasDim and the position table _pos_edge
+    (the edge pattern of each output position, or -1). x, dy: NumPy arrays of the op's input shape; g, b: self.shape.
+    Written on the position table rather than the reference's per-edge position lists."""
+
+    def _flat(self, a):
+        a = np.asarray(a)
+        N, P = a.shape[0], len(self._pos_edge)
+        return a.reshape(N, P, a.shape[-1]) if self.layout else a.reshape(N, a.shape[1], P)
+
+    def _per_position(self, p):
+        """p (edges, K) or (K, edges) -> per output position, broadcastable against _flat: 1 off the edges."""
+        e = self._pos_edge
+        p = np.asarray(p)
+        if self.layout:
+            return np.where((e >= 0)[:, None], p[np.maximum(e, 0)], 1)[None]
+        return np.where((e >= 0)[None, :], p[:, np.maximum(e, 0)], 1)[None]
+
+    def edge_bias_test(self, x, g, b):
+        if not self.edgeBiasDim:
+            return x
+        mask = (self._pos_edge >= 0)[None, :, None] if self.layout else (self._pos_edge >= 0)[None, None, :]
+        xf = self._flat(x)
+        bias = np.where(mask, self._per_position(b), 0)
+        y = np.where(mask, xf * self._per_position(g) + bias, xf)
+        return y.astype(np.asarray(x).dtype).reshape(np.shape(x))
+
+    def edge_bias_grad_test(self, dy, x, g):
+        """(dx, dg, db): dx = g * dy at edge positions, dg = sum(dy * x), db = sum(dy) per (edge, k); (dy, None, None)
+        without edges."""
+        if not self.edgeBiasDim:
+            return dy, None, None
+        d, xf = self._flat(dy), self._flat(x)
+        mask = (self._pos_edge >= 0)[None, :, None] if self.layout else (self._pos_edge >= 0)[None, None, :]
+        dx = np.where(mask, d * self._per_position(g), d).astype(np.asarray(dy).dtype).reshape(np.shape(dy))
+        E = self.edgeBiasDim
+        onehot = (self._pos_edge[:, None] == np.arange(E)[None, :]).astype(np.float64)     # (P, E)
+        if self.layout:
+            dg = np.einsum("npk,pe->ek", d * xf, onehot)
+            db = np.einsum("npk,pe->ek", d, onehot)
+        else:
+            dg = np.einsum("nkp,pe->ke", d * xf, onehot)
+            db = np.einsum("nkp,pe->ke", d, onehot)
+        return dx, dg.astype(np.float32), db.astype(np.float32)

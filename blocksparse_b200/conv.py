@@ -20,6 +20,9 @@ from .checkers import ConvCheckers
 
 __all__ = ["BlocksparseConv", "BlocksparseDeconv"]
 
+# the reference's conv module also holds these; they live in conv_bias.py and are reachable here too
+from .conv_bias import ConvEdgeBias, conv_edge_bias_init, cwise_linear, deconv_edge_bias_init  # noqa: E402,F401
+
 
 # ---- spatial helpers (reference conv.py:1003-1061) ---------------------------------------------------------------------
 def ceil_div(a, b):

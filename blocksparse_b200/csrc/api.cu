@@ -4,6 +4,7 @@
 #include <climits>
 #include "common.cuh"
 #include "conv.cuh"
+#include "conv_bias.cuh"
 #include "dense_softmax.cuh"
 #include "elementwise.cuh"
 #include "embed.cuh"
@@ -1604,5 +1605,118 @@ int bsmm_conv_l2_normalize_grad(int x_dtype, int dy_dtype, const int32_t* rows, 
     else                      conv_l2n_grad_kernel<T, T><<<grid, 32 * CN_WARPS, 0, s>>>(r, n_rows, trs, (const T*)dy, (const T*)x, gain, sum_sqr, (T*)dx, dgain, epsilon);
   });
   return check_launch("conv_l2_normalize_grad");
+}
+
+// ---- conv edge bias and cwise_linear (csrc/conv_bias.cuh) ---------------------------------------------------------------
+static int eb_args(const char* what, int dtype, int layout, const int32_t* pos_edge, const int32_t* lut, int edges,
+                   int entries, const void* x, const float* g, const void* y, long long N, long long MPQ, int K) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "%s: unsupported dtype code %d", what, dtype);
+  if (layout != 0 && layout != 1) return fail(BSMM_E_ARG, "%s: layout must be 0 (channels first) or 1, got %d", what, layout);
+  if (!pos_edge || !lut || !g || (N > 0 && (!x || !y))) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (N < 0 || MPQ <= 0 || K <= 0 || edges <= 0 || entries < edges || entries > MPQ)
+    return fail(BSMM_E_ARG, "%s: bad sizes (N %lld, MPQ %lld, K %d, edges %d, entries %d)", what, N, MPQ, K, edges, entries);
+  if (MPQ > INT_MAX || 2LL * edges + entries > INT_MAX)
+    return fail(BSMM_E_LIMIT, "%s: %lld positions exceed the int32 tables", what, MPQ);
+  if (edges > 65535) return fail(BSMM_E_LIMIT, "%s: %d edge patterns exceed grid.y", what, edges);
+  if (N > LLONG_MAX / MPQ / K) return fail(BSMM_E_LIMIT, "%s: N * MPQ * K overflows", what);
+  return 0;
+}
+
+int bsmm_edge_bias(int dtype, int layout, const int32_t* pos_edge, const int32_t* lut, int edges, int entries,
+                   const void* x, const float* g, const float* b, void* y, long long N, long long MPQ, int K,
+                   int inference, void* stream) {
+  const char* what = "bsmm_edge_bias";
+  if (int e = eb_args(what, dtype, layout, pos_edge, lut, edges, entries, x, g, y, N, MPQ, K)) return e;
+  if (!b) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (inference && x != y) return fail(BSMM_E_ARG, "%s: inference updates x in place: y must be x", what);
+  if (N == 0) return 0;
+  EbArgs a = {};
+  a.x = x; a.y = y; a.pos_edge = pos_edge; a.lut = lut; a.g = g; a.b = b;
+  a.n = N * MPQ * K; a.N = N; a.MPQ = MPQ; a.K = K; a.E = edges; a.entries = entries; a.layout = layout;
+  const cudaStream_t s = (cudaStream_t)stream;
+  const bool vec = aligned16(x) && aligned16(y) && aligned16(pos_edge);
+  if (inference) {
+    const bool kvec = vec && K % (16 / dtype_size(dtype)) == 0;
+    BSMM_DISPATCH_DTYPE(dtype, T, { return launch_edge_bias_inference<T>(a, kvec, s); });
+  }
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_edge_bias<T>(a, vec, "edge_bias", s); });
+  return 0;
+}
+
+size_t bsmm_edge_bias_grad_workspace_bytes(long long N, int edges, int max_count, int K) {
+  if (N < 0 || edges <= 0 || max_count <= 0 || K <= 0) return 0;
+  long long R;
+  int S;
+  eb_chunks(N, max_count, (long long)edges * K, R, S);
+  return (size_t)2 * S * edges * (size_t)K * sizeof(float);
+}
+
+int bsmm_edge_bias_grad(int dtype, int layout, const int32_t* pos_edge, const int32_t* lut, int edges, int entries,
+                        int max_count, const void* dy, const void* x, const float* g, void* dx, float* dg, float* db,
+                        float* workspace, long long N, long long MPQ, int K, void* stream) {
+  const char* what = "bsmm_edge_bias_grad";
+  if (int e = eb_args(what, dtype, layout, pos_edge, lut, edges, entries, dy, g, dx, N, MPQ, K)) return e;
+  if ((N > 0 && !x) || !dg || !db) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (max_count <= 0 || max_count > entries) return fail(BSMM_E_ARG, "%s: max_count %d", what, max_count);
+  if ((long long)edges * K > INT_MAX) return fail(BSMM_E_LIMIT, "%s: edges * K = %d * %d exceeds int32", what, edges, K);
+  EbArgs a = {};
+  a.x = dy; a.x2 = x; a.y = dx; a.pos_edge = pos_edge; a.lut = lut; a.g = g; a.b = nullptr; a.part = workspace;
+  a.n = N * MPQ * K; a.N = N; a.MPQ = MPQ; a.K = K; a.E = edges; a.entries = entries; a.layout = layout;
+  eb_chunks(N, max_count, (long long)edges * K, a.R, a.S);
+  if (a.S > 0 && !workspace) return fail(BSMM_E_ARG, "%s: null workspace", what);
+  const bool vec = aligned16(dy) && aligned16(dx) && aligned16(pos_edge);
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_edge_bias_grad<T>(a, vec, dg, db, (cudaStream_t)stream); });
+  return 0;
+}
+
+static int cw_args(const char* what, int dtype, const void* x, const float* a, const float* b, long long N, int C,
+                   long long DHW) {
+  if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "%s: unsupported dtype code %d", what, dtype);
+  if (!x && N > 0) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (!a && !b) return fail(BSMM_E_ARG, "%s: neither a gain nor a bias", what);
+  if (N < 0 || C <= 0 || DHW <= 0) return fail(BSMM_E_ARG, "%s: bad sizes (N %lld, C %d, DHW %lld)", what, N, C, DHW);
+  if (N > LLONG_MAX / C / DHW) return fail(BSMM_E_LIMIT, "%s: N * C * DHW overflows", what);
+  if (DHW > 1 && (N * DHW + CW_SEG - 1) / CW_SEG > INT_MAX)
+    return fail(BSMM_E_LIMIT, "%s: N * DHW = %lld exceeds the grid", what, N * DHW);
+  return 0;
+}
+
+int bsmm_cwise_linear(int dtype, const void* x, const float* a, const float* b, void* y, long long N, int C,
+                      long long DHW, int relu, int swap, void* stream) {
+  const char* what = "bsmm_cwise_linear";
+  if (int e = cw_args(what, dtype, x, a, b, N, C, DHW)) return e;
+  if (!y && N > 0) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (N == 0) return 0;
+  CwArgs c = {};
+  c.x = x; c.y = y; c.a = a; c.b = b; c.n = N * C * DHW; c.N = N; c.DHW = DHW; c.C = C; c.relu = relu != 0;
+  c.swap = swap != 0;
+  const bool vec = aligned16(x) && aligned16(y);
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_cwise_linear<T>(c, vec, (cudaStream_t)stream); });
+  return 0;
+}
+
+size_t bsmm_cwise_linear_grad_workspace_bytes(long long N, int C, long long DHW) {
+  if (N < 0 || C <= 0 || DHW <= 0) return 0;
+  return (size_t)2 * cw_parts(N, C, DHW) * C * sizeof(float);
+}
+
+int bsmm_cwise_linear_grad(int dtype, const void* dy, const void* xy, const float* a, const float* b, void* dx,
+                           float* da, float* db, void* workspace, long long N, int C, long long DHW, int relu, int swap,
+                           void* stream) {
+  const char* what = "bsmm_cwise_linear_grad";
+  if (int e = cw_args(what, dtype, dy, a, b, N, C, DHW)) return e;
+  if (!a != !da || !b != !db) return fail(BSMM_E_ARG, "%s: da is written iff a is given, db iff b is", what);
+  const bool rd = a || relu;
+  if (rd && N > 0 && (!xy || !dx)) return fail(BSMM_E_ARG, "%s: null x / y or dx", what);
+  CwArgs c = {};
+  c.x = dy; c.src = xy; c.y = dx; c.a = a; c.b = b; c.part = (float*)workspace; c.n = N * C * DHW; c.N = N;
+  c.DHW = DHW; c.C = C; c.relu = relu != 0; c.swap = swap != 0; c.want_a = a != nullptr; c.want_b = b != nullptr;
+  c.rp = cw_rows_per_part(N, C);
+  c.parts = cw_parts(N, C, DHW);
+  if (c.parts > 0 && !workspace) return fail(BSMM_E_ARG, "%s: null workspace", what);
+  const int V = 16 / dtype_size(dtype);
+  const bool vec = aligned16(dy) && (!rd || (aligned16(xy) && aligned16(dx))) && (DHW == 1 ? C : DHW) % V == 0;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_cwise_linear_grad<T>(c, vec, da, db, (cudaStream_t)stream); });
+  return 0;
 }
 }  // extern "C"

@@ -64,6 +64,14 @@
  *   bsmm_conv_updat       <- the xconv_blocksparse_* updat cubins of the same op (src/blocksparse_conv_op.cc:284-360)
  *   bsmm_conv_l2_normalize(_grad) <- L2NormalizeKCTRS / L2NormalizeCKTRS, their Gain variants and gradients
  *                            (src/blocksparse_l2_norm_op_gpu.cu:27-147,378-394,428-586,893-909)
+ *   bsmm_edge_bias        <- EdgeBiasForward (src/edge_bias_op_gpu.cu:192-219), launched by EdgeBiasOp
+ *                            (src/edge_bias_op.cc:44-122)
+ *   bsmm_edge_bias_grad   <- EdgeBiasBackward (src/edge_bias_op_gpu.cu:221-244), launched by EdgeBiasGradOp
+ *                            (src/edge_bias_op.cc:153-223)
+ *   bsmm_cwise_linear     <- CWiseLinear_Forward (src/cwise_linear_op_gpu.cu:187-205), launched by CWiseLinearOp
+ *                            (src/cwise_linear_op.cc:37-79)
+ *   bsmm_cwise_linear_grad <- CWiseLinear_Backward (src/cwise_linear_op_gpu.cu:208-236), launched by
+ *                            CWiseLinearGradOp (src/cwise_linear_op.cc:125-191)
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer except `err` strings is DEVICE memory
@@ -851,6 +859,70 @@ int bsmm_conv_l2_normalize(int x_dtype, int y_dtype, const int32_t* rows, int n_
 int bsmm_conv_l2_normalize_grad(int x_dtype, int dy_dtype, const int32_t* rows, int n_rows, int trs, const void* dy,
                                 const void* x, const float* gain, const float* sum_sqr, void* dx, float* dgain,
                                 float epsilon, void* stream);
+
+/* ---- conv edge bias and channel-wise linear (the rest of the reference's conv module) ------------------------------ */
+
+/*
+ * Edge bias of a conv output x, [N][MPQ][K] (layout 1, channels last) or [N][K][MPQ] (layout 0): a gain and a bias per
+ * channel and per edge pattern, applied to the output positions whose receptive field hangs over the padding.
+ * Tables, int32 device memory built by the host layer (blocksparse_b200/conv_bias.py):
+ *   pos_edge [MPQ]            the edge pattern of each output position, or -1;
+ *   lut      [2 edges + entries]  the reference's table: (offset, count) per edge, then the positions of each edge
+ *                             (offsets count from the table's start; entries positions in all).
+ * g and b are fp32, [edges][K] for layout 1 and [K][edges] for layout 0.
+ * bsmm_edge_bias: y = x * g + b at edge positions and x elsewhere, formed in fp32 and rounded once, in one streaming
+ * pass (kernel edge_bias). The reference copies x to y and then runs a second kernel over the edges. inference != 0
+ * updates x in place over the edge positions only, through lut (each entry finds its edge in lut's header; y must be
+ * x; kernel edge_bias_inference). x and y may be NULL when N = 0.
+ * Errors before any launch (BSMM_E_ARG): a bad dtype or layout, a null pointer, N < 0, MPQ <= 0, K <= 0, edges <= 0,
+ * entries outside [edges, MPQ], inference with y != x. BSMM_E_LIMIT: MPQ or the table
+ * past 2^31 - 1, more than 65535 edges. N = 0 launches nothing. 64-bit element offsets.
+ */
+int bsmm_edge_bias(int dtype, int layout, const int32_t* pos_edge, const int32_t* lut, int edges, int entries,
+                   const void* x, const float* g, const float* b, void* y, long long N, long long MPQ, int K,
+                   int inference, void* stream);
+
+/*
+ * Gradient of bsmm_edge_bias: dx = dy * g at edge positions and dy elsewhere, into dx in one streaming pass (the
+ * reference scales dy in place); dg = sum dy * x and db = sum dy per (edge, k) over N and the edge's positions, fp32 in
+ * g's layout. The (n, position) pairs of each edge are cut into chunks whose size depends on (N, max_count, edges, K)
+ * only (max_count: the largest count in lut); each chunk writes fp32 partials to workspace
+ * (bsmm_edge_bias_grad_workspace_bytes) and a last kernel adds them in a fixed order, so dg and db are bitwise
+ * reproducible. The reference gives each (edge, k) one thread or warp over all of N. Errors as bsmm_edge_bias, plus a
+ * null x / dg / db, max_count outside [1, entries], a null workspace when N > 0 (BSMM_E_ARG), edges * K past 2^31 - 1
+ * (BSMM_E_LIMIT). N = 0 writes zeros to dg and db. Kernel: edge_bias_grad.
+ */
+int bsmm_edge_bias_grad(int dtype, int layout, const int32_t* pos_edge, const int32_t* lut, int edges, int entries,
+                        int max_count, const void* dy, const void* x, const float* g, void* dx, float* dg, float* db,
+                        float* workspace, long long N, long long MPQ, int K, void* stream);
+size_t bsmm_edge_bias_grad_workspace_bytes(long long N, int edges, int max_count, int K);
+
+/*
+ * Channel-wise linear on x [N][C][DHW] (NC(DHW), DHW the product of the spatial dims, 1 for rank 2): y = a * x + b, or
+ * a * (x + b) with swap, then max(y, 0) with relu; formed in fp32 and rounded once. a and b are fp32 [C], either may
+ * be NULL (not both). One flat streaming kernel with 16-byte accesses where the pointers allow (kernel cwise_linear);
+ * the reference launches one CTA per (c, n), 32 threads wide when DHW is small.
+ * Errors before any launch (BSMM_E_ARG): a bad dtype, null x / y, a and b both NULL, N < 0, C <= 0, DHW <= 0;
+ * BSMM_E_LIMIT: N * C * DHW past 2^63 - 1. N = 0 launches nothing. 64-bit element offsets.
+ */
+int bsmm_cwise_linear(int dtype, const void* x, const float* a, const float* b, void* y, long long N, int C,
+                      long long DHW, int relu, int swap, void* stream);
+
+/*
+ * Gradient of bsmm_cwise_linear. With a gain, xy is x: dy' = dy masked by the forward's relu (the same fp32 expression),
+ * dx = dy' * a, da = sum dy' * x (dy' * (x + b) with swap), db = sum dy' (dy' * a with swap). Without a gain, xy is y
+ * (read for relu only): dx = dy masked by y > 0, db = sum of that; without relu too, dx is dy itself and neither xy nor
+ * dx is touched (both may be NULL). da is written iff a is given, db iff b is (fp32 [C]). The sums go into fp32
+ * partials over fixed chunks of each channel (rows of (N, C) when DHW = 1, 8192-element segments of the channel's
+ * N * DHW otherwise), in workspace (bsmm_cwise_linear_grad_workspace_bytes); a last kernel adds them in a fixed order,
+ * so the result is bitwise reproducible, and every channel is split across many CTAs (the reference gives each one CTA).
+ * Errors as bsmm_cwise_linear, plus da / db not matching a / b, a null xy or dx where read, a null workspace with
+ * N > 0 (BSMM_E_ARG). N = 0 writes zeros. Kernels: cwise_linear_grad_nc (DHW = 1), cwise_linear_grad_ncdhw.
+ */
+int bsmm_cwise_linear_grad(int dtype, const void* dy, const void* xy, const float* a, const float* b, void* dx,
+                           float* da, float* db, void* workspace, long long N, int C, long long DHW, int relu, int swap,
+                           void* stream);
+size_t bsmm_cwise_linear_grad_workspace_bytes(long long N, int C, long long DHW);
 
 /* ---- measurement helper (the reference's `bench` op attribute, op.cc:99-106) ---------
  * Records two events around whatever the caller enqueues between begin and end.      */

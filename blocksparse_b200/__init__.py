@@ -13,9 +13,10 @@ multiply, sigmoid, tanh, float_cast, filter_tensor, add_n, concrete_gate, fancy_
 listed in elementwise.__all__ and also reachable as blocksparse_b200.ewops.<name>), and of its quantize module
 (QuantizeSpec, quantize, log_stats, with quantize_state and reset_quantize_states; listed in quantize.__all__), and of its conv module (BlocksparseConv, BlocksparseDeconv; listed in conv.__all__; ConvEdgeBias,
 conv_edge_bias_init, deconv_edge_bias_init, cwise_linear; listed in conv_bias.__all__ and also reachable as
-blocksparse_b200.conv.<name>).
+blocksparse_b200.conv.<name>), and its top-level dw_matmul_large_n (importable from here, not listed in __all__).
 """
-from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, group_param_grads)
+from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, dw_matmul_large_n,
+                     group_param_grads)
 from .optimize import (AdafactorOptimizer, AdamOptimizer, ClipGlobalNorm, Ema, blocksparse_l2_decay, blocksparse_norm,
                        blocksparse_prune, clip_by_global_norm, global_norm)
 from .transformer import (BlocksparseTransformer, masked_softmax, masked_top_k_softmax, rectified_top_k, softmax,

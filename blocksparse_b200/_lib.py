@@ -97,6 +97,8 @@ SIGNATURES = {
     "bsmm_cwise_linear": (_i, [_i, _vp, _vp, _vp, _vp, _ll, _i, _ll, _i, _i, _vp]),
     "bsmm_cwise_linear_grad": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _ll, _i, _i, _vp]),
     "bsmm_cwise_linear_grad_workspace_bytes": (_c.c_size_t, [_ll, _i, _ll]),
+    "bsmm_dw_matmul_large_n": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _vp, _i, _vp]),
+    "bsmm_dw_matmul_large_n_workspace_bytes": (_c.c_size_t, [_i, _ll, _i, _i]),
     "bsmm_block_norm":(_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),

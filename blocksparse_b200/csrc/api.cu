@@ -5,6 +5,7 @@
 #include "common.cuh"
 #include "conv.cuh"
 #include "conv_bias.cuh"
+#include "dense_dw.cuh"
 #include "dense_softmax.cuh"
 #include "elementwise.cuh"
 #include "embed.cuh"
@@ -1718,5 +1719,62 @@ int bsmm_cwise_linear_grad(int dtype, const void* dy, const void* xy, const floa
   const bool vec = aligned16(dy) && (!rd || (aligned16(xy) && aligned16(dx))) && (DHW == 1 ? C : DHW) % V == 0;
   BSMM_DISPATCH_DTYPE(dtype, T, { return launch_cwise_linear_grad<T>(c, vec, da, db, (cudaStream_t)stream); });
   return 0;
+}
+// ---- dw_matmul_large_n ------------------------------------------------------------------------------------------
+// Workspace of either route the call may take: a 16-bit call whose shape fits the wgmma route still runs the FMA one
+// with misaligned pointers or BSMM_FLAG_FORCE_GENERIC.
+size_t bsmm_dw_matmul_large_n_workspace_bytes(int dtype, long long N, int C, int K) {
+  if (dtype != BSMM_F32 && dtype != BSMM_F16 && dtype != BSMM_BF16) return 0;
+  if (N < 0 || C <= 0 || K <= 0) return 0;
+  const size_t fma = dense_dw_workspace(N, C, K, false);
+  if (!dense_dw_tc_shape(dtype, N, C, K)) return fma;
+  const size_t tc = dense_dw_workspace(N, C, K, true);
+  return tc > fma ? tc : fma;
+}
+
+int bsmm_dw_matmul_large_n(int dtype, const void* x, const void* e, float* u, long long N, int C, int K,
+                           void* workspace, int flags, void* stream) {
+  const char* what = "bsmm_dw_matmul_large_n";
+  if (dtype != BSMM_F32 && dtype != BSMM_F16 && dtype != BSMM_BF16) return fail(BSMM_E_ARG, "%s: bad dtype %d", what, dtype);
+  if (N < 0 || C < 0 || K < 0) return fail(BSMM_E_ARG, "%s: negative size (N=%lld, C=%d, K=%d)", what, N, C, K);
+  if ((flags & BSMM_FLAG_FORCE_GENERIC) && (flags & BSMM_FLAG_FORCE_TC)) return fail(BSMM_E_ARG, "%s: contradictory flags", what);
+  if (flags & BSMM_FLAG_FORCE_TC) {
+    if (dtype == BSMM_F32) return fail(BSMM_E_ARG, "%s: no wgmma kernel for fp32 (it runs on CUDA cores, as in the reference)", what);
+    if (!dense_dw_tc_shape(dtype, N, C, K))
+      return fail(BSMM_E_ARG, "%s: the wgmma kernel needs C %% 8 == 0, K %% 8 == 0 and N < 2^31 (C=%d, K=%d, N=%lld)", what, C, K, N);
+  }
+  if (C == 0 || K == 0) return 0;
+  if (!u) return fail(BSMM_E_ARG, "%s: null u", what);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (N == 0) {
+    cudaError_t err = cudaMemsetAsync(u, 0, (size_t)C * K * sizeof(float), s);
+    if (err != cudaSuccess) { cudaGetLastError(); return fail((int)err, "%s: %s", what, cudaGetErrorString(err)); }
+    kernel_name_slot() = "memset_dense_dw";
+    return 0;
+  }
+  if (!x || !e) return fail(BSMM_E_ARG, "%s: null x or e", what);
+  const bool aligned = (((uintptr_t)x | (uintptr_t)e) & 15) == 0 && ((uintptr_t)u & 7) == 0 && ((uintptr_t)workspace & 7) == 0;
+  bool tc = false;
+  if (!(flags & BSMM_FLAG_FORCE_GENERIC) && dense_dw_tc_shape(dtype, N, C, K)) {
+    if (!aligned) fail(0, "x and e must be 16-byte aligned, u and the workspace 8-byte aligned, for TMA");
+    tc = aligned && wgmma_device();
+    if (!tc) {
+      if (flags & BSMM_FLAG_FORCE_TC) {
+        char why[512];
+        snprintf(why, sizeof(why), "%s", err_buf());
+        return fail(BSMM_E_ARG, "%s: no wgmma kernel for this call (%s)", what, why);
+      }
+      note_fallback(what, dtype);
+    }
+  } else if (dtype != BSMM_F32 && !(flags & BSMM_FLAG_FORCE_GENERIC)) {
+    fail(0, "C and K must be multiples of 8 and N below 2^31");
+    note_fallback(what, dtype);
+  }
+  const DwSplit d = dense_dw_split(N, C, K, tc);
+  if (d.tiles * d.S > INT_MAX) return fail(BSMM_E_LIMIT, "%s: more than 2^31 - 1 output tiles", what);
+  if (d.S > 1 && !workspace)
+    return fail(BSMM_E_ARG, "%s: null workspace (bsmm_dw_matmul_large_n_workspace_bytes gives its size)", what);
+  if (!device_info().ok) return fail(BSMM_E_NODEV, "no CUDA device");
+  return dense_dw_run(tc, dtype, x, e, u, N, C, K, (float*)workspace, s);
 }
 }  // extern "C"

@@ -6,6 +6,7 @@ operates on torch tensors and calls the sm_90a kernels through the C ABI in
 include/bsmm_b200.h.  There is no CPU path: tensors must live on a CUDA device.
 """
 import ctypes
+import math
 import os
 
 import numpy as np
@@ -594,6 +595,55 @@ def block_reduced_full_dw(pairs, scale=1.0, norm="max", group_size=8, bsize=32, 
         chunk = pairs[off:off + group_size]
         dw, _, _ = blocksparse_reduced_dw([p[0] for p in chunk], [p[1] for p in chunk], scale, dw, bsize=bsize, norm=norm, axis=axis)
     return dw
+
+
+_DW_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def dw_matmul_large_n(x, e, *, flags=0):
+    """U = X^T . E in fp32 over a very large effective minibatch (the reference's top-level dw_matmul_large_n,
+    src/matmul_op.cc DwMatmulLargeN), e.g. the weight gradient of a dense layer summed over batch x time.
+
+    x (..., C) and e (..., K) have the same rank and the same leading dims, whose product N is the minibatch; both are
+    fp32, fp16 or bf16, of one dtype, on one CUDA device.  Returns a new fp32 (C, K) tensor.  Any C, K, N >= 0 work
+    (the reference needs C, K % 4 == 0 and N % 32 == 0): N = 0 gives zeros, C = 0 or K = 0 an empty tensor.
+
+    The minibatch is split into segments whose number depends on (N, C, K) and the route only, each reduced in fp32,
+    and the segments' partials are added in a fixed order: the result is bitwise reproducible on any device, stream or
+    SM margin.  fp16 / bf16 with C and K multiples of 8 run on a wgmma kernel, everything else (fp32 included) on a true
+    fp32 FMA kernel.  `flags` takes _lib.FLAG_FORCE_GENERIC / FLAG_FORCE_TC, as BlocksparseMatMul.fprop does.
+
+    The op has no gradient, as in the reference: the result never requires grad.
+    """
+    if not torch.is_tensor(x) or not torch.is_tensor(e):
+        raise ValueError("dw_matmul_large_n takes two tensors")
+    if x.dtype != e.dtype:
+        raise ValueError("dw_matmul_large_n: x is %s, e is %s" % (x.dtype, e.dtype))
+    if x.dtype not in _DW_DTYPES:
+        raise ValueError("dw_matmul_large_n takes float32, float16 or bfloat16, got %s" % (x.dtype,))
+    if x.dim() < 1 or x.dim() != e.dim() or x.shape[:-1] != e.shape[:-1]:
+        raise ValueError("dw_matmul_large_n: x %s and e %s must have one rank and the same leading dims"
+                         % (tuple(x.shape), tuple(e.shape)))
+    if not x.is_cuda or not e.is_cuda:
+        raise ValueError("dw_matmul_large_n needs CUDA tensors (no CPU path)")
+    if x.device != e.device:
+        raise ValueError("dw_matmul_large_n: x lives on %s, e on %s" % (x.device, e.device))
+    C, K = x.shape[-1], e.shape[-1]
+    N = math.prod(x.shape[:-1])
+    u = torch.empty((C, K), dtype=torch.float32, device=x.device)
+    if C == 0 or K == 0:
+        return u
+    x2 = x.detach().reshape(N, C).contiguous()
+    e2 = e.detach().reshape(N, K).contiguous()
+    lib = _lib.load()
+    code = _lib.dtype_code(x.dtype)
+    with torch.cuda.device(x.device):
+        nbytes = lib.bsmm_dw_matmul_large_n_workspace_bytes(code, N, C, K)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device) if nbytes else None
+        rc = lib.bsmm_dw_matmul_large_n(code, x2.data_ptr(), e2.data_ptr(), u.data_ptr(), N, C, K, _lib.ptr(ws),
+                                        int(flags), _lib.stream_ptr())
+    _lib.check(rc, "bsmm_dw_matmul_large_n")
+    return u
 
 
 class _GatherRows(torch.autograd.Function):

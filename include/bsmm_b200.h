@@ -72,6 +72,8 @@
  *                            (src/cwise_linear_op.cc:37-79)
  *   bsmm_cwise_linear_grad <- CWiseLinear_Backward (src/cwise_linear_op_gpu.cu:208-236), launched by
  *                            CWiseLinearGradOp (src/cwise_linear_op.cc:125-191)
+ *   bsmm_dw_matmul_large_n <- Gemm_TN (src/matmul_op_gpu.cu:309-364), launched by DwMatmulLargeNOp
+ *                            (src/matmul_op.cc:47-87)
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer except `err` strings is DEVICE memory
@@ -923,6 +925,27 @@ int bsmm_cwise_linear_grad(int dtype, const void* dy, const void* xy, const floa
                            float* da, float* db, void* workspace, long long N, int C, long long DHW, int relu, int swap,
                            void* stream);
 size_t bsmm_cwise_linear_grad_workspace_bytes(long long N, int C, long long DHW);
+
+/* ---- dense weight gradient over a very large minibatch (the reference's top-level dw_matmul_large_n) --------------- */
+
+/*
+ * u (fp32 [C][K]) = x^T e, x [N][C] and e [N][K] row-major, both of dtype; replaces Gemm_TN (src/matmul_op_gpu.cu:309-364)
+ * as DwMatmulLargeNOp (src/matmul_op.cc:47-87) launches it, without its limits C, K % 4 == 0 and N % 32 == 0.
+ * The minibatch is split into S segments, S a function of (N, C, K, route) only (never of the SM count); with S > 1
+ * every (output tile, segment) writes an fp32 partial into workspace and a second kernel adds the partials in segment
+ * order, so u is bitwise reproducible (the reference adds its segments with atomics).
+ * Routes (bsmm_last_kernel): wgmma_dense_dw for fp16 / bf16 with C % 8 == 0, K % 8 == 0, N < 2^31, x and e 16-byte
+ * and u and workspace 8-byte aligned; fma_dense_dw (true fp32 FMA) otherwise. BSMM_FLAG_FORCE_GENERIC takes the FMA
+ * route; BSMM_FLAG_FORCE_TC on a call the wgmma route cannot take is BSMM_E_ARG.
+ * Errors before any launch (BSMM_E_ARG): a bad dtype, negative sizes, contradictory flags, a null u (C, K > 0), null x
+ * or e (N > 0), a null workspace where S > 1. C = 0 or K = 0 launches nothing; N = 0 clears u (memset_dense_dw).
+ * 64-bit offsets.
+ */
+int bsmm_dw_matmul_large_n(int dtype, const void* x, const void* e, float* u, long long N, int C, int K,
+                           void* workspace, int flags, void* stream);
+/* Bytes of workspace bsmm_dw_matmul_large_n needs for (dtype, N, C, K) on whichever route it may take (0 when S == 1
+ * on both, and for bad arguments). At most 264 * 128 * 256 * 4 = 34,603,008 bytes, whatever N is. */
+size_t bsmm_dw_matmul_large_n_workspace_bytes(int dtype, long long N, int C, int K);
 
 /* ---- measurement helper (the reference's `bench` op attribute, op.cc:99-106) ---------
  * Records two events around whatever the caller enqueues between begin and end.      */

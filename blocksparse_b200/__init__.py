@@ -8,7 +8,8 @@ softmax_cross_entropy, transpose_0213, transpose_2d), of its norms module (layer
 (AdamOptimizer, clip_by_global_norm, global_norm, Ema; AdafactorOptimizer, importable from here and from
 blocksparse_b200.optimize but not listed in __all__), and of its ewops and embed modules (bias_relu, dropout,
 set_entropy, get_entropy, embedding_lookup; listed in ewops.__all__ and embed.__all__), and of its lstm module
-(fused_lstm_gates, split4, concat4, sparse_relu; listed in lstm.__all__), and the rest of its ewops module (add,
+(fused_lstm_gates, split4, concat4, sparse_relu; listed in lstm.__all__; grouped_lstm, FusedBasicLSTMCell; listed in
+lstm_layer.__all__ and also reachable as blocksparse_b200.lstm.<name>), and the rest of its ewops module (add,
 multiply, sigmoid, tanh, float_cast, filter_tensor, add_n, concrete_gate, fancy_gather, reduce_max, assign_add, ...;
 listed in elementwise.__all__ and also reachable as blocksparse_b200.ewops.<name>), and of its quantize module
 (QuantizeSpec, quantize, log_stats, with quantize_state and reset_quantize_states; listed in quantize.__all__), and of its conv module (BlocksparseConv, BlocksparseDeconv; listed in conv.__all__; ConvEdgeBias,
@@ -25,6 +26,7 @@ from .norms import layer_norm
 from .ewops import bias_relu, dropout, get_entropy, set_entropy
 from .embed import embedding_lookup
 from .lstm import concat4, fused_lstm_gates, sparse_relu, split4
+from .lstm_layer import FusedBasicLSTMCell, grouped_lstm
 from .elementwise import (add, add_n, add_n8, assign_add, concrete_gate, concrete_gate_infer, divide, elu, exp,
                           fancy_gather, fast_gelu, filter_tensor, float_cast, gelu, log, maximum, minimum, multiply,
                           negative, reciprocal, reduce_max, relu, scale_tensor, sigmoid, sqrt, square, subtract, swish,

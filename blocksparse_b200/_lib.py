@@ -58,6 +58,11 @@ SIGNATURES = {
     "bsmm_lstm_gates": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp, _vp, _vp, _ll, _i, _f, _vp]),
     "bsmm_lstm_gates_grad": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i,
                                   _f, _vp]),
+    "bsmm_lstm_ln_gates": (_i, [_i, _i, _vp, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _ll, _i, _f, _f, _vp]),
+    "bsmm_lstm_ln_gates_grad": (_i, [_i, _i, _vp, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _ll, _i,
+                                     _f, _vp]),
+    "bsmm_lstm_ln_gates_grad_reduce": (_i, [_i, _vp, _ll, _i, _vp, _vp, _vp]),
+    "bsmm_lstm_ln_gates_workspace_bytes": (_c.c_size_t, [_ll, _i]),
     "bsmm_sparse_relu": (_i, [_i, _vp, _vp, _ll, _i, _f, _vp]),
     "bsmm_relu_mask_grad": (_i, [_i, _vp, _vp, _vp, _ll, _vp]),
     "bsmm_ew_forward": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _ll, _ll, _f, _vp]),

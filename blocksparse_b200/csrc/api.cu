@@ -749,6 +749,71 @@ int bsmm_lstm_gates_grad(int dtype, int bdtype, const void* c, const void* i, co
   return 0;
 }
 
+static int lstm_ln_args(const char* what, int dtype, int gdtype, long long N, int K, long long stride) {
+  if (!dense_dtype_ok(dtype) || !dense_dtype_ok(gdtype))
+    return fail(BSMM_E_ARG, "%s: unsupported dtype codes %d, %d", what, dtype, gdtype);
+  if (N < 0 || K <= 0 || stride < 4LL * K)
+    return fail(BSMM_E_ARG, "%s: bad sizes N %lld, K %d, stride %lld", what, N, K, stride);
+  if (K > 0x7fffffff / 4) return fail(BSMM_E_LIMIT, "%s: 4K exceeds 2^31 - 1 (K %d)", what, K);
+  if (N > LLONG_MAX / stride) return fail(BSMM_E_LIMIT, "%s: more than 2^63 elements", what);
+  return 0;
+}
+
+size_t bsmm_lstm_ln_gates_workspace_bytes(long long N, int K) {
+  if (N <= 0 || K <= 0 || K > 0x7fffffff / 4) return 0;
+  int rpu, parts;
+  lng_partition(N, rpu, parts);
+  return (size_t)2 * parts * 4 * K * sizeof(float);
+}
+
+int bsmm_lstm_ln_gates(int dtype, int gdtype, const void* c, const void* z, long long stride, const void* g,
+                       const void* b, void* c_next, void* h_next, float* mean, float* rstd, long long N, int K,
+                       float epsilon, float forget_bias, void* stream) {
+  if (int e = lstm_ln_args("bsmm_lstm_ln_gates", dtype, gdtype, N, K, stride)) return e;
+  if (!(epsilon >= 0.f)) return fail(BSMM_E_ARG, "bsmm_lstm_ln_gates: epsilon must be >= 0");
+  if (!c || !z || !g || !b || !c_next || !h_next || !mean || !rstd)
+    return fail(BSMM_E_ARG, "bsmm_lstm_ln_gates: null pointer");
+  if (N == 0) return 0;
+  LnGatesArgs a = {};
+  a.c = c; a.z = z; a.g = g; a.b = b; a.c_out = c_next; a.h_out = h_next; a.mean = mean; a.rstd = rstd;
+  a.N = N; a.zs = stride; a.K = K; a.gdt = gdtype; a.eps = epsilon; a.forget_bias = forget_bias;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_lstm_ln_gates<T>(a, false, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_lstm_ln_gates_grad(int dtype, int gdtype, const void* c, const void* z, long long stride, const void* g,
+                            const void* b, const float* mean, const float* rstd, const void* ec, const void* eh,
+                            void* dc, void* dz, void* workspace, int accumulate, long long N, int K, float forget_bias,
+                            void* stream) {
+  if (int e = lstm_ln_args("bsmm_lstm_ln_gates_grad", dtype, gdtype, N, K, stride)) return e;
+  if (!c || !z || !g || !b || !mean || !rstd || !dc || !dz || !workspace)
+    return fail(BSMM_E_ARG, "bsmm_lstm_ln_gates_grad: null pointer");
+  if (N == 0) return 0;
+  LnGatesArgs a = {};
+  a.c = c; a.z = z; a.g = g; a.b = b; a.mean = (float*)mean; a.rstd = (float*)rstd; a.ec = ec; a.eh = eh;
+  a.c_out = dc; a.h_out = dz; a.ws = (float*)workspace; a.accumulate = accumulate != 0;
+  a.N = N; a.zs = stride; a.K = K; a.gdt = gdtype; a.forget_bias = forget_bias;
+  BSMM_DISPATCH_DTYPE(dtype, T, { return launch_lstm_ln_gates<T>(a, true, (cudaStream_t)stream); });
+  return 0;
+}
+
+int bsmm_lstm_ln_gates_grad_reduce(int gdtype, const void* workspace, long long N, int K, void* dg, void* db,
+                                   void* stream) {
+  const char* what = "bsmm_lstm_ln_gates_grad_reduce";
+  if (!dense_dtype_ok(gdtype)) return fail(BSMM_E_ARG, "%s: unsupported dtype code %d", what, gdtype);
+  if (N < 0 || K <= 0) return fail(BSMM_E_ARG, "%s: bad sizes N %lld, K %d", what, N, K);
+  if (K > 0x7fffffff / 4) return fail(BSMM_E_LIMIT, "%s: 4K exceeds 2^31 - 1 (K %d)", what, K);
+  if (!workspace || !dg || !db) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (N == 0) return 0;
+  int rpu, parts;
+  lng_partition(N, rpu, parts);
+  BSMM_DISPATCH_DTYPE(gdtype, G, {
+    ln_reduce_partials_kernel<G><<<(unsigned)((4LL * K + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        (const float*)workspace, parts, 4 * K, dg, db);
+  });
+  return check_launch("lstm_ln_gates_grad_reduce");
+}
+
 int bsmm_sparse_relu(int dtype, const void* x, void* y, long long N, int K, float alpha, void* stream) {
   if (!dense_dtype_ok(dtype)) return fail(BSMM_E_ARG, "bsmm_sparse_relu: unsupported dtype code %d", dtype);
   if (N < 0 || K <= 0) return fail(BSMM_E_ARG, "bsmm_sparse_relu: bad sizes N %lld, K %d", N, K);

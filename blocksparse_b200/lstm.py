@@ -2,9 +2,9 @@
 :22-69, split4 / concat4 :72-91, sparse_relu :94-117), on torch tensors, calling the sm_90a kernels of csrc/lstm.cuh
 through bsmm_lstm_gates / bsmm_lstm_gates_grad / bsmm_sparse_relu / bsmm_relu_mask_grad.
 
-The reference's grouped_lstm, group_lstm_grads and FusedBasicLSTMCell are TensorFlow variable-scope and graph-surgery
-code with no eager counterpart and are not carried here; an unrolled loop of BlocksparseMatMul, layer_norm and
-fused_lstm_gates does their work.
+The reference's grouped_lstm and FusedBasicLSTMCell live in lstm_layer.py and are reachable here too (not listed in
+__all__). Its group_lstm_grads is TensorFlow graph surgery and is not carried: grouped_lstm's backward forms the
+kernel's gradient as one dw_matmul_large_n over all steps, the work that rewrite does.
 """
 import numbers
 
@@ -263,3 +263,7 @@ def sparse_relu(x, alpha=1.0):
         raise ValueError("sparse_relu: the last dim has %d entries, at most 2^31 - 1 are supported" % K)
     N = x.numel() // K if K else 0
     return _SparseReluFunction.apply(x.contiguous(), N, max(K, 1), float(alpha))
+
+
+# the reference's lstm module also holds these; they live in lstm_layer.py and are reachable here too
+from .lstm_layer import FusedBasicLSTMCell, grouped_lstm  # noqa: E402,F401

@@ -32,6 +32,8 @@
  *   bsmm_dropout_mask     <- GenDropoutMask (src/ew_op.cc:524-591)
  *   bsmm_dropout_apply    <- ApplyDropoutMask (src/ew_op.cc:593-691)
  *   bsmm_lstm_gates(_grad) <- LSTMGates / LSTMGates4 and their gradients (src/lstm_op.cc)
+ *   bsmm_lstm_ln_gates(_grad, _grad_reduce) <- LayerNormSegmentedForward_NC / _Backward_NC fused with
+ *                            LSTM_Gates_Forward / _Backward, the per-step ops of grouped_lstm (blocksparse/lstm.py:153-199)
  *   bsmm_sparse_relu      <- SparseRelu (src/lstm_op.cc:430-467)
  *   bsmm_relu_mask_grad   <- ew_dx_dzza with RELU_OP, sparse_relu's gradient (blocksparse/lstm.py:106-109)
  *   bsmm_ew_forward / bsmm_ew_backward / bsmm_gain_mul_grad <- EW_Forward / EW_Backward (src/ew_op_gpu.cu:306-536)
@@ -498,6 +500,47 @@ int bsmm_lstm_gates(int dtype, int bdtype, const void* c, const void* i, const v
 int bsmm_lstm_gates_grad(int dtype, int bdtype, const void* c, const void* i, const void* u, const void* f,
                          const void* o, long long stride, const void* bias, const void* ec, const void* eh, void* dc,
                          void* di, void* du, void* df, void* d_o, long long N, int K, float forget_bias, void* stream);
+
+/*
+ * bsmm_layer_norm(z, g, b, axis 1, segments 4, epsilon) followed by bsmm_lstm_gates(c, ., forget_bias) in one pass over
+ * each row. z: (N, 4K) of dtype, the gates i, u, f, o in that column order, row n at z + n * stride (elements, stride
+ * >= 4K, so a padded buffer works); c, c_next, h_next: (N, K) of dtype, contiguous; g, b: 4K entries of gdtype (F32,
+ * F16 or BF16), read as fp32. Each segment's mean and rstd = 1 / sqrt(var + epsilon) are formed in fp32 as
+ * bsmm_layer_norm does (two passes, never E[x^2] - E[x]^2) and written to mean and rstd, fp32 [N][4]. The normalised
+ * value xhat g + b stays in fp32 and goes straight into the gates (the two-op composition rounds it to dtype first);
+ * c_next and h_next are rounded once. Replaces LayerNormSegmentedForward_NC (src/layer_norm_nc_op_gpu.cu) followed by
+ * LSTM_Gates_Forward (src/lstm_op_gpu.cu:283-339). Any alignment, 64-bit offsets. A bad dtype, N < 0, K <= 0,
+ * stride < 4K, epsilon < 0 or a null pointer: BSMM_E_ARG before any launch; 4K >= 2^31: BSMM_E_LIMIT. N = 0 launches
+ * nothing. Kernel: lstm_ln_gates (a CTA per row).
+ */
+int bsmm_lstm_ln_gates(int dtype, int gdtype, const void* c, const void* z, long long stride, const void* g,
+                       const void* b, void* c_next, void* h_next, float* mean, float* rstd, long long N, int K,
+                       float epsilon, float forget_bias, void* stream);
+
+/*
+ * dc (N, K) and dz (z's layout; only the 4K real columns of each row are written) of bsmm_lstm_ln_gates, given its
+ * c, z, g, b, mean and rstd and the incoming gradients ec of c_next and eh of h_next; either may be NULL and reads as
+ * zero. The gates and xhat are recomputed. In the same pass the fp32 partial sums of dg and db go to `workspace`
+ * (bsmm_lstm_ln_gates_workspace_bytes(N, K) bytes), laid out [2][P][4K] (dg's P rows, then db's) with P a function of
+ * N only; accumulate != 0 adds to what the buffer holds instead of overwriting it, so the backward of T steps of one
+ * shape on one stream sums into one buffer, and bsmm_lstm_ln_gates_grad_reduce turns it into dg and db once. Each
+ * partial slot belongs to one CTA per call: no atomics, bitwise reproducible. Replaces LayerNormSegmentedBackward_NC
+ * (src/layer_norm_nc_op_gpu.cu) after LSTM_Gates_Backward (src/lstm_op_gpu.cu:340-404). Errors and limits as
+ * bsmm_lstm_ln_gates (ec, eh may be NULL; workspace may not). N = 0 launches nothing. Kernel: lstm_ln_gates_grad.
+ */
+int bsmm_lstm_ln_gates_grad(int dtype, int gdtype, const void* c, const void* z, long long stride, const void* g,
+                            const void* b, const float* mean, const float* rstd, const void* ec, const void* eh,
+                            void* dc, void* dz, void* workspace, int accumulate, long long N, int K, float forget_bias,
+                            void* stream);
+
+/* dg and db (4K entries of gdtype) from the partials bsmm_lstm_ln_gates_grad left in workspace for (N, K), added in
+ * partial order (the fixed-order reduce of bsmm_layer_norm_grad). A bad gdtype, N < 0, K <= 0 or a null pointer:
+ * BSMM_E_ARG; N = 0 launches nothing. Kernel: lstm_ln_gates_grad_reduce. */
+int bsmm_lstm_ln_gates_grad_reduce(int gdtype, const void* workspace, long long N, int K, void* dg, void* db,
+                                   void* stream);
+
+/* Bytes of workspace bsmm_lstm_ln_gates_grad needs for (N, K): 0 for bad arguments or N = 0. */
+size_t bsmm_lstm_ln_gates_workspace_bytes(long long N, int K);
 
 /*
  * y = max(x - (mean + alpha std), 0) along each row of x, y (N, K) of dtype, contiguous; std is the population standard

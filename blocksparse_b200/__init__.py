@@ -15,6 +15,8 @@ listed in elementwise.__all__ and also reachable as blocksparse_b200.ewops.<name
 (QuantizeSpec, quantize, log_stats, with quantize_state and reset_quantize_states; listed in quantize.__all__), and of its conv module (BlocksparseConv, BlocksparseDeconv; listed in conv.__all__; ConvEdgeBias,
 conv_edge_bias_init, deconv_edge_bias_init, cwise_linear; listed in conv_bias.__all__ and also reachable as
 blocksparse_b200.conv.<name>), and its top-level dw_matmul_large_n (importable from here, not listed in __all__).
+Beyond the reference: fp8 fprop / bprop on the H100's fp8 tensor cores, BlocksparseMatMul.matmul_fp8, with
+quantize_fp8 (importable from here, not listed in __all__) and the raw calls in blocksparse_b200.fp8.
 """
 from .matmul import (BlocksparseMatMul, SparseProj, block_reduced_full_dw, blocksparse_reduced_dw, dw_matmul_large_n,
                      group_param_grads)
@@ -34,6 +36,7 @@ from .elementwise import (add, add_n, add_n8, assign_add, concrete_gate, concret
 from .quantize import QuantizeSpec, log_stats, quantize, quantize_state, reset_quantize_states
 from .conv import BlocksparseConv, BlocksparseDeconv
 from .conv_bias import ConvEdgeBias, conv_edge_bias_init, cwise_linear, deconv_edge_bias_init
+from .fp8 import quantize_fp8
 from .lut import z_order_2d
 from . import _lib
 

@@ -10,6 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbsmm_b200.so")
 
 F32, F16, BF16 = 0, 1, 2
+E4M3, E5M2 = 3, 4        # BSMM_E4M3 / BSMM_E5M2: accepted by the bsmm_fp8_* entries and bsmm_xprop_fp8 only
 FLAG_FORCE_GENERIC, FLAG_FORCE_TC = 1, 2
 MAX_PAIRS = 8
 E_NOKERNEL = -7          # BSMM_E_NOKERNEL: no fused kernel for the configuration
@@ -104,6 +105,9 @@ SIGNATURES = {
     "bsmm_cwise_linear_grad_workspace_bytes": (_c.c_size_t, [_ll, _i, _ll]),
     "bsmm_dw_matmul_large_n": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _vp, _i, _vp]),
     "bsmm_dw_matmul_large_n_workspace_bytes": (_c.c_size_t, [_i, _ll, _i, _i]),
+    "bsmm_fp8_quantize": (_i, [_i, _i, _vp, _ll, _vp, _vp, _vp, _vp]),
+    "bsmm_fp8_weights": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bsmm_xprop_fp8": (_i, [_i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "bsmm_block_norm":(_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),
@@ -191,6 +195,21 @@ def dtype_code(torch_dtype):
         return _DTYPE_CODES[torch_dtype]
     except KeyError:
         raise ValueError("unsupported dtype %s (float32, float16, bfloat16 only)" % (torch_dtype,))
+
+
+_FP8_CODES = None
+
+
+def fp8_code(torch_dtype):
+    """dtype code of an fp8 torch dtype (dtype_code maps the fp32 / fp16 / bf16 codes only)."""
+    global _FP8_CODES
+    if _FP8_CODES is None:
+        import torch
+        _FP8_CODES = {torch.float8_e4m3fn: E4M3, torch.float8_e5m2: E5M2}
+    try:
+        return _FP8_CODES[torch_dtype]
+    except KeyError:
+        raise ValueError("unsupported fp8 dtype %s (float8_e4m3fn, float8_e5m2 only)" % (torch_dtype,))
 
 
 LABEL_U8, LABEL_U16, LABEL_I32, LABEL_I64 = 0, 1, 2, 3     # BSMM_LABEL_*

@@ -17,6 +17,7 @@
 #include "quantize.cuh"
 #include "softmax.cuh"
 #include "tc.cuh"
+#include "tc_fp8.cuh"
 #include "transpose.cuh"
 #include "wutil.cuh"
 
@@ -1841,5 +1842,63 @@ int bsmm_dw_matmul_large_n(int dtype, const void* x, const void* e, float* u, lo
     return fail(BSMM_E_ARG, "%s: null workspace (bsmm_dw_matmul_large_n_workspace_bytes gives its size)", what);
   if (!device_info().ok) return fail(BSMM_E_NODEV, "no CUDA device");
   return dense_dw_run(tc, dtype, x, e, u, N, C, K, (float*)workspace, s);
+}
+// ---- fp8 quantisation and xprop ---------------------------------------------------------------------------------
+static int fp8_src_ok(int dt) { return dt == BSMM_F32 || dt == BSMM_F16 || dt == BSMM_BF16; }
+
+int bsmm_fp8_quantize(int src_dtype, int fp8_dtype, const void* x, long long n, float* amax, float* scale_inv, void* y,
+                      void* stream) {
+  const char* what = "bsmm_fp8_quantize";
+  if (!fp8_src_ok(src_dtype) || !fp8_code(fp8_dtype))
+    return fail(BSMM_E_DTYPE, "%s: needs an fp32 / fp16 / bf16 source and an e4m3 / e5m2 target, got %d -> %d", what, src_dtype, fp8_dtype);
+  if (n < 0) return fail(BSMM_E_ARG, "%s: negative size %lld", what, n);
+  if (!amax || !scale_inv || (n > 0 && (!x || !y))) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  cudaStream_t s = (cudaStream_t)stream;
+  uint8_t* q = (uint8_t*)y;
+  BSMM_DISPATCH_DTYPE(src_dtype, T, {
+    const T* xt = (const T*)x;
+    return fp8_dtype == BSMM_E5M2 ? launch_fp8_quantize<T, BSMM_E5M2>(xt, n, amax, scale_inv, q, s)
+                                  : launch_fp8_quantize<T, BSMM_E4M3>(xt, n, amax, scale_inv, q, s);
+  });
+  return 0;
+}
+
+int bsmm_fp8_weights(int src_dtype, int fp8_dtype, int bsize, int blocks, const void* w, float* amax, float* scale_inv,
+                     void* wq, void* wq_t, void* stream) {
+  const char* what = "bsmm_fp8_weights";
+  if (bsize != 32 && bsize != 64) return fail(BSMM_E_BSIZE, "%s: fp8 weights need block size 32 or 64, got %d", what, bsize);
+  if (!fp8_src_ok(src_dtype) || !fp8_code(fp8_dtype))
+    return fail(BSMM_E_DTYPE, "%s: needs an fp32 / fp16 / bf16 source and an e4m3 / e5m2 target, got %d -> %d", what, src_dtype, fp8_dtype);
+  if (blocks <= 0) return fail(BSMM_E_ARG, "%s: blocks must be positive, got %d", what, blocks);
+  if (!w || !amax || !scale_inv || !wq || !wq_t) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (((uintptr_t)wq | (uintptr_t)wq_t) & 15) return fail(BSMM_E_ALIGN, "%s: wq and wq_t must be 16-byte aligned", what);
+  cudaStream_t s = (cudaStream_t)stream;
+  uint8_t *q = (uint8_t*)wq, *qt = (uint8_t*)wq_t;
+  BSMM_DISPATCH_DTYPE(src_dtype, T, {
+    const T* wt = (const T*)w;
+    return fp8_dtype == BSMM_E5M2 ? launch_fp8_weights<T, BSMM_E5M2>(bsize, blocks, wt, amax, scale_inv, q, qt, s)
+                                  : launch_fp8_weights<T, BSMM_E4M3>(bsize, blocks, wt, amax, scale_inv, q, qt, s);
+  });
+  return 0;
+}
+
+int bsmm_xprop_fp8(int x_dtype, int w_dtype, int y_dtype, int axis, int bsize, int bprop, const int32_t* lut, int n_out,
+                   int n_in, int blocks, const void* x, const void* w, void* y, int N, const float* x_scale_inv,
+                   const float* w_scale_inv, void* stream) {
+  const char* what = "bsmm_xprop_fp8";
+  if (axis != 1) return fail(BSMM_E_BSIZE, "%s: fp8 xprop needs feature axis 1, got %d", what, axis);
+  if (bsize != 32 && bsize != 64) return fail(BSMM_E_BSIZE, "%s: fp8 xprop needs block size 32 or 64, got %d", what, bsize);
+  if (!fp8_code(x_dtype) || !fp8_code(w_dtype) || (y_dtype != BSMM_F16 && y_dtype != BSMM_BF16))
+    return fail(BSMM_E_DTYPE, "%s: needs e4m3 / e5m2 x and w and an fp16 / bf16 y, got x %d, w %d, y %d", what, x_dtype,
+                w_dtype, y_dtype);
+  if (!lut || !x || !w || !y || !x_scale_inv || !w_scale_inv) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  // fprop and bprop run the same kernel: the direction is in the LUT and the weight layout the caller passes
+  if (bprop != 0 && bprop != 1) return fail(BSMM_E_ARG, "%s: bprop must be 0 or 1, got %d", what, bprop);
+  if (n_out <= 0 || n_in <= 0 || blocks < 0 || N < 0) return fail(BSMM_E_ARG, "%s: bad sizes", what);
+  if (n_out >= 65536 || n_in >= 65536) return fail(BSMM_E_LIMIT, "%s: more than 65535 blocks per dimension", what);
+  if (((uintptr_t)x | (uintptr_t)w | (uintptr_t)y) & 15) return fail(BSMM_E_ALIGN, "%s: x, w and y must be 16-byte aligned", what);
+  if (N == 0) return 0;
+  return tc_xprop_fp8(x_dtype, w_dtype, y_dtype, bsize, lut, n_out, n_in, blocks, x, w, y, N, x_scale_inv, w_scale_inv,
+                      (cudaStream_t)stream);
 }
 }  // extern "C"

@@ -36,16 +36,21 @@ inline TmapEncodeFn tmap_encoder() {
   }();
   return fn;
 }
-// 2-D row-major 16-bit tensor [outer][inner]; box = box_outer rows x box_inner elements.
+// Element size of a tensor-map dtype code: 1 byte for the fp8 codes, 2 for fp16 / bf16.
+inline uint64_t tmap_elem_bytes(int dtype) { return dtype == BSMM_E4M3 || dtype == BSMM_E5M2 ? 1 : 2; }
+// 2-D row-major tensor [outer][inner] of 16-bit (fp16 / bf16) or 1-byte (fp8, encoded as UINT8) elements;
+// box = box_outer rows x box_inner elements.
 inline int make_tmap_2d(CUtensorMap* m, int dtype, const void* base, uint64_t inner, uint64_t outer, uint64_t row_pitch_elems,
                         uint32_t box_inner, uint32_t box_outer, CUtensorMapSwizzle swz) {
   TmapEncodeFn enc = tmap_encoder();
   if (!enc) return fail(BSMM_E_NODEV, "cuTensorMapEncodeTiled entry point not available");
+  const uint64_t esize = tmap_elem_bytes(dtype);
   cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {row_pitch_elems * 2};
+  cuuint64_t strides[1] = {row_pitch_elems * esize};
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
-  CUtensorMapDataType dt = dtype == BSMM_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMapDataType dt = esize == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                           : dtype == BSMM_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUresult r = enc(m, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(BSMM_E_ARG, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);

@@ -14,6 +14,7 @@ import torch
 
 from . import _lib
 from .checkers import MatmulCheckers
+from .fp8 import check_config as _fp8_check_config, quantize_fp8, quantize_fp8_weights, xprop_fp8
 from .lut import MatmulLuts, WIDE_REC, XPROP_GROUP, pick_xprop_tile
 
 # 32 x 32 blocks and 16-bit dtypes: the default route picks, per layout, direction and minibatch, between one output block
@@ -363,6 +364,32 @@ class BlocksparseMatMul(MatmulCheckers):
             self._bench_op("fprop", lambda: self.fprop(I, W, gate), I, bench, name or self.name)
         return _BsmmFunction.apply(I, W, gate, self, bool(gate_grad), bool(dw_gated), int(bench), name or self.name)
 
+    def matmul_fp8(self, I, W, name=None):
+        """y = bsmm(I, W) on fp8 tensor cores, with gradients for I and W (DESIGN.md 6e).
+
+        Forward: I and W are quantised to e4m3 with one scale each (fp8.quantize_fp8 / quantize_fp8_weights) and the fp8
+        fprop runs; y comes out in I's dtype. Backward: dy is quantised to e5m2 and the fp8 bprop runs against the saved
+        e4m3 weights, so dx comes out in I's dtype; dw is the 16-bit updat of the saved I and dy, exactly as in
+        bsmm(I, W)'s backward (group_param_grads included), so it is bit-identical to it.
+        I (..., C) and W (blocks, bs, bs) are float16 or bfloat16 CUDA tensors of one dtype; feature_axis 1 and block
+        sizes 32 / 64 only. There is no gate argument. `name` is accepted for symmetry with __call__."""
+        _fp8_check_config(self)
+        for t in (I, W):
+            if not torch.is_tensor(t) or t.dtype not in (torch.float16, torch.bfloat16):
+                raise ValueError("matmul_fp8 takes float16 or bfloat16 tensors, got %s" % (getattr(t, "dtype", type(t)),))
+        if W.dtype != I.dtype:
+            raise ValueError("matmul_fp8: I is %s, W is %s" % (I.dtype, W.dtype))
+        if not I.is_cuda or not W.is_cuda:
+            raise _lib.BsmmError("BlocksparseMatMul needs CUDA tensors (no CPU path)")
+        if tuple(W.shape) != self.w_shape:
+            raise ValueError("W must have shape %s, got %s" % (self.w_shape, tuple(W.shape)))
+        if I.dim() < 1 or I.shape[-1] != self.C:
+            raise ValueError("expected feature dim %d on the last axis, got shape %s" % (self.C, tuple(I.shape)))
+        if I.device != W.device:
+            raise ValueError("matmul_fp8: I lives on %s, W on %s" % (I.device, W.device))
+        self.count += 1
+        return _Fp8MatmulFunction.apply(I, W, self)
+
     def _bench_op(self, what, fn, I, repeat, name):
         """The reference's `bench` attribute (op.cc:99-106,181-185, gpu_types.cc:43-87): repeat the launch `repeat` times
         between two CUDA events and print one line; applies to fprop and, through the backward pass, to bprop and updat."""
@@ -410,12 +437,41 @@ class _BsmmFunction(torch.autograd.Function):
             dg = bsmm.gate_grad(raw, w).to(gate.dtype)
             dw = raw * gate.to(raw.dtype).view(-1, 1, 1)
         elif ctx.needs_input_grad[1]:
-            pending = _pending_group(bsmm, w)
-            if pending is not None:
-                dw = pending.add(x, dy, gate, ctx.dw_gated)
-            else:
-                dw = bsmm.updat([x], [dy], gate=gate, dw_gated=ctx.dw_gated)
+            dw = _weight_grad(bsmm, x, w, dy, gate, ctx.dw_gated)
         return dx, dw, dg, None, None, None, None, None
+
+
+def _weight_grad(bsmm, x, w, dy, gate=None, dw_gated=False):
+    """dw of one use of w: handed to the open group_param_grads block of (bsmm, w) if there is one, else one updat."""
+    pending = _pending_group(bsmm, w)
+    if pending is not None:
+        return pending.add(x, dy, gate, dw_gated)
+    return bsmm.updat([x], [dy], gate=gate, dw_gated=dw_gated)
+
+
+class _Fp8MatmulFunction(torch.autograd.Function):
+    """BlocksparseMatMul.matmul_fp8: e4m3 fprop, e5m2 x e4m3 bprop, 16-bit updat."""
+
+    @staticmethod
+    def forward(ctx, x, w, bsmm):
+        xq, xs = quantize_fp8(x, torch.float8_e4m3fn)
+        wq, wq_t, ws = quantize_fp8_weights(bsmm, w, torch.float8_e4m3fn)
+        ctx.bsmm = bsmm
+        ctx.save_for_backward(x, w, wq, ws)
+        return xprop_fp8(bsmm, xq, wq_t, xs, ws, bprop=False, out_dtype=x.dtype)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w, wq, ws = ctx.saved_tensors
+        bsmm = ctx.bsmm
+        dy = dy.contiguous()
+        dx = dw = None
+        if ctx.needs_input_grad[0]:
+            dq, ds = quantize_fp8(dy, torch.float8_e5m2)
+            dx = xprop_fp8(bsmm, dq, wq, ds, ws, bprop=True, out_dtype=x.dtype)
+        if ctx.needs_input_grad[1]:
+            dw = _weight_grad(bsmm, x, w, dy)
+        return dx, dw, None
 
 
 # ---------------------------------------------------------------------------------------

@@ -76,6 +76,8 @@
  *                            CWiseLinearGradOp (src/cwise_linear_op.cc:125-191)
  *   bsmm_dw_matmul_large_n <- Gemm_TN (src/matmul_op_gpu.cu:309-364), launched by DwMatmulLargeNOp
  *                            (src/matmul_op.cc:47-87)
+ *   bsmm_fp8_quantize / bsmm_fp8_weights / bsmm_xprop_fp8 <- no reference counterpart: fp8 fprop / bprop on the
+ *                            H100's fp8 tensor cores, which the reference's Volta target does not have
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer except `err` strings is DEVICE memory
@@ -989,6 +991,66 @@ int bsmm_dw_matmul_large_n(int dtype, const void* x, const void* e, float* u, lo
 /* Bytes of workspace bsmm_dw_matmul_large_n needs for (dtype, N, C, K) on whichever route it may take (0 when S == 1
  * on both, and for bad arguments). At most 264 * 128 * 256 * 4 = 34,603,008 bytes, whatever N is. */
 size_t bsmm_dw_matmul_large_n_workspace_bytes(int dtype, long long N, int C, int K);
+
+/* ---- fp8 block-sparse matmul (no reference counterpart: Volta has no fp8 tensor cores) ----------------------------- */
+
+/*
+ * The fp8 dtype codes BSMM_E4M3 and BSMM_E5M2 are accepted by the three entries below only; every other entry rejects
+ * them as it rejects any unknown dtype code. Storage is one byte per element, the OCP FP8 encodings torch calls
+ * float8_e4m3fn (largest finite 448, no infinities) and float8_e5m2 (largest finite 57344).
+ *
+ * Per-tensor scaling with the current amax. With FP8_MAX = 448 (e4m3) or 57344 (e5m2), every value in fp32:
+ *   amax      = max |x| over the whole tensor: NaN if any element is NaN, else +inf if any is infinite;
+ *   s         = 1 if amax == 0, else FP8_MAX / amax                     (one IEEE fp32 division, round to nearest);
+ *   scale_inv = 1 if amax == 0, NaN if amax is not finite, else amax / FP8_MAX     (its own IEEE fp32 division,
+ *               not 1 / s);
+ *   y         = cvt.rn.satfinite(x * s): the fp32 product x * s, rounded to nearest even into the format, with
+ *               magnitudes past FP8_MAX (infinities included) saturated to +-FP8_MAX, subnormals kept and the sign of
+ *               zero kept; a NaN product becomes the canonical NaN 0x7f (sign dropped).
+ * So x ~= y * scale_inv. A non-finite amax makes scale_inv NaN, and with it every product an fp8 matmul forms from y.
+ * amax is an order-independent maximum, so all outputs are deterministic. Nothing synchronises the host, and amax and
+ * scale_inv stay on the device (CUDA-graph capturable).
+ */
+enum { BSMM_E4M3 = 3, BSMM_E5M2 = 4 };
+
+/*
+ * y (n bytes, fp8_dtype) = x (n elements, src_dtype BSMM_F32 / F16 / BF16) quantised as above; amax and scale_inv are
+ * one fp32 each. The call clears amax (cudaMemsetAsync), folds max |x| into it (kernel fp8_amax, atomicMax on the
+ * bits of |x|, exact and order-independent), then casts (kernel fp8_quantize), which also writes scale_inv.
+ * Errors before any launch: a bad src or fp8 dtype (BSMM_E_DTYPE); n < 0, a null amax or scale_inv, or a null x or y
+ * with n > 0 (BSMM_E_ARG). n = 0 stores amax = 0 and scale_inv = 1 (fp8_quantize with one CTA, no fp8_amax). 64-bit
+ * offsets.
+ */
+int bsmm_fp8_quantize(int src_dtype, int fp8_dtype, const void* x, long long n, float* amax, float* scale_inv, void* y,
+                      void* stream);
+
+/*
+ * The same scaling over a whole block-sparse weight tensor w [blocks][bsize][bsize] (rows = input features c, columns
+ * = output features k), with one amax for the tensor: wq [blocks][bsize][bsize] holds the blocks as stored (read by the
+ * bprop of bsmm_xprop_fp8), wq_t the same bytes with each block transposed, wq_t[b][k][c] = wq[b][c][k] (read by its
+ * fprop). Kernels fp8_amax, then fp8_weights (one pass writing both).
+ * Errors before any launch: bsize other than 32 or 64 (BSMM_E_BSIZE); a bad src or fp8 dtype (BSMM_E_DTYPE); blocks
+ * <= 0 or a null pointer (BSMM_E_ARG).
+ */
+int bsmm_fp8_weights(int src_dtype, int fp8_dtype, int bsize, int blocks, const void* w, float* amax, float* scale_inv,
+                     void* wq, void* wq_t, void* stream);
+
+/*
+ * Block-sparse fprop (bprop = 0) or bprop (bprop = 1) with fp8 operands, feature axis 1: y [N][n_out * bsize] from
+ * x [N][n_in * bsize] (x_dtype) and the weight blocks w (w_dtype): fprop takes wq_t and the fprop row LUT, bprop takes
+ * wq and the bprop row LUT (the LUT format above). Block size 32 or 64; x and w e4m3 or e5m2 each; y fp16 or bf16.
+ * Each LUT entry's product (bsize features) is summed by one wgmma chain (m64n{32,64}k32, fp8 inputs) into a zeroed
+ * fragment, which is then added in fp32 on CUDA cores to the output's total, in LUT order. The epilogue writes
+ * y = total * (x_scale_inv[0] * w_scale_inv[0]), fp32, rounded once to y's dtype; output blocks with an empty LUT row
+ * get zeros. No atomics: results are bitwise reproducible. Kernel: wgmma_xprop_fp8_bs32 / _bs64.
+ * Errors before any launch: axis other than 1 or bsize other than 32 / 64 (BSMM_E_BSIZE); any other dtype combination
+ * (BSMM_E_DTYPE); a null pointer, n_out / n_in <= 0, blocks < 0 or N < 0 (BSMM_E_ARG); n_out or n_in of 65536 or more
+ * (BSMM_E_LIMIT); x, w or y not 16-byte aligned (BSMM_E_ALIGN); no sm_90 device (BSMM_E_NODEV). There is no other
+ * path for these dtypes. N = 0 launches nothing. 64-bit offsets.
+ */
+int bsmm_xprop_fp8(int x_dtype, int w_dtype, int y_dtype, int axis, int bsize, int bprop, const int32_t* lut, int n_out,
+                   int n_in, int blocks, const void* x, const void* w, void* y, int N, const float* x_scale_inv,
+                   const float* w_scale_inv, void* stream);
 
 /* ---- measurement helper (the reference's `bench` op attribute, op.cc:99-106) ---------
  * Records two events around whatever the caller enqueues between begin and end.      */

@@ -40,6 +40,12 @@ SIGNATURES = {
     "bst_attention_train": (_i, [_i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp]),
     "bst_attention_grad": (_i, [_i, _i, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                 _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp]),
+    "bst_attention_dropout": (_i, [_i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i,
+                                   _c.c_double, _vp, _vp]),
+    "bst_attention_train_dropout": (_i, [_i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i,
+                                         _i, _i, _c.c_double, _vp, _vp]),
+    "bst_attention_grad_dropout": (_i, [_i, _i, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                        _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _c.c_double, _vp, _vp]),
     "bst_autoregressive_mask": (_i, [_i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     "bst_dense_softmax": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),
     "bst_dense_softmax_grad": (_i, [_i, _vp, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),

@@ -412,6 +412,77 @@ int bst_attention_grad(int dtype, int bsize, const int32_t* nn_lut, const int32_
   return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
 }
 
+// The dropout entries: keep_prob 1 runs the counterpart's kernels, keep_prob in (0, 1) their DROP instantiations.
+static int check_attention_dropout(const char* op, double keep_prob, const int64_t* seed_call, BstAttnDrop& drop) {
+  if (!(keep_prob > 0.0 && keep_prob <= 1.0)) return fail(BSMM_E_ARG, "%s: keep_prob must be in (0, 1]", op);
+  if (keep_prob < 1.0 && !seed_call) return fail(BSMM_E_ARG, "%s: null seed_call", op);
+  drop.keep_prob = keep_prob;
+  drop.seed_call = reinterpret_cast<const long long*>(seed_call);
+  return 0;
+}
+
+int bst_attention_dropout(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                          const void* mask, int mask_heads, int autoregress_at_key,
+                          const void* q, const void* k, const void* v, void* o, float scale,
+                          int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                          double keep_prob, const int64_t* seed_call, void* stream) {
+  BstAttnDrop drop;
+  if (int e = check_attention_dropout("bst_attention_dropout", keep_prob, seed_call, drop)) return e;
+  if (int e = check_bst(bsize, lut_heads, heads, head_state, batch, blocks)) return e;
+  if (!nn_lut || !q || !k || !v || !o) return fail(BSMM_E_ARG, "bst_attention_dropout: null pointer");
+  if (ctx_blks_q <= 0 || ctx_blks_k <= 0) return fail(BSMM_E_ARG, "bst_attention_dropout: bad context sizes");
+  if (autoregress_at_key >= 0 && !mask) return fail(BSMM_E_ARG, "bst_attention_dropout: autoregress_at_key needs a mask");
+  if (mask && mask_heads != 1 && mask_heads != heads) return fail(BSMM_E_ARG, "bst_attention_dropout: mask_heads must be 1 or heads");
+  const int rc = tc_bst_attention(dtype, bsize, nn_lut, lut_heads, blocks, mask, mask_heads, autoregress_at_key, q, k, v, o,
+                                  scale, batch, heads, head_state, ctx_blks_q, ctx_blks_k, (cudaStream_t)stream, nullptr,
+                                  nullptr, keep_prob < 1.0 ? &drop : nullptr);
+  return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
+}
+
+int bst_attention_train_dropout(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                                const void* mask, int mask_heads, int autoregress_at_key,
+                                const void* q, const void* k, const void* v, void* o, float* row_max, float* row_sum,
+                                float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                                double keep_prob, const int64_t* seed_call, void* stream) {
+  BstAttnDrop drop;
+  if (int e = check_attention_dropout("bst_attention_train_dropout", keep_prob, seed_call, drop)) return e;
+  if (int e = check_bst(bsize, lut_heads, heads, head_state, batch, blocks)) return e;
+  if (!nn_lut || !q || !k || !v || !o || !row_max || !row_sum)
+    return fail(BSMM_E_ARG, "bst_attention_train_dropout: null pointer");
+  if (ctx_blks_q <= 0 || ctx_blks_k <= 0) return fail(BSMM_E_ARG, "bst_attention_train_dropout: bad context sizes");
+  if (autoregress_at_key >= 0 && !mask)
+    return fail(BSMM_E_ARG, "bst_attention_train_dropout: autoregress_at_key needs a mask");
+  if (mask && mask_heads != 1 && mask_heads != heads)
+    return fail(BSMM_E_ARG, "bst_attention_train_dropout: mask_heads must be 1 or heads");
+  const int rc = tc_bst_attention(dtype, bsize, nn_lut, lut_heads, blocks, mask, mask_heads, autoregress_at_key, q, k, v, o,
+                                  scale, batch, heads, head_state, ctx_blks_q, ctx_blks_k, (cudaStream_t)stream, row_max,
+                                  row_sum, keep_prob < 1.0 ? &drop : nullptr);
+  return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
+}
+
+int bst_attention_grad_dropout(int dtype, int bsize, const int32_t* nn_lut, const int32_t* tn_lut, const int32_t* tn_order,
+                               int lut_heads, int blocks, const void* mask, int mask_heads, int autoregress_at_key,
+                               const void* q, const void* k, const void* v, const void* o, const void* dy,
+                               const float* row_max, const float* row_sum, float* delta, void* dq, void* dk, void* dv,
+                               float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                               double keep_prob, const int64_t* seed_call, void* stream) {
+  BstAttnDrop drop;
+  if (int e = check_attention_dropout("bst_attention_grad_dropout", keep_prob, seed_call, drop)) return e;
+  if (int e = check_bst(bsize, lut_heads, heads, head_state, batch, blocks)) return e;
+  if (!nn_lut || !tn_lut || !tn_order || !q || !k || !v || !o || !dy || !row_max || !row_sum || !delta || !dq || !dk || !dv)
+    return fail(BSMM_E_ARG, "bst_attention_grad_dropout: null pointer");
+  if (ctx_blks_q <= 0 || ctx_blks_k <= 0) return fail(BSMM_E_ARG, "bst_attention_grad_dropout: bad context sizes");
+  if (autoregress_at_key >= 0 && !mask)
+    return fail(BSMM_E_ARG, "bst_attention_grad_dropout: autoregress_at_key needs a mask");
+  if (mask && mask_heads != 1 && mask_heads != heads)
+    return fail(BSMM_E_ARG, "bst_attention_grad_dropout: mask_heads must be 1 or heads");
+  const int rc = tc_bst_attention_grad(dtype, bsize, nn_lut, tn_lut, tn_order, lut_heads, blocks, mask, mask_heads,
+                                       autoregress_at_key, q, k, v, o, dy, row_max, row_sum, delta, dq, dk, dv, scale, batch,
+                                       heads, head_state, ctx_blks_q, ctx_blks_k, (cudaStream_t)stream,
+                                       keep_prob < 1.0 ? &drop : nullptr);
+  return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
+}
+
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,
                             const void* mask_in, void* mask_out, int autoregress_at_key, void* stream) {
   if (!nt_lut || !mask_in || !mask_out || lut_heads <= 0 || blocks <= 0)

@@ -19,6 +19,7 @@
 // and every replay of a captured graph draws a new one.
 #pragma once
 #include "dense_softmax.cuh"
+#include "philox.cuh"
 
 namespace bsmm {
 
@@ -213,19 +214,7 @@ int launch_bias_act(BrArgs& a, int axis, bool grad, bool vec, void* db, cudaStre
   return check_launch(name);
 }
 
-// ---- dropout ---------------------------------------------------------------------------------------------------------
-// Philox4x32-10 (Salmon et al., SC'11; the constants of Random123's philox4x32)
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-  for (int i = 0; i < 10; ++i) {
-    if (i) { k.x += 0x9E3779B9u; k.y += 0xBB67AE85u; }
-    const unsigned lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
-    const unsigned lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-  }
-  return c;
-}
-
+// ---- dropout (philox4x32_10: philox.cuh) -----------------------------------------------------------------------------
 // one thread per mask word: 8 Philox blocks of 4 elements; bits at or past M stay 0
 __global__ void __launch_bounds__(EW_THREADS) dropout_mask_kernel(uint32_t* mask, long long M, unsigned long long thr,
                                                                   const long long* state) {

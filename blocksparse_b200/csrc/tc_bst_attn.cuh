@@ -16,8 +16,18 @@
 // and stores 16-bit rows; an empty LUT row is written as zeros.  Accumulation follows LUT order: results are
 // deterministic.  With STATS the epilogue also stores every row's final running max m and full sum l, which the fused
 // backward (tc_bst_attn_bwd.cuh) needs to recompute P = exp(s - m) / l; o is the same either way.
+//
+// With DROP, attention dropout on the normalised probabilities: o_i = sum_j Z_ij exp(s_ij - m_i) v_j / (keep_prob l_i),
+// l the sum over every visible key (Z does not enter it; nor m and l as stored), Z_ij the keep bit of element
+// e = (((b heads + h) blocks + block id) 64 + i) 64 + j of the (batch, heads, blocks, 64, 64) probabilities, drawn as
+// bsmm_dropout_mask draws it from the device (seed, call) (philox.cuh).  Z is applied to the unnormalised P before it
+// enters P V, and 1 / keep_prob is folded into the epilogue's 1 / l.  A thread holds 2 rows x 16 keys of an entry; one
+// Philox block covers 4 consecutive keys of a row, which two neighbouring lanes share, so each lane draws the blocks of
+// one of its rows and the pair trade the halves they need in one shuffle: 8 Philox blocks per thread and entry, drawn
+// while S = Q K^T runs on the tensor cores.
 #pragma once
 #include <float.h>
+#include "philox.cuh"
 #include "softmax.cuh"
 #include "tc_bst.cuh"
 
@@ -37,10 +47,29 @@ struct BstAttnParams {
   void* o;
   float* row_max;                 // STATS: [batch][heads][ctx_rows_q] final running max m and full sum l of each row
   float* row_sum;
+  const long long* seed_call;     // DROP: device [seed, call], read only
+  unsigned long long keep_thr;    // DROP: floor(keep_prob 2^32)
+  float keep_prob, rkeep;         // DROP: keep_prob and fp32(1 / keep_prob)
+  int blocks;                     // blocks of the layout (the element index of the dropout mask)
 };
+
+// Keep bits of this thread's two rows r0 + 8hh (hh = 0, 1) and 16 keys of one entry: bit 4j + x of kw[hh] is key
+// 8j + 2(lane%4) + x (accumulator layout, ptx.cuh).  rows0 = (b heads + h) blocks + block id, the entry's first row of
+// the mask in 64-row units.
+__device__ __forceinline__ void attn_keep_bits(uint32_t (&kw)[2], unsigned long long rows0, int r0, int lane,
+                                               unsigned long long call, uint2 key, unsigned long long thr) {
+  const int pp = lane & 1;                              // this lane draws row r0 + 8pp, its partner lane ^ 1 the other
+  const unsigned long long g0 = (rows0 * 64 + r0 + 8 * pp) * 16 + ((lane % 4) >> 1);
+  uint32_t mine = 0;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) mine |= philox_keep4(g0 + 2 * j, call, key, thr) << (4 * j);
+  const uint32_t other = __shfl_xor_sync(0xffffffffu, mine, 1);
+  kw[0] = (pp == 0 ? mine : other) >> (2 * pp);         // this lane's keys are words 2pp, 2pp + 1 of each block
+  kw[1] = (pp == 1 ? mine : other) >> (2 * pp);
+}
 struct BstAttnTmaps { CUtensorMap q, k, v; };
 
-template <bool BF16, int CH, bool STATS = false>      // CH = head_state / 64
+template <bool BF16, int CH, bool STATS = false, bool DROP = false>      // CH = head_state / 64
 __global__ void __launch_bounds__(BST_THREADS)
 wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps maps) {
   constexpr int ST = BST_ATTN_STAGES;
@@ -92,6 +121,13 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[c][i] = 0.f;
   float m[2] = {-FLT_MAX, -FLT_MAX}, l[2] = {0.f, 0.f};   // l: this thread's part of the row sum
+  uint2 key = make_uint2(0u, 0u);
+  unsigned long long call = 0;
+  if constexpr (DROP) {
+    const unsigned long long seed = (unsigned long long)p.seed_call[0];
+    call = (unsigned long long)p.seed_call[1];
+    key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  }
   if (count > 0 && !ptx::mbar_wait(&qbar, 0)) g_tc_error = 41;
 
   for (int e = 0; e < count; ++e) {
@@ -108,6 +144,9 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
         ptx::wgmma_n64<BF16, 0, 0>(s, ptx::make_desc(base + c * BST_TILE + ks * 32, 16, 1024, ptx::SWZ_128B),
                                    ptx::make_desc(st + c * BST_TILE + ks * 32, 16, 1024, ptx::SWZ_128B));
     ptx::wg_commit();
+    uint32_t kw[2];                                     // the entry's keep bits, drawn while the MMAs run
+    if constexpr (DROP)
+      attn_keep_bits(kw, ((unsigned long long)b * p.heads + h) * p.blocks + ent[e].x, r0, lane, call, key, p.keep_thr);
     ptx::wg_wait<0>();
     ptx::wg_fence_regs(s);
 
@@ -150,6 +189,7 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
           float& v = s[4 * j + 2 * hh + x];
           v = exp2f((v - mx) * LOG2E);
           acc += v;
+          if constexpr (DROP) if (!((kw[hh] >> (4 * j + x)) & 1u)) v = 0.f;   // after the row sum: l is not affected
         }
       l[hh] = l[hh] * alpha[hh] + acc;
     }
@@ -186,7 +226,9 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
     float sum = l[hh];
     sum += __shfl_xor_sync(0xffffffffu, sum, 1);
     sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-    const float inv = count > 0 ? 1.f / sum : 0.f;
+    float inv;
+    if constexpr (DROP) inv = count > 0 ? p.rkeep / sum : 0.f;
+    else inv = count > 0 ? 1.f / sum : 0.f;
     const int row = r0 + 8 * hh;
     if (STATS && lane % 4 == 0) {                       // m is already the quad's common value
       const long long r = ((long long)b * p.heads + h) * p.ctx_rows_q + qb * 64 + row;
@@ -205,10 +247,25 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
 }
 
 // ------------------------------------------------------------------------------------------------
+// Dropout of the fused kernels: keep_prob in (0, 1), seed_call the device [seed, call] (never written).  A null
+// BstAttnDrop runs the kernels without dropout.
+struct BstAttnDrop {
+  double keep_prob;
+  const long long* seed_call;
+};
+
+template <typename P> inline void set_drop(P& p, const BstAttnDrop* drop) {
+  p.seed_call = drop ? drop->seed_call : nullptr;
+  p.keep_thr = drop ? (unsigned long long)floor(drop->keep_prob * 4294967296.0) : 0;   // as bsmm_dropout_mask
+  p.keep_prob = drop ? (float)drop->keep_prob : 1.f;
+  p.rkeep = drop ? (float)(1.0 / drop->keep_prob) : 1.f;                              // as bsmm_dropout_apply
+}
+
 inline int tc_bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks, const void* mask,
                             int mask_heads, int autoregress_at_key, const void* q, const void* k, const void* v, void* o,
                             float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
-                            cudaStream_t s, float* row_max = nullptr, float* row_sum = nullptr) {
+                            cudaStream_t s, float* row_max = nullptr, float* row_sum = nullptr,
+                            const BstAttnDrop* drop = nullptr) {
   if ((uintptr_t)o & 15) { fail(0, "pointers must be 16-byte aligned for TMA"); return TC_NOT_APPLICABLE; }
   if (!bst_tc_applicable(dtype, bsize, head_state, q, k, v)) return TC_NOT_APPLICABLE;
   const uint64_t S = (uint64_t)heads * head_state;
@@ -224,22 +281,28 @@ inline int tc_bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut
   p.n_q = ctx_blks_q; p.heads = heads; p.head_state = head_state;
   p.ctx_rows_q = ctx_blks_q * 64; p.ctx_rows_k = ctx_blks_k * 64; p.o = o;
   p.row_max = row_max; p.row_sum = row_sum;
+  set_drop(p, drop);
+  p.blocks = blocks;
   const bool stats = row_max != nullptr;
   const int ch = head_state / 64;
   const size_t smem = (size_t)(1 + 2 * BST_ATTN_STAGES) * ch * BST_TILE + SMEM_ALIGN_SLACK;
   const unsigned grid = (unsigned)((long long)batch * heads * ctx_blks_q);
-#define BSMM_LAUNCH_ATTN(BFV, CHV, STV)                                                  \
-  { auto kern = wgmma_bst_attention<BFV, CHV, STV>;                                      \
+#define BSMM_LAUNCH_ATTN(BFV, CHV, STV, DRV)                                             \
+  { auto kern = wgmma_bst_attention<BFV, CHV, STV, DRV>;                                 \
     static thread_local uint64_t cfg = 0;                                                \
     if (int e = ensure_dyn_smem(kern, smem, cfg)) return e;                              \
     kern<<<grid, BST_THREADS, smem, s>>>(p, maps); }
-#define BSMM_LAUNCH_ATTN_CH(BFV, STV) \
-  { if (ch == 2) BSMM_LAUNCH_ATTN(BFV, 2, STV) else BSMM_LAUNCH_ATTN(BFV, 1, STV) }
+#define BSMM_LAUNCH_ATTN_CH(BFV, STV, DRV) \
+  { if (ch == 2) BSMM_LAUNCH_ATTN(BFV, 2, STV, DRV) else BSMM_LAUNCH_ATTN(BFV, 1, STV, DRV) }
+#define BSMM_LAUNCH_ATTN_BF(STV, DRV) \
+  { if (bf) BSMM_LAUNCH_ATTN_CH(true, STV, DRV) else BSMM_LAUNCH_ATTN_CH(false, STV, DRV) }
   const bool bf = dtype == BSMM_BF16;
-  if (stats) { if (bf) BSMM_LAUNCH_ATTN_CH(true, true) else BSMM_LAUNCH_ATTN_CH(false, true) }
-  else { if (bf) BSMM_LAUNCH_ATTN_CH(true, false) else BSMM_LAUNCH_ATTN_CH(false, false) }
+  if (drop) { if (stats) BSMM_LAUNCH_ATTN_BF(true, true) else BSMM_LAUNCH_ATTN_BF(false, true) }
+  else { if (stats) BSMM_LAUNCH_ATTN_BF(true, false) else BSMM_LAUNCH_ATTN_BF(false, false) }
+#undef BSMM_LAUNCH_ATTN_BF
 #undef BSMM_LAUNCH_ATTN_CH
 #undef BSMM_LAUNCH_ATTN
+  if (drop) return check_launch(stats ? "wgmma_bst_attention_train_dropout" : "wgmma_bst_attention_dropout");
   return check_launch(stats ? "wgmma_bst_attention_train" : "wgmma_bst_attention");
 }
 

@@ -26,6 +26,14 @@
 // An empty LUT row writes zeros (dQ of a query block no key is listed for, dK / dV of a key block no query sees).  No
 // atomics; accumulation follows LUT order: results are deterministic.  A row whose keys are all masked has m = -FLT_MAX
 // and uniform P = 1 / l; as in the chain, its dS = scale * P o (dP - D) reaches dQ and dK.
+//
+// With DROP, the backward of attention dropout (tc_bst_attn.cuh) with the forward's keep bits Z, regenerated from the
+// same device (seed, call): dV = (P o Z)^T dO / keep_prob, dP = (dO V^T) o Z / keep_prob, D as above (dO . O),
+// dS = scale P o (dP - D), computed as (scale / keep_prob) P o (Z o dO V^T - keep_prob D) so that 1 / keep_prob costs
+// no multiply per element (the staged D is multiplied by keep_prob once per row, dV by 1 / keep_prob in the epilogue).
+// The dq kernel draws the bits of its rows as the forward does; the dkdv kernel, whose threads hold key rows, draws
+// each entry's 64 x 64 bits cooperatively into 64 shared words laid out as its mask words (bit key of word query).
+// Both draw while the entry's S and dP MMAs run.
 #pragma once
 #include <float.h>
 #include "tc_bst_attn.cuh"
@@ -51,6 +59,10 @@ struct BstAttnBwdParams {
   const float* row_sum;
   float* delta;                   // [batch][heads][ctx_rows_q]: written by the dq kernel, read by the dkdv kernel
   void *dq, *dk, *dv;
+  const long long* seed_call;     // DROP: as BstAttnParams
+  unsigned long long keep_thr;
+  float keep_prob, rkeep;
+  int blocks;
 };
 struct BstAttnBwdTmaps { CUtensorMap q, k, v, dy; };
 
@@ -81,7 +93,7 @@ template <bool BF16> __device__ __forceinline__ void store_rows(uint16_t* out, l
 }
 
 // ------------------------------------------------------------------------------------------------
-template <bool BF16, int CH>      // CH = head_state / 64
+template <bool BF16, int CH, bool DROP = false>      // CH = head_state / 64
 __global__ void __launch_bounds__(BST_THREADS)
 wgmma_bst_attention_bwd_dq(const BstAttnBwdParams p, const __grid_constant__ BstAttnBwdTmaps maps) {
   constexpr int ST = BST_BWD_STAGES;
@@ -161,6 +173,14 @@ wgmma_bst_attention_bwd_dq(const BstAttnBwdParams p, const __grid_constant__ Bst
     m[hh] = p.row_max[stat0 + r0 + 8 * hh];
     il[hh] = count > 0 ? 1.f / p.row_sum[stat0 + r0 + 8 * hh] : 0.f;
     dd[hh] = s_delta[r0 + 8 * hh];
+    if constexpr (DROP) dd[hh] *= p.keep_prob;
+  }
+  uint2 key = make_uint2(0u, 0u);
+  unsigned long long call = 0;
+  if constexpr (DROP) {
+    const unsigned long long seed = (unsigned long long)p.seed_call[0];
+    call = (unsigned long long)p.seed_call[1];
+    key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
   }
   float dq[CH][32];
 #pragma unroll
@@ -186,6 +206,9 @@ wgmma_bst_attention_bwd_dq(const BstAttnBwdParams p, const __grid_constant__ Bst
                                    ptx::make_desc(st + T_BYTES + c * BST_TILE + ks * 32, 16, 1024, ptx::SWZ_128B));
       }
     ptx::wg_commit();
+    uint32_t kw[2];                                     // the entry's keep bits, drawn while the MMAs run
+    if constexpr (DROP)
+      attn_keep_bits(kw, ((unsigned long long)b * p.heads + h) * p.blocks + ent[e].x, r0, lane, call, key, p.keep_thr);
     ptx::wg_wait<0>();
     ptx::wg_fence_regs(s);
     ptx::wg_fence_regs(dp);
@@ -214,7 +237,12 @@ wgmma_bst_attention_bwd_dq(const BstAttnBwdParams p, const __grid_constant__ Bst
     for (int i = 0; i < 32; ++i) {
       const int hh = (i >> 1) & 1;
       const float pr = exp2f((s[i] - m[hh]) * LOG2E) * il[hh];   // subtract first: -FLT_MAX * LOG2E overflows
-      s[i] = p.scale * (pr * (dp[i] - dd[hh]));
+      if constexpr (DROP) {                             // dd = keep_prob D
+        const float dpz = (kw[hh] >> (4 * (i >> 2) + (i & 1))) & 1u ? dp[i] : 0.f;
+        s[i] = (p.scale * p.rkeep) * (pr * (dpz - dd[hh]));
+      } else {
+        s[i] = p.scale * (pr * (dp[i] - dd[hh]));
+      }
     }
     uint32_t a[4][4];
 #pragma unroll
@@ -242,7 +270,7 @@ wgmma_bst_attention_bwd_dq(const BstAttnBwdParams p, const __grid_constant__ Bst
 }
 
 // ------------------------------------------------------------------------------------------------
-template <bool BF16, int CH>      // CH = head_state / 64 = warpgroups; warpgroup g owns state columns [64g, 64g + 64)
+template <bool BF16, int CH, bool DROP = false>   // CH = head_state / 64 = warpgroups; warpgroup g owns state columns [64g, 64g + 64)
 __global__ void __launch_bounds__(BST_THREADS * CH)
 wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ BstAttnBwdTmaps maps) {
   constexpr int ST = BST_BWD_STAGES;
@@ -253,6 +281,7 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
   __shared__ uint64_t kvbar, full[ST];
   __shared__ uint64_t s_mask[64];
   __shared__ float s_m[64], s_il[64], s_d[64];
+  __shared__ uint64_t s_keep[DROP ? 64 : 1];           // DROP: keep bit of (query j, key i) = bit i of word j
   const uint32_t base = aligned_smem_base(smem_raw);    // K, V, then the ring
   const uint32_t vb = base + T_BYTES, ring = base + 2 * T_BYTES;
   const int tid = threadIdx.x, wg = tid / BST_THREADS, warp = (tid % BST_THREADS) / 32, lane = tid % 32;
@@ -300,6 +329,13 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
   float dk[32], dv[32];
 #pragma unroll
   for (int n = 0; n < 32; ++n) { dk[n] = 0.f; dv[n] = 0.f; }
+  uint2 key = make_uint2(0u, 0u);
+  unsigned long long call = 0;
+  if constexpr (DROP) {
+    const unsigned long long seed = (unsigned long long)p.seed_call[0];
+    call = (unsigned long long)p.seed_call[1];
+    key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  }
   if (count > 0 && !ptx::mbar_wait(&kvbar, 0)) g_tc_error = 53;
 
   for (int e = 0; e < count; ++e) {
@@ -316,6 +352,7 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
       s_m[tid] = p.row_max[r];
       s_il[tid] = 1.f / p.row_sum[r];
       s_d[tid] = p.delta[r];
+      if constexpr (DROP) s_d[tid] *= p.keep_prob;
     }
     if (!ptx::mbar_wait(&full[e % ST], (uint32_t)(e / ST) & 1)) g_tc_error = 54;
     float s[32], dp[32];
@@ -332,6 +369,19 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
                                    ptx::make_desc(st + T_BYTES + c * BST_TILE + ks * 32, 16, 1024, ptx::SWZ_128B));
       }
     ptx::wg_commit();
+    if constexpr (DROP) {   // the entry's keep bits while the MMAs run: TPR neighbouring threads per query row
+      constexpr int TPR = 2 * CH, GPT = 16 / TPR;       // GPT Philox blocks (4 keys each) per thread
+      const int qr = tid / TPR, part = tid % TPR;
+      const unsigned long long g0 =
+          ((((unsigned long long)b * p.heads + h) * p.blocks + bq.x) * 64 + qr) * 16 + part * GPT;
+      unsigned long long bits = 0;
+#pragma unroll
+      for (int u = 0; u < GPT; ++u)
+        bits |= (unsigned long long)philox_keep4(g0 + u, call, key, p.keep_thr) << (4 * (part * GPT + u));
+#pragma unroll
+      for (int o = 1; o < TPR; o <<= 1) bits |= __shfl_xor_sync(0xffffffffu, bits, o);
+      if (part == 0) s_keep[qr] = bits;
+    }
     __syncthreads();                                    // the entry's mask words and statistics are in shared memory
     ptx::wg_wait<0>();
     ptx::wg_fence_regs(s);
@@ -351,8 +401,14 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
           float v = s[n] * p.scale;
           if (!((w >> (r0 + 8 * hh)) & 1ull)) v = -FLT_MAX;
           const float pr = exp2f((v - mq) * LOG2E) * ilq;
-          s[n] = pr;                                    // P^T
-          dp[n] = p.scale * (pr * (dp[n] - dq_));       // dS^T
+          if constexpr (DROP) {                         // dq_ = keep_prob D
+            const bool keep = (s_keep[q] >> (r0 + 8 * hh)) & 1ull;
+            s[n] = keep ? pr : 0.f;                     // (P o Z)^T
+            dp[n] = (p.scale * p.rkeep) * (pr * ((keep ? dp[n] : 0.f) - dq_));   // dS^T
+          } else {
+            s[n] = pr;                                  // P^T
+            dp[n] = p.scale * (pr * (dp[n] - dq_));     // dS^T
+          }
         }
       }
     uint32_t a[4][4], g[4][4];
@@ -378,6 +434,10 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
   }
 
   // epilogue (a key block no query sees writes zeros)
+  if constexpr (DROP) {
+#pragma unroll
+    for (int n = 0; n < 32; ++n) dv[n] *= p.rkeep;
+  }
   const long long off = krow0 * S + col0 + wg * 64;
   store_rows<BF16>(reinterpret_cast<uint16_t*>(p.dk) + off, S, r0, lane, dk);
   store_rows<BF16>(reinterpret_cast<uint16_t*>(p.dv) + off, S, r0, lane, dv);
@@ -398,7 +458,7 @@ inline int tc_bst_attention_grad(int dtype, int bsize, const int32_t* nn_lut, co
                                  int autoregress_at_key, const void* q, const void* k, const void* v, const void* o,
                                  const void* dy, const float* row_max, const float* row_sum, float* delta, void* dq,
                                  void* dk, void* dv, float scale, int batch, int heads, int head_state, int ctx_blks_q,
-                                 int ctx_blks_k, cudaStream_t s) {
+                                 int ctx_blks_k, cudaStream_t s, const BstAttnDrop* drop = nullptr) {
   const void* const all[8] = {q, k, v, o, dy, dq, dk, dv};
   if (!bst_attention_grad_applicable(dtype, bsize, head_state, all)) return TC_NOT_APPLICABLE;
   const uint64_t S = (uint64_t)heads * head_state;
@@ -419,24 +479,29 @@ inline int tc_bst_attention_grad(int dtype, int bsize, const int32_t* nn_lut, co
   p.ctx_rows_q = ctx_blks_q * 64; p.ctx_rows_k = ctx_blks_k * 64;
   p.o = o; p.dy = dy; p.row_max = row_max; p.row_sum = row_sum; p.delta = delta;
   p.dq = dq; p.dk = dk; p.dv = dv;
+  set_drop(p, drop);
+  p.blocks = blocks;
   const int ch = head_state / 64;
   const size_t smem = (size_t)(2 + 2 * BST_BWD_STAGES) * ch * BST_TILE + SMEM_ALIGN_SLACK;
   const unsigned grid_q = (unsigned)((long long)batch * heads * ctx_blks_q);
   const unsigned grid_k = (unsigned)((long long)batch * heads * ctx_blks_k);
-#define BSMM_LAUNCH_BWD(BFV, CHV)                                                        \
-  { auto kq = wgmma_bst_attention_bwd_dq<BFV, CHV>;                                      \
-    auto kk = wgmma_bst_attention_bwd_dkdv<BFV, CHV>;                                    \
+#define BSMM_LAUNCH_BWD(BFV, CHV, DRV)                                                   \
+  { auto kq = wgmma_bst_attention_bwd_dq<BFV, CHV, DRV>;                                 \
+    auto kk = wgmma_bst_attention_bwd_dkdv<BFV, CHV, DRV>;                               \
     static thread_local uint64_t cfg_q = 0, cfg_k = 0;                                   \
     if (int e = ensure_dyn_smem(kq, smem, cfg_q)) return e;                              \
     if (int e = ensure_dyn_smem(kk, smem, cfg_k)) return e;                              \
     kq<<<grid_q, BST_THREADS, smem, s>>>(p, maps);                                       \
-    if (int e = check_launch("wgmma_bst_attention_bwd_dq")) return e;                    \
+    if (int e = check_launch(DRV ? "wgmma_bst_attention_bwd_dq_dropout" : "wgmma_bst_attention_bwd_dq")) return e; \
     kk<<<grid_k, BST_THREADS * CHV, smem, s>>>(p, maps); }
+#define BSMM_LAUNCH_BWD_CH(BFV, DRV) \
+  { if (ch == 2) BSMM_LAUNCH_BWD(BFV, 2, DRV) else BSMM_LAUNCH_BWD(BFV, 1, DRV) }
   const bool bf = dtype == BSMM_BF16;
-  if (ch == 2) { if (bf) BSMM_LAUNCH_BWD(true, 2) else BSMM_LAUNCH_BWD(false, 2) }
-  else { if (bf) BSMM_LAUNCH_BWD(true, 1) else BSMM_LAUNCH_BWD(false, 1) }
+  if (drop) { if (bf) BSMM_LAUNCH_BWD_CH(true, true) else BSMM_LAUNCH_BWD_CH(false, true) }
+  else { if (bf) BSMM_LAUNCH_BWD_CH(true, false) else BSMM_LAUNCH_BWD_CH(false, false) }
+#undef BSMM_LAUNCH_BWD_CH
 #undef BSMM_LAUNCH_BWD
-  return check_launch("wgmma_bst_attention_bwd_dkdv");
+  return check_launch(drop ? "wgmma_bst_attention_bwd_dkdv_dropout" : "wgmma_bst_attention_bwd_dkdv");
 }
 
 }  // namespace bsmm

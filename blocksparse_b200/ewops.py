@@ -189,6 +189,18 @@ def _gen_mask(x, M, keep_prob):
 
 
 @_on_device_of
+def _mask_at(x, M, keep_prob, state):
+    """The mask _gen_mask would draw for M elements if the device state held `state` (int64 [seed, call] on x's device).
+    It is drawn from a copy, so neither `state` nor the device state moves: a backward or a recomputation redraws the
+    mask of its forward from a snapshot."""
+    mask = torch.empty((M + 31) // 32, dtype=torch.int32, device=x.device)
+    if M:
+        rc = _lib.load().bsmm_dropout_mask(mask.data_ptr(), M, keep_prob, state.clone().data_ptr(), _lib.stream_ptr())
+        _lib.check(rc, "bsmm_dropout_mask")
+    return mask
+
+
+@_on_device_of
 def _apply_mask(x, mask, shape, strides, keep_prob):
     y = torch.empty_like(x)
     if x.numel() == 0:

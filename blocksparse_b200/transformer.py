@@ -159,9 +159,10 @@ class BlocksparseTransformer(TransformerCheckers):
         return dx
 
     @_lib.guarded
-    def _attention(self, q, k, v, scale, autoregress_at_key):
+    def _attention(self, q, k, v, scale, autoregress_at_key, keep_prob=1.0, seed_call=None):
         """Fused NT -> (masked) softmax -> NN in one launch, or None where the library has no fused kernel for the
-        call (BSMM_E_NOKERNEL): the caller then composes the three ops."""
+        call (BSMM_E_NOKERNEL): the caller then composes the three ops. keep_prob < 1 adds dropout on the probabilities
+        (bst_attention_dropout), its mask drawn at the int64 [seed, call] device tensor seed_call, which is not moved."""
         lib = _lib.load()
         if not q.is_cuda:
             raise _lib.BsmmError("BlocksparseTransformer needs CUDA tensors (no CPU path)")
@@ -176,19 +177,27 @@ class BlocksparseTransformer(TransformerCheckers):
         ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
         # one dtype code stands for q, k and v; mixed dtypes name none, and the library answers with E_NOKERNEL
         dt = _lib.dtype_code(q.dtype) if v.dtype == q.dtype else -1
-        rc = lib.bst_attention(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
-                               _lib.ptr(d["mask"]), self.lut_heads, ak,
-                               q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), float(scale),
-                               batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k, _lib.stream_ptr())
+        if keep_prob == 1.0:
+            rc = lib.bst_attention(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
+                                   _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                   q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), float(scale),
+                                   batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k, _lib.stream_ptr())
+        else:
+            rc = lib.bst_attention_dropout(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
+                                           _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                           q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), float(scale),
+                                           batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
+                                           float(keep_prob), _lib.ptr(seed_call), _lib.stream_ptr())
         if rc == _lib.E_NOKERNEL:
             return None
-        _lib.check(rc, "bst_attention")
+        _lib.check(rc, "bst_attention" if keep_prob == 1.0 else "bst_attention_dropout")
         return o
 
     @_lib.guarded
-    def _attention_train(self, q, k, v, scale, autoregress_at_key):
+    def _attention_train(self, q, k, v, scale, autoregress_at_key, keep_prob=1.0, seed_call=None):
         """_attention that also returns each query row's softmax statistics (max m and sum l, float32
-        (batch, heads, ctx_q)) for _attention_grad; None where the library has no fused kernel for the call."""
+        (batch, heads, ctx_q)) for _attention_grad; None where the library has no fused kernel for the call. keep_prob
+        and seed_call: as _attention (bst_attention_train_dropout); m and l do not depend on them."""
         lib = _lib.load()
         if not q.is_cuda:
             raise _lib.BsmmError("BlocksparseTransformer needs CUDA tensors (no CPU path)")
@@ -204,20 +213,28 @@ class BlocksparseTransformer(TransformerCheckers):
         d = self._device_luts(q.device)
         ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
         dt = _lib.dtype_code(q.dtype) if v.dtype == q.dtype else -1
-        rc = lib.bst_attention_train(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
-                                     _lib.ptr(d["mask"]), self.lut_heads, ak,
-                                     q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), m.data_ptr(), l.data_ptr(),
-                                     float(scale), batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
-                                     _lib.stream_ptr())
+        if keep_prob == 1.0:
+            rc = lib.bst_attention_train(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
+                                         _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                         q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), m.data_ptr(), l.data_ptr(),
+                                         float(scale), batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
+                                         _lib.stream_ptr())
+        else:
+            rc = lib.bst_attention_train_dropout(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
+                                                 _lib.ptr(d["mask"]), self.lut_heads, ak, q.data_ptr(), k.data_ptr(),
+                                                 v.data_ptr(), o.data_ptr(), m.data_ptr(), l.data_ptr(), float(scale),
+                                                 batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
+                                                 float(keep_prob), _lib.ptr(seed_call), _lib.stream_ptr())
         if rc == _lib.E_NOKERNEL:
             return None
-        _lib.check(rc, "bst_attention_train")
+        _lib.check(rc, "bst_attention_train" if keep_prob == 1.0 else "bst_attention_train_dropout")
         return o, m, l
 
     @_lib.guarded
-    def _attention_grad(self, q, k, v, o, dy, m, l, scale, autoregress_at_key):
-        """dq, dk, dv of the fused attention from what _attention_train saved, in one bst_attention_grad call. The
-        forward ran the fused kernel, so the call is inside its envelope; dy is made contiguous and aligned."""
+    def _attention_grad(self, q, k, v, o, dy, m, l, scale, autoregress_at_key, keep_prob=1.0, seed_call=None):
+        """dq, dk, dv of the fused attention from what _attention_train saved, in one bst_attention_grad call
+        (bst_attention_grad_dropout with the forward's keep_prob and seed_call). The forward ran the fused kernel, so
+        the call is inside its envelope; dy is made contiguous and aligned."""
         lib = _lib.load()
         dy = _aligned(dy.to(o.dtype))
         batch, ctx_q, S = q.shape
@@ -225,14 +242,24 @@ class BlocksparseTransformer(TransformerCheckers):
         delta = torch.empty_like(m)
         d = self._device_luts(q.device)
         ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
-        rc = lib.bst_attention_grad(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(), d["tn"].data_ptr(),
-                                    d["tn_order"].data_ptr(), self.lut_heads, self.blocks,
-                                    _lib.ptr(d["mask"]), self.lut_heads, ak,
-                                    q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dy.data_ptr(),
-                                    m.data_ptr(), l.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
-                                    float(scale), batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
-                                    _lib.stream_ptr())
-        _lib.check(rc, "bst_attention_grad")
+        if keep_prob == 1.0:
+            rc = lib.bst_attention_grad(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(), d["tn"].data_ptr(),
+                                        d["tn_order"].data_ptr(), self.lut_heads, self.blocks,
+                                        _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                        q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dy.data_ptr(),
+                                        m.data_ptr(), l.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+                                        float(scale), batch, self.heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
+                                        _lib.stream_ptr())
+        else:
+            rc = lib.bst_attention_grad_dropout(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(),
+                                                d["tn"].data_ptr(), d["tn_order"].data_ptr(), self.lut_heads, self.blocks,
+                                                _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                                q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dy.data_ptr(),
+                                                m.data_ptr(), l.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(),
+                                                dv.data_ptr(), float(scale), batch, self.heads, S // self.heads,
+                                                self.ctx_blks_q, self.ctx_blks_k, float(keep_prob), _lib.ptr(seed_call),
+                                                _lib.stream_ptr())
+        _lib.check(rc, "bst_attention_grad" if keep_prob == 1.0 else "bst_attention_grad_dropout")
         return dq, dk, dv
 
     def partial_autoregressive_mask(self, autoregress_at_key, device="cuda"):
@@ -310,7 +337,8 @@ class BlocksparseTransformer(TransformerCheckers):
         dtype = dtype or self.softmax_dtype or x.dtype
         return _SoftmaxFunction.apply(x, self, float(scale), False, None, dtype)
 
-    def attention(self, q, k, v, scale=1.0, autoregress_at_key=None, fused_backward=False):
+    def attention(self, q, k, v, scale=1.0, autoregress_at_key=None, fused_backward=False, keep_prob=1.0,
+                  dropout_state=None):
         """weight_value_op(masked_softmax(query_key_op(q, k), scale, autoregress_at_key), v) -- softmax without a
         mask_callback -- as one fused kernel that never writes the (batch, heads, blocks, bs, bs) scores or
         probabilities; the backward pass recomputes them from q and k. Returns (batch, ctx_q, heads*head_state) in
@@ -321,16 +349,59 @@ class BlocksparseTransformer(TransformerCheckers):
         chain's, which rounds the scores and dS to bfloat16 and holds several sparse tensors during the backward.
         True: the forward also keeps each row's softmax max and sum, and the backward is two fused kernels that keep the
         scores in fp32 and store nothing of sparse shape. The output is the same either way; so is the fallback to the
-        three ops outside the fused kernels' envelope."""
+        three ops outside the fused kernels' envelope.
+
+        keep_prob < 1 applies dropout to the probabilities, inside the fused kernels: the result is that of
+        weight_value_op(ewops.dropout(masked_softmax(...), keep_prob)[0], v), with the very mask dropout would draw for
+        the (batch, heads, blocks, bs, bs) probabilities at the same state, and nothing of sparse shape is stored.
+        Without dropout_state the mask is drawn from the device state ewops.get_entropy(q.device), whose call advances
+        by one, as one dropout call's would. A dropout_state (int64 CUDA tensor [seed, call] on q's device) is used as
+        it is and never advanced, so a block recomputed under checkpointing draws its forward's mask again. Autograd
+        keeps a copy of (seed, call) on the device and the backward redraws the mask from it; nothing synchronises with
+        the host, so forward and backward can be captured in a CUDA graph. fused_backward=False keeps its contract:
+        gradients bit-identical to the chain's with ewops.dropout in it. Outside the fused envelope the op runs that
+        chain with the same mask. keep_prob == 1.0 runs exactly the code without dropout and reads no state."""
         if autoregress_at_key is not None and self.softmax_mask_np is None:
             raise ValueError("autoregress_at_key only applies to ops with mask_callback defined.")
+        kp = _keep_prob(keep_prob)
+        if dropout_state is not None and not (torch.is_tensor(dropout_state) and dropout_state.dtype == torch.int64
+                                              and dropout_state.numel() == 2 and dropout_state.device == q.device):
+            raise ValueError("attention: dropout_state must be an int64 CUDA tensor [seed, call] on %s, got %s" % (
+                q.device, (dropout_state.dtype, dropout_state.device, tuple(dropout_state.shape))
+                if torch.is_tensor(dropout_state) else type(dropout_state)))
+        if kp == 1.0:
+            try:
+                if fused_backward:
+                    return _AttentionTrainFunction.apply(q, k, v, self, float(scale), autoregress_at_key, 1.0, None)
+                return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key, 1.0, None)
+            except _NoFusedKernel:
+                w = self.query_key_op(q, k)
+                return self.weight_value_op(self.masked_softmax(w, scale, autoregress_at_key), v)
+        from . import ewops
+        if dropout_state is None:
+            state = ewops.get_entropy(q.device)
+            snap = state.clone()
+            state[1:].add_(1)
+        else:
+            snap = dropout_state.detach().reshape(2).clone()
         try:
             if fused_backward:
-                return _AttentionTrainFunction.apply(q, k, v, self, float(scale), autoregress_at_key)
-            return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key)
+                return _AttentionTrainFunction.apply(q, k, v, self, float(scale), autoregress_at_key, kp, snap)
+            return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key, kp, snap)
         except _NoFusedKernel:
-            w = self.query_key_op(q, k)
-            return self.weight_value_op(self.masked_softmax(w, scale, autoregress_at_key), v)
+            p = self.masked_softmax(self.query_key_op(q, k), scale, autoregress_at_key)
+            p, _ = ewops.dropout(p, kp, mask=ewops._mask_at(p, p.numel(), kp, snap))
+            return self.weight_value_op(p, v)
+
+
+def _keep_prob(keep_prob):
+    """keep_prob as a float in (0, 1] (ValueError otherwise, as ewops.dropout)."""
+    if not isinstance(keep_prob, (int, float)) or isinstance(keep_prob, bool):
+        raise ValueError("attention: keep_prob must be a Python float, got %r" % (keep_prob,))
+    kp = float(keep_prob)
+    if not 0.0 < kp <= 1.0:
+        raise ValueError("attention: keep_prob must be in (0, 1], got %r" % (keep_prob,))
+    return kp
 
 
 class _NtFunction(torch.autograd.Function):
@@ -380,58 +451,78 @@ class _NoFusedKernel(Exception):
 
 
 class _AttentionFunction(torch.autograd.Function):
-    """Fused attention. Saves q, k and v only; the backward recomputes the scores and the probabilities with the
-    chain's own NT and softmax kernels, then runs the chain's backward ops (_XnFunction, _SoftmaxFunction and
-    _NtFunction in turn) on them, so its gradients are bit-identical to the three-op chain's."""
+    """Fused attention. Saves q, k and v only (and with dropout the [seed, call] snapshot); the backward recomputes the
+    scores and the probabilities with the chain's own NT and softmax kernels, then runs the chain's backward ops
+    (_XnFunction, _DropoutFunction with the mask redrawn from the snapshot, _SoftmaxFunction and _NtFunction in turn)
+    on them, so its gradients are bit-identical to the chain's."""
 
     @staticmethod
-    def forward(ctx, q, k, v, bst, scale, autoregress_at_key):
-        o = bst._attention(q, k, v, scale, autoregress_at_key)
+    def forward(ctx, q, k, v, bst, scale, autoregress_at_key, keep_prob, snap):
+        o = bst._attention(q, k, v, scale, autoregress_at_key, keep_prob, snap)
         if o is None:
             raise _NoFusedKernel()
-        ctx.bst, ctx.scale, ctx.ak = bst, scale, autoregress_at_key
-        ctx.save_for_backward(q, k, v)
+        ctx.bst, ctx.scale, ctx.ak, ctx.keep_prob = bst, scale, autoregress_at_key, keep_prob
+        if snap is None:
+            ctx.save_for_backward(q, k, v)
+        else:
+            ctx.save_for_backward(q, k, v, snap)
         return o
 
     @staticmethod
     def backward(ctx, dy):
-        q, k, v = ctx.saved_tensors
-        bst, scale = ctx.bst, ctx.scale
+        q, k, v = ctx.saved_tensors[:3]
+        bst, scale, kp = ctx.bst, ctx.scale, ctx.keep_prob
         dy = dy.contiguous()
         # forward of the chain up to the probabilities: bf16 scores, probabilities in q's dtype (query_key_op)
         p = bst._softmax(bst._nt(q, k, torch.bfloat16), scale, bst.softmax_mask_np is not None, ctx.ak, q.dtype)
+        pd, drop = p, None
+        if kp != 1.0:                      # the chain's dropout of p, with the forward's mask
+            from . import ewops
+            shape = tuple(p.shape)
+            mask = ewops._mask_at(p, p.numel(), kp, ctx.saved_tensors[3])
+            drop = lambda x: ewops._apply_mask(x.contiguous(), mask, shape, ewops._mask_strides(x, shape), kp)
+            pd = drop(p)
         dq = dk = dv = None
         if ctx.needs_input_grad[2]:
-            dv = bst._xn(p, dy, True)
+            dv = bst._xn(pd, dy, True)
         if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
-            dw = bst._softmax_grad(bst._nt(dy, v, p.dtype), p, scale).to(torch.bfloat16).contiguous()
+            dp = bst._nt(dy, v, p.dtype)
+            if drop is not None:
+                dp = drop(dp)
+            dw = bst._softmax_grad(dp, p, scale).to(torch.bfloat16).contiguous()
             if ctx.needs_input_grad[1]:
                 dk = bst._xn(dw, q, True)
             if ctx.needs_input_grad[0]:
                 dq = bst._xn(dw, k, False)
-        return dq, dk, dv, None, None, None
+        return dq, dk, dv, None, None, None, None, None
 
 
 class _AttentionTrainFunction(torch.autograd.Function):
-    """Fused attention with a fused backward. Saves q, k, v, o and the row statistics (nothing of sparse shape); the
-    backward computes dq, dk and dv in one bst_attention_grad call and returns the requested ones."""
+    """Fused attention with a fused backward. Saves q, k, v, o and the row statistics (and with dropout the
+    [seed, call] snapshot; nothing of sparse shape); the backward computes dq, dk and dv in one bst_attention_grad call
+    and returns the requested ones."""
 
     @staticmethod
-    def forward(ctx, q, k, v, bst, scale, autoregress_at_key):
-        r = bst._attention_train(q, k, v, scale, autoregress_at_key)
+    def forward(ctx, q, k, v, bst, scale, autoregress_at_key, keep_prob, snap):
+        r = bst._attention_train(q, k, v, scale, autoregress_at_key, keep_prob, snap)
         if r is None:
             raise _NoFusedKernel()
         o, m, l = r
-        ctx.bst, ctx.scale, ctx.ak = bst, scale, autoregress_at_key
-        ctx.save_for_backward(q.contiguous(), k.contiguous(), v.contiguous(), o, m, l)
+        ctx.bst, ctx.scale, ctx.ak, ctx.keep_prob = bst, scale, autoregress_at_key, keep_prob
+        if snap is None:
+            ctx.save_for_backward(q.contiguous(), k.contiguous(), v.contiguous(), o, m, l)
+        else:
+            ctx.save_for_backward(q.contiguous(), k.contiguous(), v.contiguous(), o, m, l, snap)
         return o
 
     @staticmethod
     def backward(ctx, dy):
-        q, k, v, o, m, l = ctx.saved_tensors
-        dq, dk, dv = ctx.bst._attention_grad(q, k, v, o, dy, m, l, ctx.scale, ctx.ak)
+        q, k, v, o, m, l = ctx.saved_tensors[:6]
+        snap = ctx.saved_tensors[6] if ctx.keep_prob != 1.0 else None
+        dq, dk, dv = ctx.bst._attention_grad(q, k, v, o, dy, m, l, ctx.scale, ctx.ak, ctx.keep_prob, snap)
         need = ctx.needs_input_grad
-        return dq if need[0] else None, dk if need[1] else None, dv if need[2] else None, None, None, None
+        return (dq if need[0] else None, dk if need[1] else None, dv if need[2] else None,
+                None, None, None, None, None)
 
 
 class _SoftmaxFunction(torch.autograd.Function):

@@ -19,6 +19,7 @@
  *   bst_softmax_grad      <- BlocksparseSoftmaxGrad<T,V>   (src/bst_op.cc:443-512)
  *   bst_autoregressive_mask <- BstPartialAutoregressiveMask (src/bst_op.cc:519-575)
  *   bst_attention         <- no single launcher: replaces bst_nt + bst_masked_softmax + bst_xn (NN)
+ *   bst_attention_dropout <- no single launcher: the same with bsmm_dropout_mask + bsmm_dropout_apply on the probabilities
  *   bst_dense_softmax(_grad) <- MaskedSoftmax / MaskedSoftmaxGrad (src/transformer_op.cc:211-367)
  *   bst_topk_softmax      <- MaskedTopKSoftmax (src/transformer_op.cc:145-208)
  *   bst_topk              <- TopK behind Topk / RectifiedTopK (src/transformer_op.cc:20-141)
@@ -310,6 +311,48 @@ int bst_attention_grad(int dtype, int bsize, const int32_t* nn_lut, const int32_
                        const void* q, const void* k, const void* v, const void* o, const void* dy,
                        const float* row_max, const float* row_sum, float* delta, void* dq, void* dk, void* dv, float scale,
                        int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k, void* stream);
+
+/*
+ * Attention dropout inside the fused kernels: bst_attention, bst_attention_train and bst_attention_grad with dropout
+ * on the normalised probabilities, each taking its counterpart's arguments plus keep_prob and seed_call (before
+ * stream).  The result is that of bst_nt + bst_masked_softmax + bsmm_dropout_apply(mask of bsmm_dropout_mask) +
+ * bst_xn(NN) at the same (seed, call), computed as
+ *   o_i = sum_j Z_ij exp(s_ij - m_i) v_j / (keep_prob l_i),
+ * with m and l the row max and sum over every visible key: Z does not enter them, and the row_max / row_sum that
+ * bst_attention_train_dropout stores are bst_attention_train's.  The gradients are those of this o:
+ * dv = (P o Z)^T dy / keep_prob, dP = (dy v^T) o Z / keep_prob, delta = rowsum(dy o o), dS = scale P o (dP - delta).
+ * Z is the mask bsmm_dropout_mask draws for the chain's (batch, heads, blocks, 64, 64) probabilities, bit for bit:
+ *   element e = (((b * heads + h) * blocks + blk) * 64 + i) * 64 + j   (64-bit; h enters e with lut_heads = 1 too)
+ *   of batch b, head h, block blk (the block id of the nn_lut / tn_lut entry, as the softmax mask indexes it), query row
+ *   i of the block and key column j, is kept iff word e % 4 of Philox4x32-10(counter = (e / 4 as 64 bits, call as 64
+ *   bits), key = seed) is below floor(keep_prob * 2^32), compared in 64 bits.
+ * A fully masked row has uniform P and is dropped like any other; an empty LUT row still writes zeros.
+ * seed_call: device int64 [seed, call], read by the kernels and never written; advancing call (as one
+ * bsmm_dropout_mask call does) is the caller's job, which lets a backward or a recomputed forward redraw the same mask.
+ * keep_prob is a double so that the threshold is bsmm_dropout_mask's.  keep_prob 1 runs the counterpart's kernels and
+ * reads nothing (seed_call may then be null).  keep_prob outside (0, 1], or a null seed_call with keep_prob < 1:
+ * BSMM_E_ARG before any launch; otherwise the counterpart's argument checks, envelope and BSMM_E_NOKERNEL (before any
+ * launch) apply.  No reference launcher corresponds to them.  Kernels: wgmma_bst_attention_dropout,
+ * wgmma_bst_attention_train_dropout, wgmma_bst_attention_bwd_dq_dropout + wgmma_bst_attention_bwd_dkdv_dropout.
+ */
+int bst_attention_dropout(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                          const void* mask, int mask_heads, int autoregress_at_key,
+                          const void* q, const void* k, const void* v, void* o, float scale,
+                          int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                          double keep_prob, const int64_t* seed_call, void* stream);
+
+int bst_attention_train_dropout(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                                const void* mask, int mask_heads, int autoregress_at_key,
+                                const void* q, const void* k, const void* v, void* o, float* row_max, float* row_sum,
+                                float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                                double keep_prob, const int64_t* seed_call, void* stream);
+
+int bst_attention_grad_dropout(int dtype, int bsize, const int32_t* nn_lut, const int32_t* tn_lut, const int32_t* tn_order,
+                               int lut_heads, int blocks, const void* mask, int mask_heads, int autoregress_at_key,
+                               const void* q, const void* k, const void* v, const void* o, const void* dy,
+                               const float* row_max, const float* row_sum, float* delta, void* dq, void* dk, void* dv,
+                               float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                               double keep_prob, const int64_t* seed_call, void* stream);
 
 /* mask_out[hl][blk][r] = mask_in[hl][blk][r] & (ones >> shift(r)), same layout as bst_softmax's mask */
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,

@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbsmm_b200.so")
 
 F32, F16, BF16 = 0, 1, 2
-E4M3, E5M2 = 3, 4        # BSMM_E4M3 / BSMM_E5M2: accepted by the bsmm_fp8_* entries and bsmm_xprop_fp8 only
+E4M3, E5M2 = 3, 4        # BSMM_E4M3 / BSMM_E5M2: accepted by the bsmm_fp8_* entries, bsmm_xprop_fp8 and bsmm_updat_fp8 only
 FLAG_FORCE_GENERIC, FLAG_FORCE_TC = 1, 2
 MAX_PAIRS = 8
 E_NOKERNEL = -7          # BSMM_E_NOKERNEL: no fused kernel for the configuration
@@ -114,6 +114,9 @@ SIGNATURES = {
     "bsmm_fp8_quantize": (_i, [_i, _i, _vp, _ll, _vp, _vp, _vp, _vp]),
     "bsmm_fp8_weights": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bsmm_xprop_fp8": (_i, [_i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "bsmm_fp8_quantize_t": (_i, [_i, _i, _vp, _ll, _ll, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "bsmm_updat_fp8": (_i, [_i, _i, _i, _i, _i, _i, _i, _c.POINTER(_vp), _c.POINTER(_vp), _c.POINTER(_vp),
+                            _c.POINTER(_vp), _i, _vp, _ll, _ll, _f, _vp, _i, _i, _vp]),
     "bsmm_block_norm":(_i, [_i, _i, _i, _vp, _vp, _i, _vp]),
     "bsmm_l2_decay": (_i, [_i, _i, _i, _vp, _vp, _f, _f, _vp]),
     "bsmm_threshold_prune": (_i, [_i, _i, _i, _vp, _vp, _f, _i, _vp]),

@@ -18,6 +18,7 @@
 #include "softmax.cuh"
 #include "tc.cuh"
 #include "tc_fp8.cuh"
+#include "tc_updat_fp8.cuh"
 #include "transpose.cuh"
 #include "wutil.cuh"
 
@@ -1971,5 +1972,65 @@ int bsmm_xprop_fp8(int x_dtype, int w_dtype, int y_dtype, int axis, int bsize, i
   if (N == 0) return 0;
   return tc_xprop_fp8(x_dtype, w_dtype, y_dtype, bsize, lut, n_out, n_in, blocks, x, w, y, N, x_scale_inv, w_scale_inv,
                       (cudaStream_t)stream);
+}
+
+int bsmm_fp8_quantize_t(int src_dtype, int fp8_dtype, const void* x, long long rows, long long cols, float* amax,
+                        float* scale_inv, void* y, void* yt, long long yt_pitch, void* stream) {
+  const char* what = "bsmm_fp8_quantize_t";
+  if (!fp8_src_ok(src_dtype) || !fp8_code(fp8_dtype))
+    return fail(BSMM_E_DTYPE, "%s: needs an fp32 / fp16 / bf16 source and an e4m3 / e5m2 target, got %d -> %d", what, src_dtype, fp8_dtype);
+  if (rows < 0 || cols < 0) return fail(BSMM_E_ARG, "%s: negative size %lld x %lld", what, rows, cols);
+  if (!amax || !scale_inv || (!y && !yt)) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (rows * cols > 0 && !x) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (yt) {
+    if (yt_pitch < rows) return fail(BSMM_E_ARG, "%s: yt_pitch %lld below rows %lld", what, yt_pitch, rows);
+    if (yt_pitch % 16) return fail(BSMM_E_ALIGN, "%s: yt_pitch %lld is not a multiple of 16", what, yt_pitch);
+    if ((uintptr_t)yt & 3) return fail(BSMM_E_ALIGN, "%s: yt must be 4-byte aligned", what);
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  uint8_t *q = (uint8_t*)y, *qt = (uint8_t*)yt;
+  BSMM_DISPATCH_DTYPE(src_dtype, T, {
+    const T* xt = (const T*)x;
+    return fp8_dtype == BSMM_E5M2 ? launch_fp8_quantize_t<T, BSMM_E5M2>(xt, rows, cols, amax, scale_inv, q, qt, yt_pitch, s)
+                                  : launch_fp8_quantize_t<T, BSMM_E4M3>(xt, rows, cols, amax, scale_inv, q, qt, yt_pitch, s);
+  });
+  return 0;
+}
+
+int bsmm_updat_fp8(int x_dtype, int dy_dtype, int dw_dtype, int bsize, int blocks, int n_c_blocks, int n_k_blocks,
+                   const void* const* xts, const void* const* dyts, const float* const* x_scale_invs,
+                   const float* const* dy_scale_invs, int pcount, void* dw, long long N, long long pitch, float beta,
+                   const int32_t* sched, int sched_tiles, int sched_tile_blocks, void* stream) {
+  const char* what = "bsmm_updat_fp8";
+  if (bsize != 32 && bsize != 64) return fail(BSMM_E_BSIZE, "%s: fp8 updat needs block size 32 or 64, got %d", what, bsize);
+  if (!fp8_code(x_dtype) || !fp8_code(dy_dtype) || !fp8_src_ok(dw_dtype))
+    return fail(BSMM_E_DTYPE, "%s: needs e4m3 / e5m2 xt and dyt and an fp32 / fp16 / bf16 dw, got xt %d, dyt %d, dw %d", what,
+                x_dtype, dy_dtype, dw_dtype);
+  if (pcount < 1 || pcount > BSMM_MAX_PAIRS)
+    return fail(BSMM_E_ARG, "%s: pcount must be in [1,%d], got %d", what, BSMM_MAX_PAIRS, pcount);
+  if (!xts || !dyts || !x_scale_invs || !dy_scale_invs || !dw || !sched) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  for (int i = 0; i < pcount; ++i)
+    if (!xts[i] || !dyts[i] || !x_scale_invs[i] || !dy_scale_invs[i]) return fail(BSMM_E_ARG, "%s: null pointer in pair %d", what, i);
+  if (N < 0) return fail(BSMM_E_ARG, "%s: negative N %lld", what, N);
+  if (pitch < N) return fail(BSMM_E_ARG, "%s: pitch %lld below N %lld", what, pitch, N);
+  if (pitch % 16) return fail(BSMM_E_ALIGN, "%s: pitch %lld is not a multiple of 16", what, pitch);
+  if (beta != 0.f && beta != 1.f) return fail(BSMM_E_ARG, "%s: beta must be 0 or 1", what);
+  if (blocks <= 0 || n_c_blocks <= 0 || n_k_blocks <= 0 || sched_tiles <= 0) return fail(BSMM_E_ARG, "%s: bad sizes", what);
+  if (sched_tile_blocks != 256 / bsize)
+    return fail(BSMM_E_ARG, "%s: schedule built for %d slots per tile, kernel needs %d", what, sched_tile_blocks, 256 / bsize);
+  if (N > INT_MAX) return fail(BSMM_E_LIMIT, "%s: N above 2^31 - 1", what);
+  if ((uintptr_t)dw & 15) return fail(BSMM_E_ALIGN, "%s: dw must be 16-byte aligned", what);
+  for (int i = 0; i < pcount; ++i)
+    if (((uintptr_t)xts[i] | (uintptr_t)dyts[i]) & 15) return fail(BSMM_E_ALIGN, "%s: xt and dyt must be 16-byte aligned", what);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (N == 0) {                                        // as bsmm_updat: an empty sum, so dw = 0 (beta 0) or unchanged
+    if (beta != 0.f) return 0;
+    const size_t bytes = (size_t)blocks * bsize * bsize * (dw_dtype == BSMM_F32 ? 4 : 2);
+    cudaError_t e = cudaMemsetAsync(dw, 0, bytes, s);
+    if (e != cudaSuccess) { cudaGetLastError(); return fail((int)e, "%s: %s", what, cudaGetErrorString(e)); }
+    return 0;
+  }
+  return tc_updat_fp8(x_dtype, dy_dtype, dw_dtype, bsize, n_c_blocks, n_k_blocks, xts, dyts, x_scale_invs, dy_scale_invs,
+                      pcount, dw, N, pitch, beta != 0.f ? 1 : 0, sched, sched_tiles, s);
 }
 }  // extern "C"

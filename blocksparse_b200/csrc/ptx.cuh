@@ -301,7 +301,7 @@ __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b)
   else wgmma_n256<BF16, TA, TB>(d, a, b);
 }
 
-// D[64 x N] (fp32, registers) = A[64 x 32] * B[32 x N] (+ D when scale_d != 0), fp8 operands: AT / BT = 0 for e4m3,
+// D[64 x N] (fp32, registers, N = 32, 64 or 128) = A[64 x 32] * B[32 x N] (+ D when scale_d != 0), fp8 operands: AT / BT = 0 for e4m3,
 // 1 for e5m2. fp8 wgmma takes no transpose flags, so both operands are K-major. Accumulator layout as above.
 #define BSMM_WG8_N32(types)                                                                                      \
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"                                               \
@@ -314,6 +314,16 @@ __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b)
                "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"                                        \
                "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}\n"    \
                : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24)                           \
+               : "l"(a), "l"(b), "r"(scale_d))
+#define BSMM_WG8_N128(types)                                                                                     \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n128k32.f32." types " "                                         \
+               "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"                                        \
+               "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"                               \
+               "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"                               \
+               "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}\n"    \
+               : BSMM_WG_OPS8(0), BSMM_WG_OPS8(8), BSMM_WG_OPS8(16), BSMM_WG_OPS8(24),                          \
+                 BSMM_WG_OPS8(32), BSMM_WG_OPS8(40), BSMM_WG_OPS8(48), BSMM_WG_OPS8(56)                         \
                : "l"(a), "l"(b), "r"(scale_d))
 template <int AT, int BT>
 __device__ __forceinline__ void wgmma_fp8_n32(float (&d)[16], uint64_t a, uint64_t b, int scale_d) {
@@ -329,11 +339,20 @@ __device__ __forceinline__ void wgmma_fp8_n64(float (&d)[32], uint64_t a, uint64
   else if constexpr (BT == 0) BSMM_WG8_N64("e5m2.e4m3");
   else BSMM_WG8_N64("e5m2.e5m2");
 }
+template <int AT, int BT>
+__device__ __forceinline__ void wgmma_fp8_n128(float (&d)[64], uint64_t a, uint64_t b, int scale_d) {
+  if constexpr (AT == 0 && BT == 0) BSMM_WG8_N128("e4m3.e4m3");
+  else if constexpr (AT == 0) BSMM_WG8_N128("e4m3.e5m2");
+  else if constexpr (BT == 0) BSMM_WG8_N128("e5m2.e4m3");
+  else BSMM_WG8_N128("e5m2.e5m2");
+}
 template <int AT, int BT, int N>
 __device__ __forceinline__ void wgmma_fp8(float (&d)[N / 2], uint64_t a, uint64_t b, int scale_d) {
   if constexpr (N == 32) wgmma_fp8_n32<AT, BT>(d, a, b, scale_d);
-  else wgmma_fp8_n64<AT, BT>(d, a, b, scale_d);
+  else if constexpr (N == 64) wgmma_fp8_n64<AT, BT>(d, a, b, scale_d);
+  else wgmma_fp8_n128<AT, BT>(d, a, b, scale_d);
 }
+#undef BSMM_WG8_N128
 #undef BSMM_WG8_N64
 #undef BSMM_WG8_N32
 #undef BSMM_WG_TAIL

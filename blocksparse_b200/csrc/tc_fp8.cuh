@@ -6,6 +6,9 @@
 //   fp8_quantize  y = cvt.rn.satfinite(x * s), s = FP8_MAX / amax; block 0 also stores scale_inv = amax / FP8_MAX.
 //   fp8_weights   the same cast over a (blocks, bs, bs) weight tensor, one CTA per block, writing the block as stored
 //                 and transposed.
+//   fp8_quantize_t (bsmm_fp8_quantize_t) the same cast over a (rows, cols) tensor in 64 x 64 tiles, writing it as
+//                 stored and / or transposed with a padded pitch: the feature-major operands of the fp8 updat
+//                 (csrc/tc_updat_fp8.cuh).
 //
 // xprop (DESIGN.md "fp8 fprop / bprop"): tc_xprop_kernel's formulation (csrc/tc.cuh) with 1-byte operands. One CTA (one
 // warpgroup) owns one output block of 128 minibatch rows and walks its LUT row in order, TMA staging each entry's
@@ -116,6 +119,43 @@ __global__ void __launch_bounds__(FP8_THREADS) fp8_weights_kernel(const T* __res
   }
 }
 
+// The cast of fp8_quantize over a (rows, cols) tensor in 64 x 64 tiles, writing y (rows x cols, as fp8_quantize does)
+// and / or yt[c][r] (cols x pitch, zero in [rows, pitch)). Each tile goes through shared memory as t[c][r], so the
+// loads of x, the stores of y and the 4-byte stores of yt all run along rows. Codes are those of fp8_quantize: the
+// same fp32 product and the same per-element conversion.
+constexpr int FP8T_TILE = 64;
+template <typename T, int FMT>
+__global__ void __launch_bounds__(FP8_THREADS) fp8_quantize_t_kernel(const T* __restrict__ x, long long rows, long long cols,
+                                                                      const float* amax, float* scale_inv, uint8_t* y,
+                                                                      uint8_t* yt, long long pitch, long long row_tiles,
+                                                                      long long tiles) {
+  constexpr int TL = FP8T_TILE;
+  __shared__ __align__(4) uint8_t t[TL][TL + 4];
+  const float a = *amax, s = fp8_scale<FMT>(a);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *scale_inv = fp8_scale_inv<FMT>(a);
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const long long r0 = (tile % row_tiles) * TL, c0 = (tile / row_tiles) * TL;
+    for (int i = threadIdx.x; i < TL * TL; i += FP8_THREADS) {
+      const int r = i / TL, c = i % TL;
+      const long long gr = r0 + r, gc = c0 + c;
+      uint8_t q = 0;
+      if (gr < rows && gc < cols) {
+        q = fp8x1<FMT>(__fmul_rn(to_f32<T>(x[gr * cols + gc]), s));
+        if (y) y[gr * cols + gc] = q;
+      }
+      t[c][r] = q;
+    }
+    __syncthreads();
+    if (yt)
+      for (int i = threadIdx.x; i < TL * TL / 4; i += FP8_THREADS) {
+        const int c = i / (TL / 4), r = 4 * (i % (TL / 4));
+        const long long gc = c0 + c, gr = r0 + r;                // pitch % 16 == 0: gr < pitch covers gr + 3 too
+        if (gc < cols && gr < pitch) *reinterpret_cast<uint32_t*>(yt + gc * pitch + gr) = *reinterpret_cast<const uint32_t*>(&t[c][r]);
+      }
+    __syncthreads();
+  }
+}
+
 template <typename T>
 inline int launch_fp8_amax(const T* x, long long n, float* amax, cudaStream_t s) {
   cudaError_t e = cudaMemsetAsync(amax, 0, sizeof(float), s);
@@ -140,6 +180,19 @@ inline int launch_fp8_quantize(const T* x, long long n, float* amax, float* scal
   const unsigned grid = (unsigned)(ctas < 1 ? 1 : ctas < FP8_MAX_CTAS ? ctas : FP8_MAX_CTAS);
   fp8_quantize_kernel<T, FMT><<<grid, FP8_THREADS, 0, s>>>(x, n, vec, amax, scale_inv, y);
   return check_launch("fp8_quantize");
+}
+
+template <typename T, int FMT>
+inline int launch_fp8_quantize_t(const T* x, long long rows, long long cols, float* amax, float* scale_inv, uint8_t* y,
+                                 uint8_t* yt, long long pitch, cudaStream_t s) {
+  if (int e = launch_fp8_amax<T>(x, rows * cols, amax, s)) return e;
+  const long long span = yt && pitch > rows ? pitch : rows;      // yt's zero pad lies in rows [rows, pitch)
+  const long long row_tiles = (span + FP8T_TILE - 1) / FP8T_TILE, col_tiles = (cols + FP8T_TILE - 1) / FP8T_TILE;
+  const long long tiles = row_tiles * col_tiles;
+  const unsigned grid = (unsigned)(tiles < 1 ? 1 : tiles < 8 * FP8_MAX_CTAS ? tiles : 8 * FP8_MAX_CTAS);  // tiles = 0: scale_inv only
+  fp8_quantize_t_kernel<T, FMT><<<grid, FP8_THREADS, 0, s>>>(x, rows, cols, amax, scale_inv, y, yt, pitch,
+                                                              row_tiles > 0 ? row_tiles : 1, tiles);
+  return check_launch("fp8_quantize_t");
 }
 
 template <typename T, int FMT>

@@ -14,7 +14,7 @@ import torch
 
 from . import _lib
 from .checkers import MatmulCheckers
-from .fp8 import check_config as _fp8_check_config, quantize_fp8, quantize_fp8_weights, xprop_fp8
+from .fp8 import check_config as _fp8_check_config, quantize_fp8, quantize_fp8_t, quantize_fp8_weights, updat_fp8, xprop_fp8
 from .lut import MatmulLuts, WIDE_REC, XPROP_GROUP, pick_xprop_tile
 
 # 32 x 32 blocks and 16-bit dtypes: the default route picks, per layout, direction and minibatch, between one output block
@@ -364,13 +364,20 @@ class BlocksparseMatMul(MatmulCheckers):
             self._bench_op("fprop", lambda: self.fprop(I, W, gate), I, bench, name or self.name)
         return _BsmmFunction.apply(I, W, gate, self, bool(gate_grad), bool(dw_gated), int(bench), name or self.name)
 
-    def matmul_fp8(self, I, W, name=None):
-        """y = bsmm(I, W) on fp8 tensor cores, with gradients for I and W (DESIGN.md 6e).
+    def matmul_fp8(self, I, W, name=None, fp8_dw=False):
+        """y = bsmm(I, W) on fp8 tensor cores, with gradients for I and W (DESIGN.md 6e, 6f).
 
         Forward: I and W are quantised to e4m3 with one scale each (fp8.quantize_fp8 / quantize_fp8_weights) and the fp8
         fprop runs; y comes out in I's dtype. Backward: dy is quantised to e5m2 and the fp8 bprop runs against the saved
-        e4m3 weights, so dx comes out in I's dtype; dw is the 16-bit updat of the saved I and dy, exactly as in
-        bsmm(I, W)'s backward (group_param_grads included), so it is bit-identical to it.
+        e4m3 weights, so dx comes out in I's dtype.
+        dw: with fp8_dw=False it is the 16-bit updat of the saved I and dy, exactly as in bsmm(I, W)'s backward
+        (group_param_grads included), so it is bit-identical to it. With fp8_dw=True it is the fp8 updat (fp8.updat_fp8)
+        of the e4m3 I and the e5m2 dy, in W's dtype: the forward keeps a transposed e4m3 copy of I (quantize_fp8_t, one
+        byte per element) instead of I itself, and the backward quantises dy once for both the bprop and the updat.
+        y and dx are bit-identical to fp8_dw=False's. fp8_dw is a precision choice, not a speed switch: dw then carries
+        the quantisation error of both operands, and against the float64 product of the dequantised operands it is
+        within (2^-11 + (stages + 3) 2^-24) sum|x^||dy^| + u_out |dw|, stages being the 128-row minibatch chunks summed
+        (DESIGN.md 6f gives the bound and where the fp8 updat is faster or slower than the 16-bit one).
         I (..., C) and W (blocks, bs, bs) are float16 or bfloat16 CUDA tensors of one dtype; feature_axis 1 and block
         sizes 32 / 64 only. There is no gate argument. `name` is accepted for symmetry with __call__."""
         _fp8_check_config(self)
@@ -388,6 +395,8 @@ class BlocksparseMatMul(MatmulCheckers):
         if I.device != W.device:
             raise ValueError("matmul_fp8: I lives on %s, W on %s" % (I.device, W.device))
         self.count += 1
+        if fp8_dw:
+            return _Fp8DwMatmulFunction.apply(I, W, self)
         return _Fp8MatmulFunction.apply(I, W, self)
 
     def _bench_op(self, what, fn, I, repeat, name):
@@ -474,6 +483,38 @@ class _Fp8MatmulFunction(torch.autograd.Function):
         return dx, dw, None
 
 
+class _Fp8DwMatmulFunction(torch.autograd.Function):
+    """BlocksparseMatMul.matmul_fp8(fp8_dw=True): e4m3 fprop, e5m2 x e4m3 bprop, e4m3 x e5m2 updat. I is kept only as
+    its transposed e4m3 copy."""
+
+    @staticmethod
+    def forward(ctx, x, w, bsmm):
+        x2 = x.reshape(-1, bsmm.C)
+        xq, xq_t, xs = quantize_fp8_t(x2, torch.float8_e4m3fn)
+        wq, wq_t, ws = quantize_fp8_weights(bsmm, w, torch.float8_e4m3fn)
+        ctx.bsmm, ctx.N, ctx.x_shape = bsmm, x2.shape[0], tuple(x.shape)
+        ctx.save_for_backward(xq_t, xs, w, wq, ws)
+        return xprop_fp8(bsmm, xq.view(x.shape), wq_t, xs, ws, bprop=False, out_dtype=x.dtype)
+
+    @staticmethod
+    def backward(ctx, dy):
+        xq_t, xs, w, wq, ws = ctx.saved_tensors
+        bsmm = ctx.bsmm
+        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        dx = dw = None
+        if need_dx or need_dw:
+            dq, dq_t, ds = quantize_fp8_t(dy.reshape(-1, bsmm.K), torch.float8_e5m2, with_rows=need_dx)
+        if need_dx:
+            dx = xprop_fp8(bsmm, dq, wq, ds, ws, bprop=True, out_dtype=w.dtype).view(ctx.x_shape)
+        if need_dw:
+            pending = _pending_group(bsmm, w)
+            if pending is not None:
+                dw = pending.add_fp8(xq_t, xs, dq_t, ds, ctx.N)
+            else:
+                dw = updat_fp8(bsmm, xq_t, dq_t, xs, ds, ctx.N, dw_dtype=w.dtype)
+        return dx, dw, None
+
+
 # ---------------------------------------------------------------------------------------
 # group_param_grads: fuse the dW of a weight that is reused T times into ceil(T/8) launches
 # (reference matmul.py:612-731 rewrites the TF graph; with eager autograd the same effect is
@@ -488,8 +529,11 @@ class _Pending(object):
         self.bsmm, self.w, self.group_size = bsmm, w, group_size
         self.xs, self.dys = [], []
         self.gate, self.dw_gated = None, False
+        self.fp8 = []                    # (xt, x_scale_inv, dyt, dy_scale_inv) of matmul_fp8(fp8_dw=True) uses
+        self.fp8_n = None
         self.dw = None
-        self.launches = 0
+        self.launches = 0                # every flush, 16-bit and fp8
+        self.fp8_launches = 0
 
     def add(self, x, dy, gate, dw_gated):
         self.xs.append(x)
@@ -501,12 +545,34 @@ class _Pending(object):
         # delivered once by finish(), so intermediate uses contribute nothing.
         return None
 
+    def add_fp8(self, xt, xs, dyt, ds, N):
+        if self.fp8 and (N != self.fp8_n or xt.shape[1] != self.fp8[0][0].shape[1]):
+            self.flush_fp8()                     # one updat_fp8 launch takes one N and one pitch
+        self.fp8.append((xt, xs, dyt, ds))
+        self.fp8_n = N
+        if len(self.fp8) == self.group_size:
+            self.flush_fp8()
+        return None
+
     def flush(self):
+        self.flush_fp8()
+        self.flush_16()
+
+    def flush_16(self):
         if not self.xs:
             return
         self.dw = self.bsmm.updat(self.xs, self.dys, dw=self.dw, gate=self.gate, dw_gated=self.dw_gated)
         self.launches += 1
         self.xs, self.dys = [], []
+
+    def flush_fp8(self):
+        if not self.fp8:
+            return
+        xts, xss, dyts, dss = (list(t) for t in zip(*self.fp8))
+        self.dw = updat_fp8(self.bsmm, xts, dyts, xss, dss, self.fp8_n, dw=self.dw, dw_dtype=self.w.dtype)
+        self.launches += 1
+        self.fp8_launches += 1
+        self.fp8 = []
 
 
 def _pending_group(bsmm, w):
@@ -519,7 +585,9 @@ class group_param_grads(object):
     Inside the block every backward use of `w` through `bsmm` hands its (x, dy) pair to
     a pending list instead of launching its own updat; every `group_size` (<= 8) pairs
     are flushed as ONE multi-pair launch that accumulates in place (DW then DWA in the
-    reference, matmul.py:681-692).  On exit the total is added to w.grad.
+    reference, matmul.py:681-692).  Uses through matmul_fp8(..., fp8_dw=True) hand over their
+    fp8 operands instead and are flushed the same way through updat_fp8 into the same dw, so a
+    weight used both ways gets the sum.  On exit the total is added to w.grad.
     """
 
     def __init__(self, bsmm, w, group_size=8):

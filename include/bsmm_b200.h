@@ -77,8 +77,9 @@
  *                            CWiseLinearGradOp (src/cwise_linear_op.cc:125-191)
  *   bsmm_dw_matmul_large_n <- Gemm_TN (src/matmul_op_gpu.cu:309-364), launched by DwMatmulLargeNOp
  *                            (src/matmul_op.cc:47-87)
- *   bsmm_fp8_quantize / bsmm_fp8_weights / bsmm_xprop_fp8 <- no reference counterpart: fp8 fprop / bprop on the
- *                            H100's fp8 tensor cores, which the reference's Volta target does not have
+ *   bsmm_fp8_quantize / bsmm_fp8_quantize_t / bsmm_fp8_weights / bsmm_xprop_fp8 / bsmm_updat_fp8 <- no reference
+ *                            counterpart: fp8 fprop, bprop and updat on the H100's fp8 tensor cores, which the
+ *                            reference's Volta target does not have
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer except `err` strings is DEVICE memory
@@ -1038,7 +1039,7 @@ size_t bsmm_dw_matmul_large_n_workspace_bytes(int dtype, long long N, int C, int
 /* ---- fp8 block-sparse matmul (no reference counterpart: Volta has no fp8 tensor cores) ----------------------------- */
 
 /*
- * The fp8 dtype codes BSMM_E4M3 and BSMM_E5M2 are accepted by the three entries below only; every other entry rejects
+ * The fp8 dtype codes BSMM_E4M3 and BSMM_E5M2 are accepted by the five entries below only; every other entry rejects
  * them as it rejects any unknown dtype code. Storage is one byte per element, the OCP FP8 encodings torch calls
  * float8_e4m3fn (largest finite 448, no infinities) and float8_e5m2 (largest finite 57344).
  *
@@ -1094,6 +1095,47 @@ int bsmm_fp8_weights(int src_dtype, int fp8_dtype, int bsize, int blocks, const 
 int bsmm_xprop_fp8(int x_dtype, int w_dtype, int y_dtype, int axis, int bsize, int bprop, const int32_t* lut, int n_out,
                    int n_in, int blocks, const void* x, const void* w, void* y, int N, const float* x_scale_inv,
                    const float* w_scale_inv, void* stream);
+
+/*
+ * bsmm_fp8_quantize with a transposed copy: x is a row-major (rows, cols) tensor (src_dtype), quantised with the same
+ * amax, scale and scale_inv as bsmm_fp8_quantize (kernel fp8_amax over all rows * cols elements, the same formulas
+ * and special cases). One cast kernel (fp8_quantize_t, 64 x 64 tiles transposed through shared memory) writes
+ *   y  [rows][cols]       the bytes bsmm_fp8_quantize writes for x, and / or
+ *   yt [cols][yt_pitch]   yt[c][r] = y[r][c] for r < rows, and 0 for rows <= r < yt_pitch.
+ * Either of y and yt may be null, not both. yt is the feature-major operand of bsmm_updat_fp8: its rows must start
+ * 16 bytes apart for TMA, hence the pitch.
+ * Errors before any launch: a bad src or fp8 dtype (BSMM_E_DTYPE); rows or cols < 0, a null amax or scale_inv, y and yt
+ * both null, a null x with rows * cols > 0, or yt_pitch < rows with yt given (BSMM_E_ARG); yt_pitch not a multiple of
+ * 16 or yt not 4-byte aligned, with yt given (BSMM_E_ALIGN). rows * cols = 0 stores amax = 0 and scale_inv = 1 (and
+ * yt's zero pad). 64-bit offsets.
+ */
+int bsmm_fp8_quantize_t(int src_dtype, int fp8_dtype, const void* x, long long rows, long long cols, float* amax,
+                        float* scale_inv, void* y, void* yt, long long yt_pitch, void* stream);
+
+/*
+ * Block-sparse weight gradient with fp8 operands:
+ *   dw[w] = sum_p scale_p * XT_p[c-block of w] . DYT_p[k-block of w]^T  (+ dw[w] when beta = 1),
+ *   scale_p = x_scale_invs[p][0] * dy_scale_invs[p][0]   (read on the device: nothing synchronises the host),
+ * over pcount (1..BSMM_MAX_PAIRS) pairs of feature-major operands xts[p] [n_c_blocks * bsize][pitch] (x_dtype) and
+ * dyts[p] [n_k_blocks * bsize][pitch] (dy_dtype) -- bsmm_fp8_quantize_t's yt of x (N, C) and dy (N, K) -- whose
+ * first N columns are summed. xts, dyts, x_scale_invs and dy_scale_invs are HOST arrays of device pointers. Block size
+ * 32 or 64; xt and dyt e4m3 or e5m2 each; dw (blocks, bsize, bsize) fp32, fp16 or bf16. The schedule is
+ * build_updat_schedule's, as for bsmm_updat (sched_tile_blocks = 256 / bsize).
+ * Each 128-row stage of one pair is summed by a chain of four wgmma m64nNk32 (N <= 128) into a zeroed fragment, which
+ * is then multiplied by scale_p and added to an fp32 total on CUDA cores (one fma), stage by stage in a fixed order.
+ * The epilogue adds dw when beta = 1 and rounds once to dw's dtype; only blocks that exist are written. No atomics:
+ * results are bitwise reproducible. Kernel: wgmma_updat_fp8_bs32 / _bs64.
+ * Errors before any launch: bsize other than 32 or 64 (BSMM_E_BSIZE); any other dtype combination (BSMM_E_DTYPE);
+ * pcount out of range, a null pointer (the arrays, any of their first pcount entries, dw or sched), N < 0, pitch < N,
+ * beta other than 0 or 1, blocks / n_c_blocks / n_k_blocks / sched_tiles <= 0 or a schedule for another slot count
+ * (BSMM_E_ARG); N of 2^31 or more (BSMM_E_LIMIT); pitch not a multiple of 16, or dw, xt or dyt not 16-byte aligned
+ * (BSMM_E_ALIGN); no sm_90 device (BSMM_E_NODEV). N = 0 behaves as bsmm_updat: dw is zeroed (beta 0) or left as it is
+ * (beta 1), and no kernel runs. 64-bit offsets.
+ */
+int bsmm_updat_fp8(int x_dtype, int dy_dtype, int dw_dtype, int bsize, int blocks, int n_c_blocks, int n_k_blocks,
+                   const void* const* xts, const void* const* dyts, const float* const* x_scale_invs,
+                   const float* const* dy_scale_invs, int pcount, void* dw, long long N, long long pitch, float beta,
+                   const int32_t* sched, int sched_tiles, int sched_tile_blocks, void* stream);
 
 /* ---- measurement helper (the reference's `bench` op attribute, op.cc:99-106) ---------
  * Records two events around whatever the caller enqueues between begin and end.      */

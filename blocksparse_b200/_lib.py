@@ -46,6 +46,9 @@ SIGNATURES = {
                                          _i, _i, _c.c_double, _vp, _vp]),
     "bst_attention_grad_dropout": (_i, [_i, _i, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _c.c_double, _vp, _vp]),
+    "bst_attention_decode": (_i, [_i, _i, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _f, _i, _i, _i, _i,
+                                  _i, _vp, _vp]),
+    "bst_attention_decode_workspace_bytes": (_c.c_size_t, [_i, _i, _i, _i, _i, _i]),
     "bst_autoregressive_mask": (_i, [_i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     "bst_dense_softmax": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),
     "bst_dense_softmax_grad": (_i, [_i, _vp, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),

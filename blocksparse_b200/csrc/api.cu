@@ -17,6 +17,7 @@
 #include "quantize.cuh"
 #include "softmax.cuh"
 #include "tc.cuh"
+#include "tc_bst_decode.cuh"
 #include "tc_fp8.cuh"
 #include "tc_updat_fp8.cuh"
 #include "transpose.cuh"
@@ -482,6 +483,50 @@ int bst_attention_grad_dropout(int dtype, int bsize, const int32_t* nn_lut, cons
                                        heads, head_state, ctx_blks_q, ctx_blks_k, (cudaStream_t)stream,
                                        keep_prob < 1.0 ? &drop : nullptr);
   return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
+}
+
+// ---- attention decode ---------------------------------------------------------------------------------------------
+static bool decode_shape_ok(int bsize, int nn_max, int batch, int heads, int head_state, int n) {
+  return (bsize == 16 || bsize == 32 || bsize == 64) && n >= 1 && n <= bsize && head_state > 0 && head_state % 16 == 0 &&
+         head_state <= 256 && nn_max >= 0 && batch > 0 && heads > 0;
+}
+
+size_t bst_attention_decode_workspace_bytes(int bsize, int nn_max, int batch, int heads, int head_state, int n) {
+  if (!decode_shape_ok(bsize, nn_max, batch, heads, head_state, n)) return 0;
+  return bst_decode_workspace(nn_max, batch, heads, head_state, n);
+}
+
+int bst_attention_decode(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks, int nn_max,
+                         const void* mask, int mask_heads, int autoregress_at_key,
+                         const void* q, const void* k_cache, const void* v_cache, void* o,
+                         const int32_t* positions, int n, float scale,
+                         int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                         void* workspace, void* stream) {
+  const char* what = "bst_attention_decode";
+  if (dtype != BSMM_F16 && dtype != BSMM_BF16)
+    return fail(BSMM_E_DTYPE, "%s: fp16 or bf16 only (one dtype for q and both caches), got %d", what, dtype);
+  if (bsize != 16 && bsize != 32 && bsize != 64) return fail(BSMM_E_BSIZE, "%s: block size must be 16, 32 or 64, got %d", what, bsize);
+  if (n < 1 || n > bsize) return fail(BSMM_E_ARG, "%s: n must be in [1, block size %d], got %d", what, bsize, n);
+  if (head_state <= 0 || head_state % 16 || head_state > 256)
+    return fail(BSMM_E_ARG, "%s: head_state must be a multiple of 16 up to 256, got %d", what, head_state);
+  if (batch <= 0 || heads <= 0 || blocks <= 0 || nn_max < 0 || ctx_blks_q <= 0 || ctx_blks_k <= 0)
+    return fail(BSMM_E_ARG, "%s: bad batch / heads / blocks / nn_max / context sizes", what);
+  if (lut_heads != 1 && lut_heads != heads) return fail(BSMM_E_ARG, "%s: lut_heads must be 1 or heads", what);
+  if (mask && mask_heads != 1 && mask_heads != heads) return fail(BSMM_E_ARG, "%s: mask_heads must be 1 or heads", what);
+  if (autoregress_at_key >= 0 && !mask) return fail(BSMM_E_ARG, "%s: autoregress_at_key needs a mask", what);
+  if (!nn_lut || !q || !k_cache || !v_cache || !o || !positions) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (((uintptr_t)q | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)o) & 15)
+    return fail(BSMM_E_ARG, "%s: q, the caches and o must be 16-byte aligned", what);
+  const size_t ws = bst_decode_workspace(nn_max, batch, heads, head_state, n);
+  if (ws > 0 && !workspace)
+    return fail(BSMM_E_ARG, "%s: null workspace (bst_attention_decode_workspace_bytes gives its size)", what);
+  if ((uintptr_t)workspace & 15) return fail(BSMM_E_ARG, "%s: the workspace must be 16-byte aligned", what);
+  if ((long long)batch * heads * 2 * bst_decode_nsplit(nn_max) >= (1LL << 31) || (long long)batch * n * heads >= (1LL << 31))
+    return fail(BSMM_E_LIMIT, "%s: too many CTAs for one grid", what);
+  if (!wgmma_device()) return fail(BSMM_E_NODEV, "%s: needs an sm_90 device", what);
+  return tc_bst_attention_decode(dtype, bsize, nn_lut, lut_heads, blocks, nn_max, mask, mask_heads, autoregress_at_key,
+                                 q, k_cache, v_cache, o, positions, n, scale, batch, heads, head_state, ctx_blks_q,
+                                 ctx_blks_k, workspace, (cudaStream_t)stream);
 }
 
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,

@@ -393,6 +393,84 @@ class BlocksparseTransformer(TransformerCheckers):
             p, _ = ewops.dropout(p, kp, mask=ewops._mask_at(p, p.numel(), kp, snap))
             return self.weight_value_op(p, v)
 
+    def attention_decode(self, q, k_cache, v_cache, positions, scale=1.0, autoregress_at_key=None):
+        """Attention of n new query rows per batch entry against a key / value cache, for autoregressive sampling.
+
+        q: (batch, n, heads*head_state), 1 <= n <= block size, any strides (it is copied). k_cache, v_cache:
+        (batch, ctx_k, heads*head_state), attention's k and v layout, contiguous and 16-byte aligned: the cache is never
+        copied. The caller writes the new rows' keys and values into the cache first. positions: int32 CUDA tensor
+        (batch,); entry b's rows are query rows positions[b] + i, i < n (ragged batches are fine). It is only read on
+        the device, so a decode loop that advances it in place can be captured in a CUDA graph.
+
+        Row r of entry b is row r of attention() over the cache (scaled scores, the mask with autoregress_at_key,
+        -FLT_MAX for masked keys, fp32 online softmax, P entering P V in the input dtype), over the valid keys only:
+        cache rows < min(positions[b] + n, ctx_k). Keys beyond get probability exactly 0 whatever the cache holds
+        there, NaN and Inf included. With a causal layout and mask that is attention() exactly. A row whose valid keys
+        are all masked gets uniform weights over them; a row with no valid key, or an empty LUT row, is zeros. A bad
+        position (negative, or positions[b] + n past ctx_q) gives NaN rows for that entry only, without a fault or a
+        host synchronisation. Each row's LUT row is split into runs of 4 entries whose partials are combined in order,
+        so a row's bits depend only on the layout, the mask, its q and the valid cache: not on the batch, n or the
+        other rows.
+
+        fp16 / bf16 (one dtype for q and both caches), block size 16 / 32 / 64, head_state a multiple of 16 up to 256;
+        ValueError otherwise. Returns (batch, n, heads*head_state) in q's dtype, without autograd history (inference
+        only). Kernels: bst_attention_decode, bst_attention_decode_combine."""
+        if autoregress_at_key is not None and self.softmax_mask_np is None:
+            raise ValueError("autoregress_at_key only applies to ops with mask_callback defined.")
+        for name, t in (("q", q), ("k_cache", k_cache), ("v_cache", v_cache), ("positions", positions)):
+            if not torch.is_tensor(t):
+                raise ValueError("attention_decode: %s must be a tensor, got %s" % (name, type(t)))
+        if q.dtype not in (torch.float16, torch.bfloat16):
+            raise ValueError("attention_decode: q must be float16 or bfloat16 (no fp32 decode kernel), got %s" % q.dtype)
+        if k_cache.dtype != q.dtype or v_cache.dtype != q.dtype:
+            raise ValueError("attention_decode: q, k_cache and v_cache must share one dtype, got %s, %s, %s" % (
+                q.dtype, k_cache.dtype, v_cache.dtype))
+        bs = self.blk_size
+        if bs not in (16, 32, 64):
+            raise ValueError("attention_decode: block size must be 16, 32 or 64, got %d" % bs)
+        if q.dim() != 3 or k_cache.dim() != 3:
+            raise ValueError("attention_decode: q and the caches must be 3-d (batch, rows, heads*head_state)")
+        batch, n, S = q.shape
+        if not 1 <= n <= bs:
+            raise ValueError("attention_decode: n = %d query rows, must be in [1, block size %d]" % (n, bs))
+        if S % self.heads:
+            raise ValueError("attention_decode: state size %d is not a multiple of heads %d" % (S, self.heads))
+        hs = S // self.heads
+        if hs % 16 or not 16 <= hs <= 256:
+            raise ValueError("attention_decode: head_state must be a multiple of 16 up to 256, got %d" % hs)
+        ctx_k = self.ctx_blks_k * bs
+        if tuple(k_cache.shape) != (batch, ctx_k, S) or tuple(v_cache.shape) != (batch, ctx_k, S):
+            raise ValueError("attention_decode: caches must be (batch, ctx_k, S) = %s, got %s and %s" % (
+                (batch, ctx_k, S), tuple(k_cache.shape), tuple(v_cache.shape)))
+        for name, t in (("k_cache", k_cache), ("v_cache", v_cache)):
+            if not t.is_contiguous() or t.data_ptr() % 16:
+                raise ValueError("attention_decode: %s must be contiguous and 16-byte aligned (it is never copied)" % name)
+        if positions.dtype != torch.int32 or tuple(positions.shape) != (batch,):
+            raise ValueError("attention_decode: positions must be an int32 tensor of shape (%d,), got %s %s" % (
+                batch, positions.dtype, tuple(positions.shape)))
+        if not (q.is_cuda and k_cache.is_cuda and v_cache.is_cuda and positions.is_cuda):
+            raise ValueError("attention_decode: q, the caches and positions must be CUDA tensors (no CPU path)")
+        return self._attention_decode(q, k_cache, v_cache, positions, float(scale), autoregress_at_key)
+
+    @_lib.guarded
+    def _attention_decode(self, q, k_cache, v_cache, positions, scale, autoregress_at_key):
+        lib = _lib.load()
+        q = _aligned(q.detach())
+        batch, n, S = q.shape
+        hs = S // self.heads
+        o = torch.empty((batch, n, S), dtype=q.dtype, device=q.device)
+        ws_bytes = lib.bst_attention_decode_workspace_bytes(self.blk_size, self.nn_max, batch, self.heads, hs, n)
+        ws = torch.empty((ws_bytes + 15) // 16 * 4, dtype=torch.float32, device=q.device) if ws_bytes else None
+        d = self._device_luts(q.device)
+        ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
+        rc = lib.bst_attention_decode(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(), self.lut_heads,
+                                      self.blocks, self.nn_max, _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                      q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
+                                      positions.data_ptr(), n, scale, batch, self.heads, hs,
+                                      self.ctx_blks_q, self.ctx_blks_k, _lib.ptr(ws), _lib.stream_ptr())
+        _lib.check(rc, "bst_attention_decode")
+        return o
+
 
 def _keep_prob(keep_prob):
     """keep_prob as a float in (0, 1] (ValueError otherwise, as ewops.dropout)."""

@@ -355,6 +355,42 @@ int bst_attention_grad_dropout(int dtype, int bsize, const int32_t* nn_lut, cons
                                float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
                                double keep_prob, const int64_t* seed_call, void* stream);
 
+/*
+ * Attention decode: the attention of n new query rows (1 <= n <= bsize) of each batch entry against a key / value
+ * cache, for autoregressive sampling.  No reference launcher corresponds to it.
+ *   q, o: (batch, n, heads*head_state); k_cache, v_cache: (batch, ctx_blks_k*bsize, heads*head_state), contiguous.
+ *   positions: device int32 [batch]; the rows of entry b are query rows positions[b] + i, i < n.  Never read on the host.
+ *   nn_lut, lut_heads, blocks, mask, mask_heads, autoregress_at_key: as bst_attention; nn_max: the longest nn_lut row.
+ * Row r of entry b is row r of bst_attention over the cache (scaled scores, the mask word of the entry's block id with
+ * the autoregress_at_key rewrite, -FLT_MAX for masked keys, fp32 online softmax, P entering P V in dtype), except:
+ *   valid keys   only cache rows < L_b = min(positions[b] + n, ctx_blks_k*bsize) exist; a key at or beyond L_b gets
+ *                probability exactly 0 whatever the cache holds there (NaN and Inf included: those rows are never
+ *                read).  A row whose valid keys are all masked gets uniform weights over its valid keys; a row with no
+ *                valid key, or an empty LUT row, is written as zeros.  With a causal layout and mask this is
+ *                bst_attention exactly.
+ *   bad position positions[b] < 0 or positions[b] + n > ctx_blks_q*bsize writes NaN to entry b's n rows; no fault,
+ *                no host synchronisation, the other entries are unaffected.
+ * Split rule: the nn_lut row of each query block is cut into splits of 4 consecutive entries (split s holds entries
+ * 4s .. 4s + 3); each split's fp32 partial (running max m, row sum l, unnormalised O) goes to the workspace, and a
+ * second kernel combines a row's ceil(count / 4) partials in split order.  The split depends on the layout only, so a
+ * row's bits depend only on the layout, the mask, its q and the valid cache: not on batch, n, the other rows or their
+ * positions, the stream or a graph replay.  No atomics; the workspace holds nothing between calls.
+ * Workspace: bst_attention_decode_workspace_bytes = ceil(nn_max / 4) * batch * heads * n * (head_state + 2) * 4 bytes
+ * (0 for arguments bst_attention_decode refuses), 16-byte aligned; it may be null when that is 0.
+ * Errors before any launch: dtype other than BSMM_F16 / BSMM_BF16 (BSMM_E_DTYPE); bsize other than 16, 32, 64
+ * (BSMM_E_BSIZE); n outside [1, bsize], head_state not a multiple of 16 in [16, 256], bad sizes, lut_heads or
+ * mask_heads, autoregress_at_key without a mask, a null pointer, a null workspace when its size is not 0, q, a cache or
+ * o not 16-byte aligned (BSMM_E_ARG); no sm_90 device (BSMM_E_NODEV).  64-bit element offsets.
+ * Kernels: bst_attention_decode, then bst_attention_decode_combine.
+ */
+int bst_attention_decode(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks, int nn_max,
+                         const void* mask, int mask_heads, int autoregress_at_key,
+                         const void* q, const void* k_cache, const void* v_cache, void* o,
+                         const int32_t* positions, int n, float scale,
+                         int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                         void* workspace, void* stream);
+size_t bst_attention_decode_workspace_bytes(int bsize, int nn_max, int batch, int heads, int head_state, int n);
+
 /* mask_out[hl][blk][r] = mask_in[hl][blk][r] & (ones >> shift(r)), same layout as bst_softmax's mask */
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,
                             const void* mask_in, void* mask_out, int autoregress_at_key,

@@ -49,6 +49,14 @@ SIGNATURES = {
     "bst_attention_decode": (_i, [_i, _i, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _f, _i, _i, _i, _i,
                                   _i, _vp, _vp]),
     "bst_attention_decode_workspace_bytes": (_c.c_size_t, [_i, _i, _i, _i, _i, _i]),
+    "bst_attention_gqa": (_i, [_i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _i,
+                               _c.c_double, _vp, _vp]),
+    "bst_attention_train_gqa": (_i, [_i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i,
+                                     _i, _i, _i, _c.c_double, _vp, _vp]),
+    "bst_attention_grad_gqa": (_i, [_i, _i, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                    _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _i, _c.c_double, _vp, _vp]),
+    "bst_attention_decode_gqa": (_i, [_i, _i, _vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _f, _i, _i,
+                                      _i, _i, _i, _i, _vp, _vp]),
     "bst_autoregressive_mask": (_i, [_i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     "bst_dense_softmax": (_i, [_i, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),
     "bst_dense_softmax_grad": (_i, [_i, _vp, _vp, _vp, _vp, _ll, _i, _i, _i, _ll, _ll, _f, _vp]),

@@ -485,6 +485,77 @@ int bst_attention_grad_dropout(int dtype, int bsize, const int32_t* nn_lut, cons
   return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
 }
 
+// The grouped-query entries: kv_heads divides heads; then the counterpart's checks and envelope, on kv-head-sized k, v.
+static int check_kv_heads(const char* op, int heads, int kv_heads) {
+  if (kv_heads < 1 || kv_heads > heads || heads % kv_heads)
+    return fail(BSMM_E_ARG, "%s: kv_heads must divide heads and lie in [1, heads], got kv_heads %d, heads %d", op,
+                kv_heads, heads);
+  return 0;
+}
+
+int bst_attention_gqa(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                      const void* mask, int mask_heads, int autoregress_at_key,
+                      const void* q, const void* k, const void* v, void* o, float scale,
+                      int batch, int heads, int kv_heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                      double keep_prob, const int64_t* seed_call, void* stream) {
+  const char* what = "bst_attention_gqa";
+  BstAttnDrop drop;
+  if (int e = check_attention_dropout(what, keep_prob, seed_call, drop)) return e;
+  if (int e = check_bst(bsize, lut_heads, heads, head_state, batch, blocks)) return e;
+  if (int e = check_kv_heads(what, heads, kv_heads)) return e;
+  if (!nn_lut || !q || !k || !v || !o) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (ctx_blks_q <= 0 || ctx_blks_k <= 0) return fail(BSMM_E_ARG, "%s: bad context sizes", what);
+  if (autoregress_at_key >= 0 && !mask) return fail(BSMM_E_ARG, "%s: autoregress_at_key needs a mask", what);
+  if (mask && mask_heads != 1 && mask_heads != heads) return fail(BSMM_E_ARG, "%s: mask_heads must be 1 or heads", what);
+  const int rc = tc_bst_attention(dtype, bsize, nn_lut, lut_heads, blocks, mask, mask_heads, autoregress_at_key, q, k, v, o,
+                                  scale, batch, heads, head_state, ctx_blks_q, ctx_blks_k, (cudaStream_t)stream, nullptr,
+                                  nullptr, keep_prob < 1.0 ? &drop : nullptr, kv_heads);
+  return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
+}
+
+int bst_attention_train_gqa(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                            const void* mask, int mask_heads, int autoregress_at_key,
+                            const void* q, const void* k, const void* v, void* o, float* row_max, float* row_sum,
+                            float scale, int batch, int heads, int kv_heads, int head_state, int ctx_blks_q,
+                            int ctx_blks_k, double keep_prob, const int64_t* seed_call, void* stream) {
+  const char* what = "bst_attention_train_gqa";
+  BstAttnDrop drop;
+  if (int e = check_attention_dropout(what, keep_prob, seed_call, drop)) return e;
+  if (int e = check_bst(bsize, lut_heads, heads, head_state, batch, blocks)) return e;
+  if (int e = check_kv_heads(what, heads, kv_heads)) return e;
+  if (!nn_lut || !q || !k || !v || !o || !row_max || !row_sum) return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (ctx_blks_q <= 0 || ctx_blks_k <= 0) return fail(BSMM_E_ARG, "%s: bad context sizes", what);
+  if (autoregress_at_key >= 0 && !mask) return fail(BSMM_E_ARG, "%s: autoregress_at_key needs a mask", what);
+  if (mask && mask_heads != 1 && mask_heads != heads) return fail(BSMM_E_ARG, "%s: mask_heads must be 1 or heads", what);
+  const int rc = tc_bst_attention(dtype, bsize, nn_lut, lut_heads, blocks, mask, mask_heads, autoregress_at_key, q, k, v, o,
+                                  scale, batch, heads, head_state, ctx_blks_q, ctx_blks_k, (cudaStream_t)stream, row_max,
+                                  row_sum, keep_prob < 1.0 ? &drop : nullptr, kv_heads);
+  return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
+}
+
+int bst_attention_grad_gqa(int dtype, int bsize, const int32_t* nn_lut, const int32_t* tn_lut, const int32_t* tn_order,
+                           int lut_heads, int blocks, const void* mask, int mask_heads, int autoregress_at_key,
+                           const void* q, const void* k, const void* v, const void* o, const void* dy,
+                           const float* row_max, const float* row_sum, float* delta, void* dq, void* dk, void* dv,
+                           float scale, int batch, int heads, int kv_heads, int head_state, int ctx_blks_q,
+                           int ctx_blks_k, double keep_prob, const int64_t* seed_call, void* stream) {
+  const char* what = "bst_attention_grad_gqa";
+  BstAttnDrop drop;
+  if (int e = check_attention_dropout(what, keep_prob, seed_call, drop)) return e;
+  if (int e = check_bst(bsize, lut_heads, heads, head_state, batch, blocks)) return e;
+  if (int e = check_kv_heads(what, heads, kv_heads)) return e;
+  if (!nn_lut || !tn_lut || !tn_order || !q || !k || !v || !o || !dy || !row_max || !row_sum || !delta || !dq || !dk || !dv)
+    return fail(BSMM_E_ARG, "%s: null pointer", what);
+  if (ctx_blks_q <= 0 || ctx_blks_k <= 0) return fail(BSMM_E_ARG, "%s: bad context sizes", what);
+  if (autoregress_at_key >= 0 && !mask) return fail(BSMM_E_ARG, "%s: autoregress_at_key needs a mask", what);
+  if (mask && mask_heads != 1 && mask_heads != heads) return fail(BSMM_E_ARG, "%s: mask_heads must be 1 or heads", what);
+  const int rc = tc_bst_attention_grad(dtype, bsize, nn_lut, tn_lut, tn_order, lut_heads, blocks, mask, mask_heads,
+                                       autoregress_at_key, q, k, v, o, dy, row_max, row_sum, delta, dq, dk, dv, scale, batch,
+                                       heads, head_state, ctx_blks_q, ctx_blks_k, (cudaStream_t)stream,
+                                       keep_prob < 1.0 ? &drop : nullptr, kv_heads);
+  return rc == TC_NOT_APPLICABLE ? BSMM_E_NOKERNEL : rc;
+}
+
 // ---- attention decode ---------------------------------------------------------------------------------------------
 static bool decode_shape_ok(int bsize, int nn_max, int batch, int heads, int head_state, int n) {
   return (bsize == 16 || bsize == 32 || bsize == 64) && n >= 1 && n <= bsize && head_state > 0 && head_state % 16 == 0 &&
@@ -496,13 +567,42 @@ size_t bst_attention_decode_workspace_bytes(int bsize, int nn_max, int batch, in
   return bst_decode_workspace(nn_max, batch, heads, head_state, n);
 }
 
+static int attention_decode(const char* what, int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                            int nn_max, const void* mask, int mask_heads, int autoregress_at_key, const void* q,
+                            const void* k_cache, const void* v_cache, void* o, const int32_t* positions, int n,
+                            float scale, int batch, int heads, int kv_heads, int head_state, int ctx_blks_q,
+                            int ctx_blks_k, void* workspace, void* stream);
+
 int bst_attention_decode(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks, int nn_max,
                          const void* mask, int mask_heads, int autoregress_at_key,
                          const void* q, const void* k_cache, const void* v_cache, void* o,
                          const int32_t* positions, int n, float scale,
                          int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
                          void* workspace, void* stream) {
-  const char* what = "bst_attention_decode";
+  return attention_decode("bst_attention_decode", dtype, bsize, nn_lut, lut_heads, blocks, nn_max, mask, mask_heads,
+                          autoregress_at_key, q, k_cache, v_cache, o, positions, n, scale, batch, heads, heads,
+                          head_state, ctx_blks_q, ctx_blks_k, workspace, stream);
+}
+
+int bst_attention_decode_gqa(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks, int nn_max,
+                             const void* mask, int mask_heads, int autoregress_at_key,
+                             const void* q, const void* k_cache, const void* v_cache, void* o,
+                             const int32_t* positions, int n, float scale,
+                             int batch, int heads, int kv_heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                             void* workspace, void* stream) {
+  const char* what = "bst_attention_decode_gqa";
+  if (heads > 0 && check_kv_heads(what, heads, kv_heads)) return BSMM_E_ARG;
+  return attention_decode(what, dtype, bsize, nn_lut, lut_heads, blocks, nn_max, mask, mask_heads, autoregress_at_key, q,
+                          k_cache, v_cache, o, positions, n, scale, batch, heads, kv_heads, head_state, ctx_blks_q,
+                          ctx_blks_k, workspace, stream);
+}
+
+// bst_attention_decode(_gqa) after the kv_heads check
+static int attention_decode(const char* what, int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                            int nn_max, const void* mask, int mask_heads, int autoregress_at_key, const void* q,
+                            const void* k_cache, const void* v_cache, void* o, const int32_t* positions, int n,
+                            float scale, int batch, int heads, int kv_heads, int head_state, int ctx_blks_q,
+                            int ctx_blks_k, void* workspace, void* stream) {
   if (dtype != BSMM_F16 && dtype != BSMM_BF16)
     return fail(BSMM_E_DTYPE, "%s: fp16 or bf16 only (one dtype for q and both caches), got %d", what, dtype);
   if (bsize != 16 && bsize != 32 && bsize != 64) return fail(BSMM_E_BSIZE, "%s: block size must be 16, 32 or 64, got %d", what, bsize);
@@ -526,7 +626,7 @@ int bst_attention_decode(int dtype, int bsize, const int32_t* nn_lut, int lut_he
   if (!wgmma_device()) return fail(BSMM_E_NODEV, "%s: needs an sm_90 device", what);
   return tc_bst_attention_decode(dtype, bsize, nn_lut, lut_heads, blocks, nn_max, mask, mask_heads, autoregress_at_key,
                                  q, k_cache, v_cache, o, positions, n, scale, batch, heads, head_state, ctx_blks_q,
-                                 ctx_blks_k, workspace, (cudaStream_t)stream);
+                                 ctx_blks_k, workspace, (cudaStream_t)stream, kv_heads);
 }
 
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,

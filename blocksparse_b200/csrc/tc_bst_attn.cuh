@@ -25,6 +25,11 @@
 // Philox block covers 4 consecutive keys of a row, which two neighbouring lanes share, so each lane draws the blocks of
 // one of its rows and the pair trade the halves they need in one shuffle: 8 Philox blocks per thread and entry, drawn
 // while S = Q K^T runs on the tensor cores.
+//
+// Grouped-query attention: with k and v of kv_heads heads ((batch, ctx_k, kv_heads*head_state), group = heads /
+// kv_heads) the K and V tensor maps have rows of kv_heads*head_state and query head h stages the tiles of kv head
+// h / group.  Q, o, the statistics, the mask and the dropout elements stay query head h's, and each row walks the same
+// data in the same LUT order, so o is bit-identical to this kernel's on k and v expanded to heads heads.
 #pragma once
 #include <float.h>
 #include "philox.cuh"
@@ -51,6 +56,7 @@ struct BstAttnParams {
   unsigned long long keep_thr;    // DROP: floor(keep_prob 2^32)
   float keep_prob, rkeep;         // DROP: keep_prob and fp32(1 / keep_prob)
   int blocks;                     // blocks of the layout (the element index of the dropout mask)
+  int group;                      // query heads per key / value head: head h reads kv head h / group
 };
 
 // Keep bits of this thread's two rows r0 + 8hh (hh = 0, 1) and 16 keys of one entry: bit 4j + x of kw[hh] is key
@@ -88,6 +94,7 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
   const int first = lut[2 * qb], count = lut[2 * qb + 1];
   const int2* ent = reinterpret_cast<const int2*>(lut) + first;
   const int col0 = h * p.head_state;
+  const int kcol0 = (h / p.group) * p.head_state;       // K and V: the columns of kv head h / group
 
   auto issue = [&](int e) {                             // one thread: stage entry e = (block id, key block)
     const int kb = ent[e].y;
@@ -95,8 +102,8 @@ wgmma_bst_attention(const BstAttnParams p, const __grid_constant__ BstAttnTmaps 
     uint64_t* bar = &full[e % ST];
     ptx::mbar_expect_tx(bar, STAGE_BYTES);
     for (int c = 0; c < CH; ++c) {
-      ptx::tma_load_2d(st + c * BST_TILE, &maps.k, bar, col0 + c * 64, b * p.ctx_rows_k + kb * 64);
-      ptx::tma_load_2d(st + KV_BYTES + c * BST_TILE, &maps.v, bar, col0 + c * 64, b * p.ctx_rows_k + kb * 64);
+      ptx::tma_load_2d(st + c * BST_TILE, &maps.k, bar, kcol0 + c * 64, b * p.ctx_rows_k + kb * 64);
+      ptx::tma_load_2d(st + KV_BYTES + c * BST_TILE, &maps.v, bar, kcol0 + c * 64, b * p.ctx_rows_k + kb * 64);
     }
   };
   if (tid == 0) {
@@ -265,14 +272,15 @@ inline int tc_bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut
                             int mask_heads, int autoregress_at_key, const void* q, const void* k, const void* v, void* o,
                             float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
                             cudaStream_t s, float* row_max = nullptr, float* row_sum = nullptr,
-                            const BstAttnDrop* drop = nullptr) {
+                            const BstAttnDrop* drop = nullptr, int kv_heads = 0) {
   if ((uintptr_t)o & 15) { fail(0, "pointers must be 16-byte aligned for TMA"); return TC_NOT_APPLICABLE; }
   if (!bst_tc_applicable(dtype, bsize, head_state, q, k, v)) return TC_NOT_APPLICABLE;
-  const uint64_t S = (uint64_t)heads * head_state;
+  if (kv_heads <= 0) kv_heads = heads;                  // k and v are (batch, ctx_k, kv_heads * head_state)
+  const uint64_t S = (uint64_t)heads * head_state, SKV = (uint64_t)kv_heads * head_state;
   BstAttnTmaps maps;
   if (int e = cached_tmap_2d(&maps.q, dtype, q, S, (uint64_t)batch * ctx_blks_q * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
-  if (int e = cached_tmap_2d(&maps.k, dtype, k, S, (uint64_t)batch * ctx_blks_k * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
-  if (int e = cached_tmap_2d(&maps.v, dtype, v, S, (uint64_t)batch * ctx_blks_k * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
+  if (int e = cached_tmap_2d(&maps.k, dtype, k, SKV, (uint64_t)batch * ctx_blks_k * 64, SKV, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
+  if (int e = cached_tmap_2d(&maps.v, dtype, v, SKV, (uint64_t)batch * ctx_blks_k * 64, SKV, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   BstAttnParams p;
   p.lut = nn_lut; p.lut_head_stride = lut_heads > 1 ? 2LL * (ctx_blks_q + blocks) : 0;
   p.mask = reinterpret_cast<const uint64_t*>(mask);
@@ -283,6 +291,7 @@ inline int tc_bst_attention(int dtype, int bsize, const int32_t* nn_lut, int lut
   p.row_max = row_max; p.row_sum = row_sum;
   set_drop(p, drop);
   p.blocks = blocks;
+  p.group = heads / kv_heads;
   const bool stats = row_max != nullptr;
   const int ch = head_state / 64;
   const size_t smem = (size_t)(1 + 2 * BST_ATTN_STAGES) * ch * BST_TILE + SMEM_ALIGN_SLACK;

@@ -23,6 +23,11 @@
 //                                 1/l and D are staged in shared memory.  At head_state 128 the CTA has two warpgroups:
 //                                 both compute S^T and dP^T over the whole head_state, each owns 64 state columns of dK
 //                                 and dV (one warpgroup holding all of both would need more than 255 registers).
+// Grouped-query attention (kv_heads < heads, group g = heads / kv_heads, query head h reading kv head h / g): the dq
+// kernel stages kv head h / g's tiles and is otherwise unchanged.  The dkdv kernel runs one CTA per (key block, kv head,
+// batch), launched in the order of the group's first head; it stages K and V once and walks the tn_lut rows of the
+// group's heads h = kvh g + j, j ascending, each in LUT order, through the same ring, with head h's mask, m, l, D and
+// keep bits, so dK and dV sum the whole group in fp32 registers and are rounded once.  g = 1 is the kernel above.
 // An empty LUT row writes zeros (dQ of a query block no key is listed for, dK / dV of a key block no query sees).  No
 // atomics; accumulation follows LUT order: results are deterministic.  A row whose keys are all masked has m = -FLT_MAX
 // and uniform P = 1 / l; as in the chain, its dS = scale * P o (dP - D) reaches dQ and dK.
@@ -63,6 +68,7 @@ struct BstAttnBwdParams {
   unsigned long long keep_thr;
   float keep_prob, rkeep;
   int blocks;
+  int kv_heads, group;            // k, v, dk, dv: (batch, ctx_k, kv_heads*head_state); head h reads kv head h / group
 };
 struct BstAttnBwdTmaps { CUtensorMap q, k, v, dy; };
 
@@ -113,6 +119,7 @@ wgmma_bst_attention_bwd_dq(const BstAttnBwdParams p, const __grid_constant__ Bst
   const int first = lut[2 * qb], count = lut[2 * qb + 1];
   const int2* ent = reinterpret_cast<const int2*>(lut) + first;
   const int col0 = h * p.head_state;
+  const int kcol0 = (h / p.group) * p.head_state;       // K and V: the columns of kv head h / group
   const long long S = (long long)p.heads * p.head_state;
   const long long row0 = (long long)b * p.ctx_rows_q + qb * 64;            // first dense row of the block
   const long long stat0 = ((long long)b * p.heads + h) * p.ctx_rows_q + qb * 64;
@@ -123,8 +130,8 @@ wgmma_bst_attention_bwd_dq(const BstAttnBwdParams p, const __grid_constant__ Bst
     uint64_t* bar = &full[e % ST];
     ptx::mbar_expect_tx(bar, STAGE_BYTES);
     for (int c = 0; c < CH; ++c) {
-      ptx::tma_load_2d(st + c * BST_TILE, &maps.k, bar, col0 + c * 64, b * p.ctx_rows_k + kb * 64);
-      ptx::tma_load_2d(st + T_BYTES + c * BST_TILE, &maps.v, bar, col0 + c * 64, b * p.ctx_rows_k + kb * 64);
+      ptx::tma_load_2d(st + c * BST_TILE, &maps.k, bar, kcol0 + c * 64, b * p.ctx_rows_k + kb * 64);
+      ptx::tma_load_2d(st + T_BYTES + c * BST_TILE, &maps.v, bar, kcol0 + c * 64, b * p.ctx_rows_k + kb * 64);
     }
   };
   if (tid == 0) {
@@ -285,28 +292,48 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
   const uint32_t base = aligned_smem_base(smem_raw);    // K, V, then the ring
   const uint32_t vb = base + T_BYTES, ring = base + 2 * T_BYTES;
   const int tid = threadIdx.x, wg = tid / BST_THREADS, warp = (tid % BST_THREADS) / 32, lane = tid % 32;
-  const int Z = p.batch * p.heads;
-  const int i = (int)(blockIdx.x / (unsigned)Z);        // rank in the head's longest-first order
+  const int Z = p.batch * p.kv_heads;
+  const int i = (int)(blockIdx.x / (unsigned)Z);        // rank in the order of the group's first head
   const int z = (int)(blockIdx.x % (unsigned)Z);
-  const int b = z / p.heads, h = z % p.heads;
-  const int kb = p.tn_order[h * p.order_head_stride + i];
-  const int32_t* lut = p.tn_lut + h * p.tn_head_stride;
-  const int first = lut[2 * kb], count = lut[2 * kb + 1];
-  const int2* ent = reinterpret_cast<const int2*>(lut) + first;
-  const int col0 = h * p.head_state;
-  const long long S = (long long)p.heads * p.head_state;
+  const int b = z / p.kv_heads, kvh = z % p.kv_heads;
+  const int h0 = kvh * p.group;                         // the group's query heads are h0 .. h0 + group - 1
+  const int kb = p.tn_order[h0 * p.order_head_stride + i];
+  const int col0 = kvh * p.head_state;
+  const long long S = (long long)p.heads * p.head_state, SKV = (long long)p.kv_heads * p.head_state;
   const long long krow0 = (long long)b * p.ctx_rows_k + kb * 64;
-  const long long stat_b = ((long long)b * p.heads + h) * p.ctx_rows_q;
-
-  auto issue = [&](int e) {                             // one thread: stage entry e = (block id, query block)
-    const int qb = ent[e].y;
-    const uint32_t st = ring + (uint32_t)(e % ST) * STAGE_BYTES;
-    uint64_t* bar = &full[e % ST];
+  // The CTA walks the key block's tn_lut rows of heads h0, h0 + 1, ... in turn, each in LUT order: entry (j, e) is
+  // entry e of head h0 + j's row.  A cursor (j, e) steps through them; flat position f = entries before it.
+  auto row_of = [&](int j, int& first) {                // count (and first entry) of head h0 + j's row
+    const int32_t* lut = p.tn_lut + (long long)(h0 + j) * p.tn_head_stride;
+    first = lut[2 * kb];
+    return lut[2 * kb + 1];
+  };
+  int total = 0;
+  for (int j = 0; j < p.group; ++j) { int f; total += row_of(j, f); }
+  struct Cursor { int j, e, first, count; };
+  auto start = [&](Cursor& c) {                         // the first entry
+    c.j = 0; c.e = 0; c.count = row_of(0, c.first);
+    while (c.count == 0 && c.j + 1 < p.group) c.count = row_of(++c.j, c.first);
+  };
+  auto step = [&](Cursor& c) {                          // the next entry, skipping heads whose row is empty
+    if (++c.e < c.count) return;
+    c.e = 0;
+    do { if (++c.j >= p.group) return; c.count = row_of(c.j, c.first); } while (c.count == 0);
+  };
+  auto entry = [&](const Cursor& c) {
+    return reinterpret_cast<const int2*>(p.tn_lut + (long long)(h0 + c.j) * p.tn_head_stride)[c.first + c.e];
+  };
+  Cursor pc;                                            // tid 0: the next entry to stage
+  auto issue = [&](int f) {                             // one thread: stage flat entry f = (block id, query block)
+    const int qb = entry(pc).y, qcol0 = (h0 + pc.j) * p.head_state;
+    const uint32_t st = ring + (uint32_t)(f % ST) * STAGE_BYTES;
+    uint64_t* bar = &full[f % ST];
     ptx::mbar_expect_tx(bar, STAGE_BYTES);
     for (int c = 0; c < CH; ++c) {
-      ptx::tma_load_2d(st + c * BST_TILE, &maps.q, bar, col0 + c * 64, b * p.ctx_rows_q + qb * 64);
-      ptx::tma_load_2d(st + T_BYTES + c * BST_TILE, &maps.dy, bar, col0 + c * 64, b * p.ctx_rows_q + qb * 64);
+      ptx::tma_load_2d(st + c * BST_TILE, &maps.q, bar, qcol0 + c * 64, b * p.ctx_rows_q + qb * 64);
+      ptx::tma_load_2d(st + T_BYTES + c * BST_TILE, &maps.dy, bar, qcol0 + c * 64, b * p.ctx_rows_q + qb * 64);
     }
+    step(pc);
   };
   if (tid == 0) {
     ptx::mbar_init(&kvbar, 1);
@@ -314,18 +341,18 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
     ptx::fence_mbar_init();
   }
   __syncthreads();
-  if (tid == 0 && count > 0) {
+  if (tid == 0 && total > 0) {
     ptx::mbar_expect_tx(&kvbar, 2 * T_BYTES);
     for (int c = 0; c < CH; ++c) {
       ptx::tma_load_2d(base + c * BST_TILE, &maps.k, &kvbar, col0 + c * 64, (int)krow0);
       ptx::tma_load_2d(vb + c * BST_TILE, &maps.v, &kvbar, col0 + c * 64, (int)krow0);
     }
-    for (int e = 0; e < count && e < ST; ++e) issue(e);
+    start(pc);
+    for (int f = 0; f < total && f < ST; ++f) issue(f);
   }
 
   // This thread's two key rows r0, r0 + 8 of the block; its query columns are 8j + 2(lane%4) + x.
   const int r0 = warp * 16 + lane / 4;
-  const uint64_t* mask = p.mask ? p.mask + (p.mask_head_stride ? h * p.mask_head_stride : 0) : nullptr;
   float dk[32], dv[32];
 #pragma unroll
   for (int n = 0; n < 32; ++n) { dk[n] = 0.f; dv[n] = 0.f; }
@@ -336,13 +363,17 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
     call = (unsigned long long)p.seed_call[1];
     key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
   }
-  if (count > 0 && !ptx::mbar_wait(&kvbar, 0)) g_tc_error = 53;
+  if (total > 0 && !ptx::mbar_wait(&kvbar, 0)) g_tc_error = 53;
 
-  for (int e = 0; e < count; ++e) {
+  Cursor cc;                                            // every thread: the entry being computed
+  start(cc);
+  for (int e = 0; e < total; ++e, step(cc)) {
     const uint32_t st = ring + (uint32_t)(e % ST) * STAGE_BYTES;
-    const int2 bq = ent[e];
+    const int2 bq = entry(cc);
+    const int h = h0 + cc.j;                            // its query head: mask, statistics and keep bits are h's
+    const uint64_t* mask = p.mask ? p.mask + (p.mask_head_stride ? h * p.mask_head_stride : 0) : nullptr;
     if (tid < 64) {                                     // per query row t of the entry: its mask word and statistics
-      const long long r = stat_b + bq.y * 64 + tid;
+      const long long r = ((long long)b * p.heads + h) * p.ctx_rows_q + bq.y * 64 + tid;
       uint64_t w = ~0ull;
       if (mask) {
         w = mask[(long long)bq.x * 64 + tid];
@@ -430,17 +461,17 @@ wgmma_bst_attention_bwd_dkdv(const BstAttnBwdParams p, const __grid_constant__ B
     ptx::wg_fence_regs(dv);
     ptx::wg_fence_regs(dk);
     __syncthreads();                                    // every warp's MMAs that read this stage have retired
-    if (tid == 0 && e + ST < count) issue(e + ST);
+    if (tid == 0 && e + ST < total) issue(e + ST);
   }
 
-  // epilogue (a key block no query sees writes zeros)
+  // epilogue: dK and dV summed over the group, rounded once (a key block no query of the group sees writes zeros)
   if constexpr (DROP) {
 #pragma unroll
     for (int n = 0; n < 32; ++n) dv[n] *= p.rkeep;
   }
-  const long long off = krow0 * S + col0 + wg * 64;
-  store_rows<BF16>(reinterpret_cast<uint16_t*>(p.dk) + off, S, r0, lane, dk);
-  store_rows<BF16>(reinterpret_cast<uint16_t*>(p.dv) + off, S, r0, lane, dv);
+  const long long off = krow0 * SKV + col0 + wg * 64;
+  store_rows<BF16>(reinterpret_cast<uint16_t*>(p.dk) + off, SKV, r0, lane, dk);
+  store_rows<BF16>(reinterpret_cast<uint16_t*>(p.dv) + off, SKV, r0, lane, dv);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -458,15 +489,16 @@ inline int tc_bst_attention_grad(int dtype, int bsize, const int32_t* nn_lut, co
                                  int autoregress_at_key, const void* q, const void* k, const void* v, const void* o,
                                  const void* dy, const float* row_max, const float* row_sum, float* delta, void* dq,
                                  void* dk, void* dv, float scale, int batch, int heads, int head_state, int ctx_blks_q,
-                                 int ctx_blks_k, cudaStream_t s, const BstAttnDrop* drop = nullptr) {
+                                 int ctx_blks_k, cudaStream_t s, const BstAttnDrop* drop = nullptr, int kv_heads = 0) {
   const void* const all[8] = {q, k, v, o, dy, dq, dk, dv};
   if (!bst_attention_grad_applicable(dtype, bsize, head_state, all)) return TC_NOT_APPLICABLE;
-  const uint64_t S = (uint64_t)heads * head_state;
+  if (kv_heads <= 0) kv_heads = heads;                  // k, v, dk and dv are (batch, ctx_k, kv_heads * head_state)
+  const uint64_t S = (uint64_t)heads * head_state, SKV = (uint64_t)kv_heads * head_state;
   BstAttnBwdTmaps maps;
   if (int e = cached_tmap_2d(&maps.q, dtype, q, S, (uint64_t)batch * ctx_blks_q * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   if (int e = cached_tmap_2d(&maps.dy, dtype, dy, S, (uint64_t)batch * ctx_blks_q * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
-  if (int e = cached_tmap_2d(&maps.k, dtype, k, S, (uint64_t)batch * ctx_blks_k * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
-  if (int e = cached_tmap_2d(&maps.v, dtype, v, S, (uint64_t)batch * ctx_blks_k * 64, S, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
+  if (int e = cached_tmap_2d(&maps.k, dtype, k, SKV, (uint64_t)batch * ctx_blks_k * 64, SKV, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
+  if (int e = cached_tmap_2d(&maps.v, dtype, v, SKV, (uint64_t)batch * ctx_blks_k * 64, SKV, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return e;
   BstAttnBwdParams p;
   p.nn_lut = nn_lut; p.tn_lut = tn_lut; p.tn_order = tn_order;
   p.nn_head_stride = lut_heads > 1 ? 2LL * (ctx_blks_q + blocks) : 0;
@@ -481,10 +513,11 @@ inline int tc_bst_attention_grad(int dtype, int bsize, const int32_t* nn_lut, co
   p.dq = dq; p.dk = dk; p.dv = dv;
   set_drop(p, drop);
   p.blocks = blocks;
+  p.kv_heads = kv_heads; p.group = heads / kv_heads;
   const int ch = head_state / 64;
   const size_t smem = (size_t)(2 + 2 * BST_BWD_STAGES) * ch * BST_TILE + SMEM_ALIGN_SLACK;
   const unsigned grid_q = (unsigned)((long long)batch * heads * ctx_blks_q);
-  const unsigned grid_k = (unsigned)((long long)batch * heads * ctx_blks_k);
+  const unsigned grid_k = (unsigned)((long long)batch * kv_heads * ctx_blks_k);
 #define BSMM_LAUNCH_BWD(BFV, CHV, DRV)                                                   \
   { auto kq = wgmma_bst_attention_bwd_dq<BFV, CHV, DRV>;                                 \
     auto kk = wgmma_bst_attention_bwd_dkdv<BFV, CHV, DRV>;                               \

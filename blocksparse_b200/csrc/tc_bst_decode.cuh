@@ -23,8 +23,18 @@
 //                                 over the row's splits in split order, rounded once to the input dtype.
 // Workspace: float2 (m, l) [batch][heads][nsplit][n], then float O [batch][heads][nsplit][n][head_state], with
 // nsplit = ceil(nn_max / DECODE_SPLIT).  No atomics, no counters: every call overwrites what it reads.
+//
+// Grouped-query attention (caches of kv_heads < heads heads, g = heads / kv_heads, query head h reading kv head h / g):
+// with a shared layout every head of a group walks the same LUT rows over the same K and V, so one CTA per (split, t,
+// head slice, kv head, batch entry) stages each K / V tile once for a slice of hp = min(g, 64 / n) query heads.  Its
+// DECODE_SLOTS = 64 row slots (4 warps x 16) hold the chunk's rows of each head in turn, slot j n + (r - r_lo) being
+// block row r of head hfirst + j: rows of different heads are M rows of the same mma.sync, each with its own mask
+// word, online softmax and partial.  A row's arithmetic does not depend on its slot, so its bits are those of the kernel above on
+// the expanded cache.  Per-head layouts, and n too large to stack two heads, run hp = 1: one CTA per query head, in
+// the row slots above, reading kv head h / g.  The combine is unchanged.
 #pragma once
 #include <float.h>
+#include <algorithm>
 #include "softmax.cuh"
 #include "tc.cuh"
 
@@ -33,6 +43,7 @@ namespace bsmm {
 constexpr int DECODE_SPLIT = 4;          // LUT entries per split
 constexpr int DECODE_STAGES = 2;         // (K, V) tiles in flight per CTA
 constexpr int DECODE_THREADS = 128;
+constexpr int DECODE_SLOTS = DECODE_THREADS / 32 * 16;   // row slots of a CTA: 16 rows per warp
 
 namespace dptx {
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
@@ -68,7 +79,7 @@ struct BstDecodeParams {
   const void* mask;                // uint{bs} [mask_heads][blocks][bs] or null
   long long mask_head_stride;      // words
   int autoregress_at_key;          // < 0: off
-  const uint16_t *q, *k, *v;       // q (batch, n, S); caches (batch, ctx_rows_k, S)
+  const uint16_t *q, *k, *v;       // q (batch, n, S); caches (batch, ctx_rows_k, kv_heads*head_state)
   void* o;                         // (batch, n, S)
   const int32_t* positions;
   float scale;
@@ -76,6 +87,8 @@ struct BstDecodeParams {
   int ctx_rows_q, ctx_rows_k;
   float2* ml;                      // workspace: [batch][heads][nsplit][n] (m, l)
   float* acc;                      //            [batch][heads][nsplit][n][head_state] O
+  int kv_heads, group;             // query head h reads kv head h / group
+  int hp, hslices;                 // query heads per CTA (> 1: stacked row slots), CTAs per group: ceil(group / hp)
 };
 
 // Byte offset of 16-byte chunk c of row r in a tile of HSP 16-bit columns; the XOR keeps the eight rows an ldmatrix
@@ -98,38 +111,55 @@ bst_attention_decode(const BstDecodeParams p) {
   unsigned x = blockIdx.x;
   const int s = (int)(x % (unsigned)p.nsplit); x /= (unsigned)p.nsplit;
   const int t = (int)(x % 2u); x /= 2u;
-  const int h = (int)(x % (unsigned)p.heads), b = (int)(x / (unsigned)p.heads);
+  const int hsl = (int)(x % (unsigned)p.hslices); x /= (unsigned)p.hslices;
+  const int kvh = (int)(x % (unsigned)p.kv_heads), b = (int)(x / (unsigned)p.kv_heads);
+  const int hfirst = kvh * p.group + hsl * p.hp;       // this CTA's query heads: hfirst .. hfirst + nh - 1
+  const int nh = min(p.hp, p.group - hsl * p.hp);
+  const bool stacked = p.hp > 1;
+  const uint32_t QTILE = (stacked ? DECODE_SLOTS : BS) * HSP * 2;
   const int n = p.n, hs = p.head_state;
   const int pos = p.positions[b];
   if (pos < 0 || pos > p.ctx_rows_q - n) return;       // the combine writes NaN rows
   const int qb = pos / BS + t;
   const int r_lo = max(pos, qb * BS) - qb * BS, r_hi = min(pos + n, (qb + 1) * BS) - qb * BS;   // block rows of the chunk
   if (r_lo >= r_hi) return;
-  const int32_t* lut = p.lut + h * p.lut_head_stride;
+  const int32_t* lut = p.lut + hfirst * p.lut_head_stride;   // stacked: a shared layout, one LUT for every head
   const int count = lut[2 * qb + 1];
   const int e0 = s * DECODE_SPLIT;
   if (e0 >= count) return;                             // the combine reads ceil(count / E) splits only
   const int ne = min(DECODE_SPLIT, count - e0);
   const int2* ent = reinterpret_cast<const int2*>(lut) + lut[2 * qb] + e0;
   const int L = min(pos + n, p.ctx_rows_k);
-  const long long S = (long long)p.heads * hs;
-  const long long col0 = (long long)h * hs;
+  const long long S = (long long)p.heads * hs, SKV = (long long)p.kv_heads * hs;
+  const long long kcol0 = (long long)kvh * hs;
+  // Row slot rs holds block row slot_row(rs, j) of head hfirst + j; valid: a row of the chunk (else it is computed
+  // from zeros and never stored).
+  auto slot_row = [&](int rs, int& j, bool& valid) {
+    if (!stacked) { j = 0; valid = rs >= r_lo && rs < r_hi; return rs; }
+    j = rs / n;
+    const int r = rs % n + r_lo;
+    valid = j < nh && r < r_hi;
+    return r;
+  };
 
   // Q rows of the chunk; other rows and the columns past head_state are zeros
-  for (int idx = tid; idx < BS * CH; idx += DECODE_THREADS) {
-    const int r = idx / CH, c = idx % CH;
-    const bool ok = r >= r_lo && r < r_hi && c * 8 < hs;
-    const uint16_t* src = ok ? p.q + ((long long)b * n + (qb * BS + r - pos)) * S + col0 + c * 8 : p.q;
-    dptx::cp_async16(base + dec_off<HSP>(r, c), src, ok);
+  for (int idx = tid; idx < (int)(QTILE / (HSP * 2)) * CH; idx += DECODE_THREADS) {
+    const int rs = idx / CH, c = idx % CH;
+    int j;
+    bool ok;
+    const int r = slot_row(rs, j, ok);
+    ok = ok && c * 8 < hs;
+    const uint16_t* src = ok ? p.q + ((long long)b * n + (qb * BS + r - pos)) * S + (long long)(hfirst + j) * hs + c * 8 : p.q;
+    dptx::cp_async16(base + dec_off<HSP>(rs, c), src, ok);
   }
   auto issue = [&](int j) {                            // all threads: K and V tiles of entry j of the split
     const int kb = ent[j].y;
-    const uint32_t st = base + TILE + (uint32_t)(j % DECODE_STAGES) * 2 * TILE;
+    const uint32_t st = base + QTILE + (uint32_t)(j % DECODE_STAGES) * 2 * TILE;
     for (int idx = tid; idx < BS * CH; idx += DECODE_THREADS) {
       const int r = idx / CH, c = idx % CH;
       const int key = kb * BS + r;
       const bool ok = key < L && c * 8 < hs;           // rows past L_b never leave global memory
-      const long long off = ok ? ((long long)b * p.ctx_rows_k + key) * S + col0 + c * 8 : 0;
+      const long long off = ok ? ((long long)b * p.ctx_rows_k + key) * SKV + kcol0 + c * 8 : 0;
       dptx::cp_async16(st + dec_off<HSP>(r, c), p.k + off, ok);
       dptx::cp_async16(st + TILE + dec_off<HSP>(r, c), p.v + off, ok);
     }
@@ -140,9 +170,18 @@ bst_attention_decode(const BstDecodeParams p) {
     dptx::cp_commit();
   }
 
-  const bool active = warp * 16 < r_hi && warp * 16 + 16 > r_lo;   // this warp's 16 rows hold a row of the chunk
+  const bool active = stacked ? warp * 16 < nh * n    // this warp's 16 rows hold a row of the chunk
+                              : warp * 16 < r_hi && warp * 16 + 16 > r_lo;
   const int g = lane / 4;
-  const MW* mask = p.mask ? reinterpret_cast<const MW*>(p.mask) + h * p.mask_head_stride : nullptr;
+  int rj[2], rrow[2];                                  // this thread's two rows: head hfirst + rj, block row rrow
+  bool rvalid[2];
+  const MW* rmask[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    rrow[hh] = slot_row(warp * 16 + g + 8 * hh, rj[hh], rvalid[hh]);
+    rmask[hh] = p.mask ? reinterpret_cast<const MW*>(p.mask) + (long long)(hfirst + rj[hh]) * p.mask_head_stride : nullptr;
+    if (stacked && !rvalid[hh]) rmask[hh] = nullptr;  // its block row may lie past the block
+  }
   float o[HSP / 8][4];
 #pragma unroll
   for (int i = 0; i < HSP / 8; ++i)
@@ -154,7 +193,7 @@ bst_attention_decode(const BstDecodeParams p) {
     dptx::cp_wait<DECODE_STAGES - 1>();
     __syncthreads();
     if (active) {
-      const uint32_t kt = base + TILE + (uint32_t)(j % DECODE_STAGES) * 2 * TILE, vt = kt + TILE;
+      const uint32_t kt = base + QTILE + (uint32_t)(j % DECODE_STAGES) * 2 * TILE, vt = kt + TILE;
       float sc[NT][4];
 #pragma unroll
       for (int i = 0; i < NT; ++i)
@@ -175,14 +214,14 @@ bst_attention_decode(const BstDecodeParams p) {
         }
       }
       // scale, mask (bst_softmax's order), then the valid-key rule; sc[i][2hh + x] is key 8i + 2(lane%4) + x of
-      // block row 16 warp + g + 8hh
+      // row slot 16 warp + g + 8hh, block row rrow[hh]
       const int2 bk = ent[j];
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        const int rr = warp * 16 + g + 8 * hh;
+        const int rr = rrow[hh];
         uint64_t w = ~0ull;
-        if (mask) {
-          w = (uint64_t)mask[(long long)bk.x * BS + rr];
+        if (rmask[hh]) {
+          w = (uint64_t)rmask[hh][(long long)bk.x * BS + rr];
           if (p.autoregress_at_key >= 0) w = autoregress_word<BS>(w, p.autoregress_at_key, bk.y, qb * BS + rr);
         }
 #pragma unroll
@@ -263,9 +302,8 @@ bst_attention_decode(const BstDecodeParams p) {
     float sum = l[hh];
     sum += __shfl_xor_sync(0xffffffffu, sum, 1);
     sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-    const int rr = warp * 16 + g + 8 * hh;
-    if (rr < r_lo || rr >= r_hi) continue;
-    const long long slot = (((long long)b * p.heads + h) * p.nsplit + s) * n + (qb * BS + rr - pos);
+    if (!rvalid[hh]) continue;
+    const long long slot = (((long long)b * p.heads + hfirst + rj[hh]) * p.nsplit + s) * n + (qb * BS + rrow[hh] - pos);
     if (lane % 4 == 0) p.ml[slot] = make_float2(m[hh], sum);
     float* out = p.acc + slot * hs;
 #pragma unroll
@@ -341,7 +379,7 @@ inline int tc_bst_attention_decode(int dtype, int bsize, const int32_t* nn_lut, 
                                    const void* mask, int mask_heads, int autoregress_at_key, const void* q,
                                    const void* k_cache, const void* v_cache, void* o, const int32_t* positions, int n,
                                    float scale, int batch, int heads, int head_state, int ctx_blks_q, int ctx_blks_k,
-                                   void* workspace, cudaStream_t s) {
+                                   void* workspace, cudaStream_t s, int kv_heads = 0) {
   BstDecodeParams p;
   p.lut = nn_lut; p.lut_head_stride = lut_heads > 1 ? 2LL * (ctx_blks_q + blocks) : 0;
   p.mask = mask; p.mask_head_stride = (mask && mask_heads > 1) ? (long long)blocks * bsize : 0;
@@ -352,15 +390,23 @@ inline int tc_bst_attention_decode(int dtype, int bsize, const int32_t* nn_lut, 
   p.ctx_rows_q = ctx_blks_q * bsize; p.ctx_rows_k = ctx_blks_k * bsize;
   p.ml = (float2*)workspace;
   p.acc = (float*)((char*)workspace + (size_t)p.nsplit * batch * heads * n * sizeof(float2));
+  if (kv_heads <= 0) kv_heads = heads;
+  p.kv_heads = kv_heads; p.group = heads / kv_heads;
+  // a shared layout stacks up to 64 / n heads of a group in one CTA's row slots; per-head layouts run one head per CTA
+  p.hp = lut_heads == 1 ? std::min(p.group, DECODE_SLOTS / n) : 1;
+  if (p.hp < 2) p.hp = 1;
+  p.hslices = (p.group + p.hp - 1) / p.hp;
+  const int q_rows = p.hp > 1 ? DECODE_SLOTS : bsize;   // rows of the Q tile
   const bool bf = dtype == BSMM_BF16;
   if (p.nsplit > 0) {
     const int hsp = head_state <= 64 ? 64 : head_state <= 128 ? 128 : 256;
-    const unsigned grid = (unsigned)((long long)batch * heads * 2 * p.nsplit);
+    const unsigned grid = (unsigned)((long long)batch * kv_heads * p.hslices * 2 * p.nsplit);
 #define BSMM_LAUNCH_DEC(BFV, BSV, HSV)                                                   \
     { auto kern = bst_attention_decode<BFV, BSV, HSV>;                                   \
-      const size_t smem = (size_t)(1 + 2 * DECODE_STAGES) * BSV * HSV * 2;               \
+      const size_t smem = (size_t)(q_rows + 2 * DECODE_STAGES * BSV) * HSV * 2;          \
+      const size_t smem_max = (size_t)(std::max(DECODE_SLOTS, BSV) + 2 * DECODE_STAGES * BSV) * HSV * 2; \
       static thread_local uint64_t cfg = 0;                                              \
-      if (int e = ensure_dyn_smem(kern, smem, cfg)) return e;                            \
+      if (int e = ensure_dyn_smem(kern, smem_max, cfg)) return e;                        \
       kern<<<grid, DECODE_THREADS, smem, s>>>(p); }
 #define BSMM_LAUNCH_DEC_HS(BFV, BSV)                                                     \
     { if (hsp == 64) BSMM_LAUNCH_DEC(BFV, BSV, 64)                                       \

@@ -23,6 +23,14 @@ def _aligned(t):
     return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
+def _expand_kv(x, heads, kv_heads):
+    """k or v of kv_heads heads, (batch, ctx, kv_heads*hs), expanded to (batch, ctx, heads*hs): query head h gets kv
+    head h // (heads // kv_heads), as repeat_interleave groups them. Autograd sums the gradient over each group."""
+    B, C, Skv = x.shape
+    hs = Skv // kv_heads
+    return x.reshape(B, C, kv_heads, 1, hs).expand(B, C, kv_heads, heads // kv_heads, hs).reshape(B, C, heads * hs)
+
+
 class BlocksparseTransformer(TransformerCheckers):
     """Drop-in for blocksparse.transformer.BlocksparseTransformer (reference transformer.py:51)."""
 
@@ -159,10 +167,11 @@ class BlocksparseTransformer(TransformerCheckers):
         return dx
 
     @_lib.guarded
-    def _attention(self, q, k, v, scale, autoregress_at_key, keep_prob=1.0, seed_call=None):
+    def _attention(self, q, k, v, scale, autoregress_at_key, keep_prob=1.0, seed_call=None, kv_heads=None):
         """Fused NT -> (masked) softmax -> NN in one launch, or None where the library has no fused kernel for the
         call (BSMM_E_NOKERNEL): the caller then composes the three ops. keep_prob < 1 adds dropout on the probabilities
-        (bst_attention_dropout), its mask drawn at the int64 [seed, call] device tensor seed_call, which is not moved."""
+        (bst_attention_dropout), its mask drawn at the int64 [seed, call] device tensor seed_call, which is not moved.
+        kv_heads (not None): k and v hold kv_heads heads (bst_attention_gqa)."""
         lib = _lib.load()
         if not q.is_cuda:
             raise _lib.BsmmError("BlocksparseTransformer needs CUDA tensors (no CPU path)")
@@ -170,13 +179,24 @@ class BlocksparseTransformer(TransformerCheckers):
         batch, ctx_q, S = q.shape
         if ctx_q != self.ctx_blks_q * self.blk_size or k.shape[1] != self.ctx_blks_k * self.blk_size:
             raise ValueError("context sizes do not match the layout")
-        if S % self.heads or tuple(k.shape) != (batch, k.shape[1], S) or v.shape != k.shape or q.dtype != k.dtype:
+        Skv = S if kv_heads is None else S // self.heads * kv_heads
+        if S % self.heads or tuple(k.shape) != (batch, k.shape[1], Skv) or v.shape != k.shape or q.dtype != k.dtype:
             raise ValueError("state size / dtype mismatch")
         o = torch.empty((batch, ctx_q, S), dtype=v.dtype, device=v.device)
         d = self._device_luts(q.device)
         ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
         # one dtype code stands for q, k and v; mixed dtypes name none, and the library answers with E_NOKERNEL
         dt = _lib.dtype_code(q.dtype) if v.dtype == q.dtype else -1
+        if kv_heads is not None:
+            rc = lib.bst_attention_gqa(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
+                                       _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                       q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), float(scale),
+                                       batch, self.heads, kv_heads, S // self.heads, self.ctx_blks_q, self.ctx_blks_k,
+                                       float(keep_prob), _lib.ptr(seed_call), _lib.stream_ptr())
+            if rc == _lib.E_NOKERNEL:
+                return None
+            _lib.check(rc, "bst_attention_gqa")
+            return o
         if keep_prob == 1.0:
             rc = lib.bst_attention(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
                                    _lib.ptr(d["mask"]), self.lut_heads, ak,
@@ -194,10 +214,11 @@ class BlocksparseTransformer(TransformerCheckers):
         return o
 
     @_lib.guarded
-    def _attention_train(self, q, k, v, scale, autoregress_at_key, keep_prob=1.0, seed_call=None):
+    def _attention_train(self, q, k, v, scale, autoregress_at_key, keep_prob=1.0, seed_call=None, kv_heads=None):
         """_attention that also returns each query row's softmax statistics (max m and sum l, float32
-        (batch, heads, ctx_q)) for _attention_grad; None where the library has no fused kernel for the call. keep_prob
-        and seed_call: as _attention (bst_attention_train_dropout); m and l do not depend on them."""
+        (batch, heads, ctx_q)) for _attention_grad; None where the library has no fused kernel for the call. keep_prob,
+        seed_call and kv_heads: as _attention (bst_attention_train_dropout, bst_attention_train_gqa); m and l do not
+        depend on the first two."""
         lib = _lib.load()
         if not q.is_cuda:
             raise _lib.BsmmError("BlocksparseTransformer needs CUDA tensors (no CPU path)")
@@ -205,7 +226,8 @@ class BlocksparseTransformer(TransformerCheckers):
         batch, ctx_q, S = q.shape
         if ctx_q != self.ctx_blks_q * self.blk_size or k.shape[1] != self.ctx_blks_k * self.blk_size:
             raise ValueError("context sizes do not match the layout")
-        if S % self.heads or tuple(k.shape) != (batch, k.shape[1], S) or v.shape != k.shape or q.dtype != k.dtype:
+        Skv = S if kv_heads is None else S // self.heads * kv_heads
+        if S % self.heads or tuple(k.shape) != (batch, k.shape[1], Skv) or v.shape != k.shape or q.dtype != k.dtype:
             raise ValueError("state size / dtype mismatch")
         o = torch.empty((batch, ctx_q, S), dtype=v.dtype, device=v.device)
         m = torch.empty((batch, self.heads, ctx_q), dtype=torch.float32, device=v.device)
@@ -213,6 +235,16 @@ class BlocksparseTransformer(TransformerCheckers):
         d = self._device_luts(q.device)
         ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
         dt = _lib.dtype_code(q.dtype) if v.dtype == q.dtype else -1
+        if kv_heads is not None:
+            rc = lib.bst_attention_train_gqa(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
+                                             _lib.ptr(d["mask"]), self.lut_heads, ak, q.data_ptr(), k.data_ptr(),
+                                             v.data_ptr(), o.data_ptr(), m.data_ptr(), l.data_ptr(), float(scale),
+                                             batch, self.heads, kv_heads, S // self.heads, self.ctx_blks_q,
+                                             self.ctx_blks_k, float(keep_prob), _lib.ptr(seed_call), _lib.stream_ptr())
+            if rc == _lib.E_NOKERNEL:
+                return None
+            _lib.check(rc, "bst_attention_train_gqa")
+            return o, m, l
         if keep_prob == 1.0:
             rc = lib.bst_attention_train(dt, self.blk_size, d["nn"].data_ptr(), self.lut_heads, self.blocks,
                                          _lib.ptr(d["mask"]), self.lut_heads, ak,
@@ -231,10 +263,12 @@ class BlocksparseTransformer(TransformerCheckers):
         return o, m, l
 
     @_lib.guarded
-    def _attention_grad(self, q, k, v, o, dy, m, l, scale, autoregress_at_key, keep_prob=1.0, seed_call=None):
+    def _attention_grad(self, q, k, v, o, dy, m, l, scale, autoregress_at_key, keep_prob=1.0, seed_call=None,
+                        kv_heads=None):
         """dq, dk, dv of the fused attention from what _attention_train saved, in one bst_attention_grad call
-        (bst_attention_grad_dropout with the forward's keep_prob and seed_call). The forward ran the fused kernel, so
-        the call is inside its envelope; dy is made contiguous and aligned."""
+        (bst_attention_grad_dropout with the forward's keep_prob and seed_call, bst_attention_grad_gqa with its
+        kv_heads; dk and dv then have k's and v's kv-head shape). The forward ran the fused kernel, so the call is
+        inside its envelope; dy is made contiguous and aligned."""
         lib = _lib.load()
         dy = _aligned(dy.to(o.dtype))
         batch, ctx_q, S = q.shape
@@ -242,6 +276,17 @@ class BlocksparseTransformer(TransformerCheckers):
         delta = torch.empty_like(m)
         d = self._device_luts(q.device)
         ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
+        if kv_heads is not None:
+            rc = lib.bst_attention_grad_gqa(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(),
+                                            d["tn"].data_ptr(), d["tn_order"].data_ptr(), self.lut_heads, self.blocks,
+                                            _lib.ptr(d["mask"]), self.lut_heads, ak,
+                                            q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dy.data_ptr(),
+                                            m.data_ptr(), l.data_ptr(), delta.data_ptr(), dq.data_ptr(), dk.data_ptr(),
+                                            dv.data_ptr(), float(scale), batch, self.heads, kv_heads, S // self.heads,
+                                            self.ctx_blks_q, self.ctx_blks_k, float(keep_prob), _lib.ptr(seed_call),
+                                            _lib.stream_ptr())
+            _lib.check(rc, "bst_attention_grad_gqa")
+            return dq, dk, dv
         if keep_prob == 1.0:
             rc = lib.bst_attention_grad(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(), d["tn"].data_ptr(),
                                         d["tn_order"].data_ptr(), self.lut_heads, self.blocks,
@@ -337,8 +382,18 @@ class BlocksparseTransformer(TransformerCheckers):
         dtype = dtype or self.softmax_dtype or x.dtype
         return _SoftmaxFunction.apply(x, self, float(scale), False, None, dtype)
 
+    def _kv_heads(self, kv_heads, what):
+        """kv_heads checked (ValueError unless an int in [1, heads] that divides heads); None stands for heads."""
+        if kv_heads is None:
+            return self.heads
+        if isinstance(kv_heads, bool) or not isinstance(kv_heads, (int, np.integer)) or not 1 <= kv_heads <= self.heads:
+            raise ValueError("%s: kv_heads must be an int in [1, heads = %d], got %r" % (what, self.heads, kv_heads))
+        if self.heads % kv_heads:
+            raise ValueError("%s: kv_heads %d does not divide heads %d" % (what, kv_heads, self.heads))
+        return int(kv_heads)
+
     def attention(self, q, k, v, scale=1.0, autoregress_at_key=None, fused_backward=False, keep_prob=1.0,
-                  dropout_state=None):
+                  dropout_state=None, kv_heads=None):
         """weight_value_op(masked_softmax(query_key_op(q, k), scale, autoregress_at_key), v) -- softmax without a
         mask_callback -- as one fused kernel that never writes the (batch, heads, blocks, bs, bs) scores or
         probabilities; the backward pass recomputes them from q and k. Returns (batch, ctx_q, heads*head_state) in
@@ -360,9 +415,33 @@ class BlocksparseTransformer(TransformerCheckers):
         keeps a copy of (seed, call) on the device and the backward redraws the mask from it; nothing synchronises with
         the host, so forward and backward can be captured in a CUDA graph. fused_backward=False keeps its contract:
         gradients bit-identical to the chain's with ewops.dropout in it. Outside the fused envelope the op runs that
-        chain with the same mask. keep_prob == 1.0 runs exactly the code without dropout and reads no state."""
+        chain with the same mask. keep_prob == 1.0 runs exactly the code without dropout and reads no state.
+
+        kv_heads (grouped-query attention): k and v hold kv_heads heads, (batch, ctx_k, kv_heads*head_state), and query
+        head h reads kv head h // (heads // kv_heads), the grouping of repeat_interleave and of
+        scaled_dot_product_attention(enable_gqa=True). kv_heads must divide heads. The result is this op on k and v
+        expanded to heads heads, layout, mask, autoregress_at_key and dropout (whose elements keep the query head)
+        included; inside the fused envelope nothing is expanded: the kernels read each kv head's tiles for the query
+        heads of its group, and fused_backward=True saves k and v at kv-head size and sums dk and dv over each group
+        in fp32 registers. fused_backward=False keeps its contract: gradients bit-identical to the chain on expanded k
+        and v, autograd summing dk and dv over each group. Outside the envelope the op runs that chain. None or heads
+        runs exactly the code without kv_heads."""
         if autoregress_at_key is not None and self.softmax_mask_np is None:
             raise ValueError("autoregress_at_key only applies to ops with mask_callback defined.")
+        kv = self._kv_heads(kv_heads, "attention")
+        if kv != self.heads:
+            if not (torch.is_tensor(q) and torch.is_tensor(k) and torch.is_tensor(v)) or q.dim() != 3:
+                raise ValueError("attention: q, k and v must be 3-d tensors (batch, ctx, heads*head_state)")
+            batch, _, S = q.shape
+            if S % self.heads:
+                raise ValueError("attention: state size %d is not a multiple of heads %d" % (S, self.heads))
+            want = (batch, self.ctx_blks_k * self.blk_size, S // self.heads * kv)
+            if tuple(k.shape) != want or tuple(v.shape) != want:
+                raise ValueError("attention: with kv_heads = %d, k and v must be (batch, ctx_k, kv_heads*head_state) = "
+                                 "%s, got %s and %s" % (kv, want, tuple(k.shape), tuple(v.shape)))
+            kv_heads = kv
+        else:
+            kv_heads = None                # today's code and kernels
         kp = _keep_prob(keep_prob)
         if dropout_state is not None and not (torch.is_tensor(dropout_state) and dropout_state.dtype == torch.int64
                                               and dropout_state.numel() == 2 and dropout_state.device == q.device):
@@ -372,9 +451,12 @@ class BlocksparseTransformer(TransformerCheckers):
         if kp == 1.0:
             try:
                 if fused_backward:
-                    return _AttentionTrainFunction.apply(q, k, v, self, float(scale), autoregress_at_key, 1.0, None)
-                return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key, 1.0, None)
+                    return _AttentionTrainFunction.apply(q, k, v, self, float(scale), autoregress_at_key, 1.0, None,
+                                                         kv_heads)
+                return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key, 1.0, None, kv_heads)
             except _NoFusedKernel:
+                if kv_heads is not None:
+                    k, v = _expand_kv(k, self.heads, kv_heads), _expand_kv(v, self.heads, kv_heads)
                 w = self.query_key_op(q, k)
                 return self.weight_value_op(self.masked_softmax(w, scale, autoregress_at_key), v)
         from . import ewops
@@ -386,14 +468,16 @@ class BlocksparseTransformer(TransformerCheckers):
             snap = dropout_state.detach().reshape(2).clone()
         try:
             if fused_backward:
-                return _AttentionTrainFunction.apply(q, k, v, self, float(scale), autoregress_at_key, kp, snap)
-            return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key, kp, snap)
+                return _AttentionTrainFunction.apply(q, k, v, self, float(scale), autoregress_at_key, kp, snap, kv_heads)
+            return _AttentionFunction.apply(q, k, v, self, float(scale), autoregress_at_key, kp, snap, kv_heads)
         except _NoFusedKernel:
+            if kv_heads is not None:
+                k, v = _expand_kv(k, self.heads, kv_heads), _expand_kv(v, self.heads, kv_heads)
             p = self.masked_softmax(self.query_key_op(q, k), scale, autoregress_at_key)
             p, _ = ewops.dropout(p, kp, mask=ewops._mask_at(p, p.numel(), kp, snap))
             return self.weight_value_op(p, v)
 
-    def attention_decode(self, q, k_cache, v_cache, positions, scale=1.0, autoregress_at_key=None):
+    def attention_decode(self, q, k_cache, v_cache, positions, scale=1.0, autoregress_at_key=None, kv_heads=None):
         """Attention of n new query rows per batch entry against a key / value cache, for autoregressive sampling.
 
         q: (batch, n, heads*head_state), 1 <= n <= block size, any strides (it is copied). k_cache, v_cache:
@@ -414,9 +498,16 @@ class BlocksparseTransformer(TransformerCheckers):
 
         fp16 / bf16 (one dtype for q and both caches), block size 16 / 32 / 64, head_state a multiple of 16 up to 256;
         ValueError otherwise. Returns (batch, n, heads*head_state) in q's dtype, without autograd history (inference
-        only). Kernels: bst_attention_decode, bst_attention_decode_combine."""
+        only). Kernels: bst_attention_decode, bst_attention_decode_combine.
+
+        kv_heads (grouped-query attention, the rule of attention()): the caches are (batch, ctx_k,
+        kv_heads*head_state) and query head h reads kv head h // (heads // kv_heads); each row's bits are those of
+        attention_decode on the caches expanded to heads heads, which are never formed. With a shared layout one CTA
+        stages each K / V tile once for up to 64 / n query heads of a group, so the cache bytes read shrink by up to
+        heads / kv_heads. None or heads runs exactly the code without kv_heads."""
         if autoregress_at_key is not None and self.softmax_mask_np is None:
             raise ValueError("autoregress_at_key only applies to ops with mask_callback defined.")
+        kv = self._kv_heads(kv_heads, "attention_decode")
         for name, t in (("q", q), ("k_cache", k_cache), ("v_cache", v_cache), ("positions", positions)):
             if not torch.is_tensor(t):
                 raise ValueError("attention_decode: %s must be a tensor, got %s" % (name, type(t)))
@@ -439,9 +530,10 @@ class BlocksparseTransformer(TransformerCheckers):
         if hs % 16 or not 16 <= hs <= 256:
             raise ValueError("attention_decode: head_state must be a multiple of 16 up to 256, got %d" % hs)
         ctx_k = self.ctx_blks_k * bs
-        if tuple(k_cache.shape) != (batch, ctx_k, S) or tuple(v_cache.shape) != (batch, ctx_k, S):
-            raise ValueError("attention_decode: caches must be (batch, ctx_k, S) = %s, got %s and %s" % (
-                (batch, ctx_k, S), tuple(k_cache.shape), tuple(v_cache.shape)))
+        Skv = hs * kv
+        if tuple(k_cache.shape) != (batch, ctx_k, Skv) or tuple(v_cache.shape) != (batch, ctx_k, Skv):
+            raise ValueError("attention_decode: caches must be (batch, ctx_k, kv_heads*head_state) = %s, got %s and %s" % (
+                (batch, ctx_k, Skv), tuple(k_cache.shape), tuple(v_cache.shape)))
         for name, t in (("k_cache", k_cache), ("v_cache", v_cache)):
             if not t.is_contiguous() or t.data_ptr() % 16:
                 raise ValueError("attention_decode: %s must be contiguous and 16-byte aligned (it is never copied)" % name)
@@ -450,10 +542,11 @@ class BlocksparseTransformer(TransformerCheckers):
                 batch, positions.dtype, tuple(positions.shape)))
         if not (q.is_cuda and k_cache.is_cuda and v_cache.is_cuda and positions.is_cuda):
             raise ValueError("attention_decode: q, the caches and positions must be CUDA tensors (no CPU path)")
-        return self._attention_decode(q, k_cache, v_cache, positions, float(scale), autoregress_at_key)
+        return self._attention_decode(q, k_cache, v_cache, positions, float(scale), autoregress_at_key,
+                                      None if kv == self.heads else kv)
 
     @_lib.guarded
-    def _attention_decode(self, q, k_cache, v_cache, positions, scale, autoregress_at_key):
+    def _attention_decode(self, q, k_cache, v_cache, positions, scale, autoregress_at_key, kv_heads=None):
         lib = _lib.load()
         q = _aligned(q.detach())
         batch, n, S = q.shape
@@ -463,6 +556,14 @@ class BlocksparseTransformer(TransformerCheckers):
         ws = torch.empty((ws_bytes + 15) // 16 * 4, dtype=torch.float32, device=q.device) if ws_bytes else None
         d = self._device_luts(q.device)
         ak = -1 if autoregress_at_key is None else int(autoregress_at_key)
+        if kv_heads is not None:
+            rc = lib.bst_attention_decode_gqa(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(),
+                                              self.lut_heads, self.blocks, self.nn_max, _lib.ptr(d["mask"]),
+                                              self.lut_heads, ak, q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                              o.data_ptr(), positions.data_ptr(), n, scale, batch, self.heads, kv_heads,
+                                              hs, self.ctx_blks_q, self.ctx_blks_k, _lib.ptr(ws), _lib.stream_ptr())
+            _lib.check(rc, "bst_attention_decode_gqa")
+            return o
         rc = lib.bst_attention_decode(_lib.dtype_code(q.dtype), self.blk_size, d["nn"].data_ptr(), self.lut_heads,
                                       self.blocks, self.nn_max, _lib.ptr(d["mask"]), self.lut_heads, ak,
                                       q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
@@ -532,14 +633,16 @@ class _AttentionFunction(torch.autograd.Function):
     """Fused attention. Saves q, k and v only (and with dropout the [seed, call] snapshot); the backward recomputes the
     scores and the probabilities with the chain's own NT and softmax kernels, then runs the chain's backward ops
     (_XnFunction, _DropoutFunction with the mask redrawn from the snapshot, _SoftmaxFunction and _NtFunction in turn)
-    on them, so its gradients are bit-identical to the chain's."""
+    on them, so its gradients are bit-identical to the chain's. With kv_heads it saves k and v at kv-head size, runs
+    that backward on their expanded copies and lets autograd sum dk and dv over each group, as the chain on expanded
+    k and v would."""
 
     @staticmethod
-    def forward(ctx, q, k, v, bst, scale, autoregress_at_key, keep_prob, snap):
-        o = bst._attention(q, k, v, scale, autoregress_at_key, keep_prob, snap)
+    def forward(ctx, q, k, v, bst, scale, autoregress_at_key, keep_prob, snap, kv_heads=None):
+        o = bst._attention(q, k, v, scale, autoregress_at_key, keep_prob, snap, kv_heads)
         if o is None:
             raise _NoFusedKernel()
-        ctx.bst, ctx.scale, ctx.ak, ctx.keep_prob = bst, scale, autoregress_at_key, keep_prob
+        ctx.bst, ctx.scale, ctx.ak, ctx.keep_prob, ctx.kv_heads = bst, scale, autoregress_at_key, keep_prob, kv_heads
         if snap is None:
             ctx.save_for_backward(q, k, v)
         else:
@@ -549,6 +652,23 @@ class _AttentionFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         q, k, v = ctx.saved_tensors[:3]
+        bst = ctx.bst
+        if ctx.kv_heads is None:
+            return _AttentionFunction._chain_backward(ctx, q, k, v, dy) + (None,)
+        need = ctx.needs_input_grad
+        with torch.enable_grad():
+            kd, vd = k.detach().requires_grad_(), v.detach().requires_grad_()
+            kx, vx = _expand_kv(kd, bst.heads, ctx.kv_heads), _expand_kv(vd, bst.heads, ctx.kv_heads)
+        dq, dkx, dvx = _AttentionFunction._chain_backward(ctx, q, kx.detach(), vx.detach(), dy)[:3]
+        outs = [(x, xd, g) for x, xd, g, n in ((kx, kd, dkx, need[1]), (vx, vd, dvx, need[2])) if n]
+        grads = iter(torch.autograd.grad([x for x, _, _ in outs], [xd for _, xd, _ in outs], [g for _, _, g in outs])
+                     if outs else ())
+        dk = next(grads) if need[1] else None
+        dv = next(grads) if need[2] else None
+        return dq, dk, dv, None, None, None, None, None, None
+
+    @staticmethod
+    def _chain_backward(ctx, q, k, v, dy):
         bst, scale, kp = ctx.bst, ctx.scale, ctx.keep_prob
         dy = dy.contiguous()
         # forward of the chain up to the probabilities: bf16 scores, probabilities in q's dtype (query_key_op)
@@ -577,16 +697,16 @@ class _AttentionFunction(torch.autograd.Function):
 
 class _AttentionTrainFunction(torch.autograd.Function):
     """Fused attention with a fused backward. Saves q, k, v, o and the row statistics (and with dropout the
-    [seed, call] snapshot; nothing of sparse shape); the backward computes dq, dk and dv in one bst_attention_grad call
-    and returns the requested ones."""
+    [seed, call] snapshot; nothing of sparse shape, and with kv_heads k and v at kv-head size); the backward computes
+    dq, dk and dv in one bst_attention_grad (_gqa) call and returns the requested ones."""
 
     @staticmethod
-    def forward(ctx, q, k, v, bst, scale, autoregress_at_key, keep_prob, snap):
-        r = bst._attention_train(q, k, v, scale, autoregress_at_key, keep_prob, snap)
+    def forward(ctx, q, k, v, bst, scale, autoregress_at_key, keep_prob, snap, kv_heads=None):
+        r = bst._attention_train(q, k, v, scale, autoregress_at_key, keep_prob, snap, kv_heads)
         if r is None:
             raise _NoFusedKernel()
         o, m, l = r
-        ctx.bst, ctx.scale, ctx.ak, ctx.keep_prob = bst, scale, autoregress_at_key, keep_prob
+        ctx.bst, ctx.scale, ctx.ak, ctx.keep_prob, ctx.kv_heads = bst, scale, autoregress_at_key, keep_prob, kv_heads
         if snap is None:
             ctx.save_for_backward(q.contiguous(), k.contiguous(), v.contiguous(), o, m, l)
         else:
@@ -597,10 +717,10 @@ class _AttentionTrainFunction(torch.autograd.Function):
     def backward(ctx, dy):
         q, k, v, o, m, l = ctx.saved_tensors[:6]
         snap = ctx.saved_tensors[6] if ctx.keep_prob != 1.0 else None
-        dq, dk, dv = ctx.bst._attention_grad(q, k, v, o, dy, m, l, ctx.scale, ctx.ak, ctx.keep_prob, snap)
+        dq, dk, dv = ctx.bst._attention_grad(q, k, v, o, dy, m, l, ctx.scale, ctx.ak, ctx.keep_prob, snap, ctx.kv_heads)
         need = ctx.needs_input_grad
         return (dq if need[0] else None, dk if need[1] else None, dv if need[2] else None,
-                None, None, None, None, None)
+                None, None, None, None, None, None)
 
 
 class _SoftmaxFunction(torch.autograd.Function):

@@ -391,6 +391,52 @@ int bst_attention_decode(int dtype, int bsize, const int32_t* nn_lut, int lut_he
                          void* workspace, void* stream);
 size_t bst_attention_decode_workspace_bytes(int bsize, int nn_max, int batch, int heads, int head_state, int n);
 
+/*
+ * Grouped-query attention: k and v (and dk, dv; k_cache, v_cache) hold kv_heads heads, (batch, ctx, kv_heads*head_state),
+ * while q, o, dy and dq keep heads heads.  kv_heads divides heads; with g = heads / kv_heads query head h reads kv head
+ * h / g (the grouping of repeat_interleave).  Each entry computes what its counterpart computes on k and v expanded to
+ * heads heads; row_max, row_sum, delta, the mask and the dropout elements stay per query head.
+ *   bst_attention_gqa, bst_attention_train_gqa   bst_attention_dropout's / bst_attention_train_dropout's arguments plus
+ *                                                kv_heads; keep_prob == 1 is no dropout and reads no state.  o, row_max
+ *                                                and row_sum are bit-identical to the counterpart's on expanded k, v.
+ *   bst_attention_grad_gqa                       bst_attention_grad_dropout's arguments plus kv_heads.  dq is
+ *                                                bit-identical to the counterpart's on expanded k, v.  dk and dv sum
+ *                                                each group in fp32 and are rounded once: one CTA per (key block, kv
+ *                                                head, batch) walks the tn_lut rows of the group's heads in turn.
+ *   bst_attention_decode_gqa                     bst_attention_decode's arguments plus kv_heads; the caches are never
+ *                                                copied.  With lut_heads == 1 one CTA stages each K / V tile once for
+ *                                                up to 64 / n heads of a group.  Each row is bit-identical to
+ *                                                bst_attention_decode's on the expanded cache.  The workspace is
+ *                                                bst_attention_decode_workspace_bytes with heads = query heads.
+ * Errors: kv_heads < 1, kv_heads > heads or heads % kv_heads != 0 give BSMM_E_ARG before any launch; otherwise the
+ * counterpart's envelope and error codes apply, BSMM_E_NOKERNEL included.  kv_heads == heads is the counterpart.
+ */
+int bst_attention_gqa(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                      const void* mask, int mask_heads, int autoregress_at_key,
+                      const void* q, const void* k, const void* v, void* o, float scale,
+                      int batch, int heads, int kv_heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                      double keep_prob, const int64_t* seed_call, void* stream);
+
+int bst_attention_train_gqa(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks,
+                            const void* mask, int mask_heads, int autoregress_at_key,
+                            const void* q, const void* k, const void* v, void* o, float* row_max, float* row_sum,
+                            float scale, int batch, int heads, int kv_heads, int head_state, int ctx_blks_q,
+                            int ctx_blks_k, double keep_prob, const int64_t* seed_call, void* stream);
+
+int bst_attention_grad_gqa(int dtype, int bsize, const int32_t* nn_lut, const int32_t* tn_lut, const int32_t* tn_order,
+                           int lut_heads, int blocks, const void* mask, int mask_heads, int autoregress_at_key,
+                           const void* q, const void* k, const void* v, const void* o, const void* dy,
+                           const float* row_max, const float* row_sum, float* delta, void* dq, void* dk, void* dv,
+                           float scale, int batch, int heads, int kv_heads, int head_state, int ctx_blks_q,
+                           int ctx_blks_k, double keep_prob, const int64_t* seed_call, void* stream);
+
+int bst_attention_decode_gqa(int dtype, int bsize, const int32_t* nn_lut, int lut_heads, int blocks, int nn_max,
+                             const void* mask, int mask_heads, int autoregress_at_key,
+                             const void* q, const void* k_cache, const void* v_cache, void* o,
+                             const int32_t* positions, int n, float scale,
+                             int batch, int heads, int kv_heads, int head_state, int ctx_blks_q, int ctx_blks_k,
+                             void* workspace, void* stream);
+
 /* mask_out[hl][blk][r] = mask_in[hl][blk][r] & (ones >> shift(r)), same layout as bst_softmax's mask */
 int bst_autoregressive_mask(int bsize, const int32_t* nt_lut, int lut_heads, int blocks,
                             const void* mask_in, void* mask_out, int autoregress_at_key,
